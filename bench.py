@@ -46,7 +46,7 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "fallback (H100 SXM data sheet: 3.35 TB/s HBM3)"
 
 
 def physical_cores():
@@ -165,6 +165,24 @@ def timed_steps(st, K, W, torch, dist, world, sampler=None):
     return ms, clocks
 
 
+def dump_outputs(st, out_dir, torch, budget=64 << 20):
+    """What the timed step hands its caller after the last timed step: the sampled token ids (float64) and the logits they
+    were sampled from (float32 [B, vocab]: 39 MB at batch 64 x 152064).  Logits beyond the budget are cut to a fixed,
+    seeded sample of columns (logits_columns.npy holds their vocabulary ids)."""
+    import numpy as np
+    torch.cuda.synchronize()
+    os.makedirs(out_dir, exist_ok=True)
+    ids = st.next_ids.cpu().numpy().astype(np.float64)
+    logits = st.logits.float().cpu().numpy()
+    cap = (budget - ids.nbytes) // (4 * logits.shape[0])
+    if logits.shape[1] > cap:
+        cols = np.sort(np.random.default_rng(0).choice(logits.shape[1], size=cap - 2, replace=False))
+        logits = logits[:, cols]
+        np.save(os.path.join(out_dir, "logits_columns.npy"), cols.astype(np.float64))
+    np.save(os.path.join(out_dir, "next_ids.npy"), ids)
+    np.save(os.path.join(out_dir, "logits.npy"), np.ascontiguousarray(logits))
+
+
 def e2e_steps(st, ids, K, torch, dist, world):
     """The same step through the public API with HOST buffers: pinned H2D of the ids, D2H of the sampled ids, stream sync
     (a serving loop needs the token on the host before the next step) — wall clock, max over ranks."""
@@ -189,7 +207,7 @@ def e2e_steps(st, ids, K, torch, dist, world):
     return s
 
 
-def kernel_rooflines(st, cfg, hbm_peak, torch, traffic):
+def kernel_rooflines(st, cfg, hbm_peak, torch):
     """Per-kernel achieved HBM GB/s at the stack's CURRENT batch, measured live with CUDA events (each launch reads a
     different layer's weights / cache: >> L2)."""
     B, ws, xn = st.B, st.ws, st.xn
@@ -199,34 +217,34 @@ def kernel_rooflines(st, cfg, hbm_peak, torch, traffic):
     io = {"gate": (xn, st.gate), "gateup": (xn, st.gate), "up": (xn, st.up), "qkv": (xn, st.qkv), "o": (st.ao, st.x),
           "down": (st.gate, st.x)}
 
-    def entry(name, t, nb, per_step, tkey, note=None):
+    def entry(name, t, nb, per_step, note=None):
         e = {"us": round(t * 1e6, 2), "GBps": round(nb / t / 1e9, 1), "frac": round(nb / t / 1e9 / hbm_peak, 3),
-             "algo_bytes": nb, "launches_per_step": per_step, "traffic": traffic.get("%s B=%d" % (tkey, B))}
+             "algo_bytes": nb, "launches_per_step": per_step}
         if note:
             e["note"] = note
         kern[name] = e
 
-    def gemm_entry(name, key, tkey, act=0):
+    def gemm_entry(name, key, act=0):
         src, dst = io[key]
         fns = [(lambda L=L: L[key](src, ws, out=dst, act=act)) for L in st.layers]
         t = time_kernel_loop(fns, rounds, torch)
-        entry(name, t, st.layers[0][key].op.algo_bytes(B), nl, tkey)
+        entry(name, t, st.layers[0][key].op.algo_bytes(B), nl)
 
     from b200spark._lib import ACT_SILU
     if st.fuse_swiglu:
-        gemm_entry("wq_gemm[gate+up SwiGLU %dx2x%d]" % (cfg.hidden, cfg.inter), "gateup", "wq_gemm[gate+up]")
+        gemm_entry("wq_gemm[gate+up SwiGLU %dx2x%d]" % (cfg.hidden, cfg.inter), "gateup")
     else:
-        gemm_entry("wq_gemm[gate %dx%d]" % (cfg.hidden, cfg.inter), "gate", "wq_gemm[gate]", ACT_SILU)
-        gemm_entry("wq_gemm[up %dx%d]" % (cfg.hidden, cfg.inter), "up", "wq_gemm[up]")
-    gemm_entry("wq_gemm[down %dx%d]" % (cfg.inter, cfg.hidden), "down", "wq_gemm[down]")
-    gemm_entry("wq_gemm[qkv %dx%d]" % (cfg.hidden, (cfg.n_heads + 2 * cfg.n_kv) * 128), "qkv", "wq_gemm[qkv]")
-    gemm_entry("wq_gemm[o %dx%d]" % (cfg.n_heads * 128, cfg.hidden), "o", "wq_gemm[o]")
+        gemm_entry("wq_gemm[gate %dx%d]" % (cfg.hidden, cfg.inter), "gate", ACT_SILU)
+        gemm_entry("wq_gemm[up %dx%d]" % (cfg.hidden, cfg.inter), "up")
+    gemm_entry("wq_gemm[down %dx%d]" % (cfg.inter, cfg.hidden), "down")
+    gemm_entry("wq_gemm[qkv %dx%d]" % (cfg.hidden, (cfg.n_heads + 2 * cfg.n_kv) * 128), "qkv")
+    gemm_entry("wq_gemm[o %dx%d]" % (cfg.n_heads * 128, cfg.hidden), "o")
     cur = int(st.lens_new[0].item())
     fns = [(lambda L=L: st.attn(st.q, L["cache"], st.lens_new, st.max_len, ws, out=st.ao)) for L in st.layers]
     t = time_kernel_loop(fns, rounds, torch)
-    entry("span_attn[B=%d,ctx=%d]" % (B, cur), t, st.attn.algo_bytes(B * cur), nl, "span_attn")
+    entry("span_attn[B=%d,ctx=%d]" % (B, cur), t, st.attn.algo_bytes(B * cur), nl)
     t = time_kernel_loop([lambda: st.lm_head(xn, ws, out=st.logits)], 10, torch)
-    entry("wq_gemm[lm_head bf16 %dx%d]" % (cfg.hidden, cfg.vocab), t, st.lm_head.op.algo_bytes(B), 1, "wq_gemm[lm_head]",
+    entry("wq_gemm[lm_head bf16 %dx%d]" % (cfg.hidden, cfg.vocab), t, st.lm_head.op.algo_bytes(B), 1,
           note="same weights every launch; 1.09 GB >> L2")
     tot = sum(v["us"] * v["launches_per_step"] for v in kern.values())
     for v in kern.values():
@@ -248,7 +266,7 @@ def measure_tp(args, world, rank, hbm_peak, torch, dist):
     from b200spark import model
     cfg = model.QWEN2_72B
     B, ctx = args.tp_batch, args.tp_ctx
-    K, W = max(5, min(args.steps, 20)), 3
+    K, W = args.steps, max(args.warmup, 3)
     t0 = time.time()
     st = model.DecodeStack(cfg, B, ctx + 3 * K + W + 16, wbits=4, group=-1, kv="none", span=128, tp_rank=rank, tp_size=world,
                            layers=args.tp_layers)
@@ -296,20 +314,18 @@ def run_gpu(args):
     ids = torch.randint(0, cfg.vocab, (B,), generator=torch.Generator().manual_seed(4321), dtype=torch.int64)
     st.ids.copy_(ids.cuda())
     ms, clocks = timed_steps(st, K, W, torch, dist, world, ClockSampler(local) if rank == 0 else None)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(st, args.dump_outputs, torch)
     replicas = 1 if tp > 1 else world  # TP: the ranks share one batch; replicas: every rank has its own
     value = replicas * B * K / (ms * 1e-3)
     e2e_s = e2e_steps(st, ids, K, torch, dist, world)
     e2e_val = replicas * B * K / e2e_s
     launches = st.launches_per_step * K
-    try:
-        traffic = json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))
-    except Exception:
-        traffic = {}
 
     out = None
     kern = step = None
     if rank == 0:
-        kern = kernel_rooflines(st, cfg, hbm_peak, torch, traffic)
+        kern = kernel_rooflines(st, cfg, hbm_peak, torch)
         step = step_roofline(st, ctx, ms / K, hbm_peak)
 
     # ---------------- the metric's other batches on the same weights and caches (every rank takes part: barriers inside)
@@ -330,7 +346,7 @@ def run_gpu(args):
                "e2e_tokens_per_s": round(replicas * b * K / e2e_b, 2), "gpu_launches": st.launches_per_step * K}
         if rank == 0:
             rec["step"] = step_roofline(st, ctx, ms_b / K, hbm_peak)
-            rec["kernels"] = kernel_rooflines(st, cfg, hbm_peak, torch, traffic)
+            rec["kernels"] = kernel_rooflines(st, cfg, hbm_peak, torch)
         batches[str(b)] = rec
     st.set_batch(B)
 
@@ -353,7 +369,7 @@ def run_gpu(args):
     if rank == 0:
         dom = max(kern, key=lambda k: kern[k]["share_of_kernel_time"])
         roof = {"bound": "hbm", "kernel": dom, "achieved": kern[dom]["GBps"], "peak": hbm_peak, "unit": "GB/s",
-                "frac": kern[dom]["frac"], "traffic": kern[dom]["traffic"], "peak_source": peak_src,
+                "frac": kern[dom]["frac"], "peak_source": peak_src,
                 "share_of_kernel_time": kern[dom]["share_of_kernel_time"], "step": step}
         if tp > 1:
             roof["step"]["note"] = "per-rank algorithmic bytes; tokens/s is for the whole TP group"
@@ -362,12 +378,12 @@ def run_gpu(args):
             "ms_per_step": round(ms / K, 4), "higher_is_better": True, "scaling": "strong" if tp > 1 else "weak", "vs_baseline": None,
             "dtype": "bf16 activations x int%d weights (fp32 accumulate), %s KV" % (args.wbits, args.kv),
             "data": "synthetic (seeded N(0,0.02^2) weights quantized with the IQ formula; N(0,1) KV rows written by the append kernel)",
-            "config": {"workload": "%s IQ-int%d%s weight-only decode, batch %d, ctx %d, 1xB200 per replica" %
+            "config": {"workload": "%s IQ-int%d%s weight-only decode, batch %d, ctx %d, 1xH100 per replica" %
                                    (cfg.name, args.wbits, "" if args.group == -1 else " g%d" % args.group, B, ctx),
                        "batch": B, "ctx": ctx, "layers": args.layers or cfg.layers, "kv_cache": args.kv, "span": args.span,
                        "parallelism": ("tp%d (column/row split, all-reduce after o_proj and down_proj, vocab-split lm_head)" % tp)
                                       if tp > 1 else "replicas x%d (no data-path collective)" % world,
-                       "l2": "inputs larger than L2: %.2f GB streamed per step vs 126 MB L2" % (step["algo_bytes"] / 1e9),
+                       "l2": "inputs larger than L2: %.2f GB streamed per step vs 50 MB L2" % (step["algo_bytes"] / 1e9),
                        "cuda_graph": True, "pdl": os.environ.get("B2_PDL", "1") != "0"},
             "e2e": {"value": round(e2e_val, 2), "unit": "tokens/s", "h2d_bytes_per_step": B * 8, "d2h_bytes_per_step": B * 8},
             "gpu_launches": launches,
@@ -446,6 +462,8 @@ def main():
     ap.add_argument("--tp-batch", type=int, default=16)
     ap.add_argument("--tp-ctx", type=int, default=4096)
     ap.add_argument("--tp-layers", type=int, default=None, help="debug: fewer layers in the TP record (INVALID as a bench number)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the headline batch's last sampled ids and logits as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

@@ -1,4 +1,4 @@
-"""Build the in-tree native libraries for sm_100a with nvcc (no GPU needed to compile).
+"""Build the in-tree native libraries for sm_90a (H100) with nvcc (no GPU needed to compile).
 
   lib/libb200spark.so      CUDA kernels + the C ABI of include/b200spark.h   (csrc/*.cu)
   lib/liballspark_b200.so  allspark-shaped C++ operator layer over the C ABI  (host/*.cpp), if present
@@ -16,7 +16,7 @@ ROOT = os.path.dirname(HERE)
 LIB = os.path.join(HERE, "lib")
 OBJ = os.path.join(HERE, "build")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 CUFLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
            "-Xptxas", "-v" if os.environ.get("B2_PTXAS_V") else "-warn-spills"] + os.environ.get("B2_EXTRA_NVCC", "").split()
 

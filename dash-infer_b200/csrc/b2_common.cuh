@@ -1,4 +1,4 @@
-// b200spark — shared device helpers (sm_100a only): mbarrier, TMA bulk copy, cp.async, mma.sync,
+// b200spark — shared device helpers (sm_90a): mbarrier, TMA bulk copy, cp.async, mma.sync,
 // ldmatrix, programmatic dependent launch, error plumbing.
 #pragma once
 #include <cuda_bf16.h>

@@ -27,12 +27,12 @@ bool pdl_enabled() { return g_pdl != 0; }
 int sm_count() {
   static thread_local int cached_dev = -1, cached = 0;
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 132;
   if (dev != cached_dev) {
     cudaDeviceGetAttribute(&cached, cudaDevAttrMultiProcessorCount, dev);
     cached_dev = dev;
   }
-  return cached > 0 ? cached : 148;
+  return cached > 0 ? cached : 132;
 }
 
 int max_smem_optin() {
@@ -61,7 +61,7 @@ const char* b2_status_string(int s) {
 
 const char* b2_last_error(void) { return b2::g_last_error; }
 
-const char* b2_version(void) { return "b200spark 0.1 sm_100a"; }
+const char* b2_version(void) { return "b200spark 0.1 sm_90a"; }
 
 void b2_set_pdl(int enabled) { b2::g_pdl = enabled ? 1 : 0; }
 

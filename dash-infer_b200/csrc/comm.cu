@@ -1,4 +1,4 @@
-// b200spark — tensor-parallel exchange over NVLink peer memory, sm_100a.
+// b200spark — tensor-parallel exchange over NVLink peer memory, sm_90a.
 //
 // Replaces the reference's AllReduceOp (csrc/core/operator/nccl/allreduce/allreduce_op.cpp:73-115: ncclAllReduce on the
 // op's stream preceded by a ctx_->Synchronize() of the whole device) for the decode step's exchanges: [batch, hidden]

@@ -43,7 +43,7 @@ __global__ void __launch_bounds__(256) rmsnorm_kernel(__nv_bfloat16* __restrict_
   }
 }
 
-// ---- fp8 activations for the tcgen05 kind::f8f6f4 GEMM (b2_gemm_wq_run_fp8): per-token dynamic scale
+// ---- fp8 activations for the e4m3 wgmma GEMM (b2_gemm_wq_run_fp8): per-token dynamic scale
 //   scale[r] = max(|x[r,:]|, tiny) / 448 ;  y = e4m3(x / scale) (round to nearest even, saturating)
 // optional fused RMSNorm (gamma != NULL): x is first normalised exactly like rmsnorm_kernel (result rounded to bf16).
 // Layout of y ("b2 fp8 activation layout"): inside every aligned group of 8 k the bytes hold k = (0,2,4,6,1,3,5,7) — the

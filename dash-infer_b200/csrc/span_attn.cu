@@ -1,4 +1,4 @@
-// b200spark — SpanAttention decode: paged KV (spans) single-query attention, GQA, sm_100a.
+// b200spark — SpanAttention decode: paged KV (spans) single-query attention, GQA, sm_90a.
 //
 // Replaces the reference's three-kernel pipeline with a materialised score matrix
 // (span-attention/src/attn/qk/qk_gemv.cuh, softmax/block_softmax.cuh, qkv/qkv_gemv.cuh + reduce)

@@ -1,4 +1,4 @@
-// b200spark — weight-only quantized GEMV/GEMM for the decode step (small M), sm_100a.
+// b200spark — weight-only quantized GEMV/GEMM for the decode step (small M), sm_90a.
 //
 // Replaces the reference's K1/K2/K3/K6/K7/K8 kernels and the dequant+cuBLAS fallbacks
 // (csrc/core/kernel/cuda/gemm_lowp/gemm_a16w4_{perc,subc}_kernel.cu, gemm_a16w8_*_kernel.cu,
@@ -856,7 +856,7 @@ struct b2_gemm_wq {
   bool own_sz = false;
   unsigned* counters = nullptr;
   Plan plans[3];  // MT = 1, 2, 4
-  int tc_S = 0;   // split-K of the tcgen05 path (0 = not planned)
+  int tc_S = 0;   // split-K of the wgmma path (0 = not planned)
   int tc_S2 = 0;  // same for the two-CTAs-per-SM variant (int4, bf16 activations)
   bool pair = false;  // gate/up pair image (SwiGLU epilogue): physical channels = 2 * N
   int device = 0;
@@ -1009,7 +1009,7 @@ int b2_gemm_wq_create(b2_gemm_wq_t* out, const b2_gemm_wq_desc* d) {
   if (d->wbits == 8 && d->qtype != B2_DT_U8 && d->qtype != B2_DT_I8) return B2_ERR_PARAM;
   if (d->K % 8 != 0) return B2_ERR_UNSUPPORTED;
   bool general_groups = false;  // group sizes that do not divide the 64-k tile (reference: any multiple of 8 >= 32 through its
-                                // dequantize + cuBLAS path, gemm_a16w4.cpp:57-63): int4 only, tcgen05 kernel at every batch
+                                // dequantize + cuBLAS path, gemm_a16w4.cpp:57-63): int4 only, wgmma kernel at every batch
   if (d->wbits != 16 && d->group_size != -1) {
     if (d->group_size <= 0) return B2_ERR_UNSUPPORTED;
     if (d->group_size % kBK != 0) {
@@ -1129,7 +1129,7 @@ int b2_gemm_wq_attach_packed(b2_gemm_wq_t h, const void* packed, const void* sca
 }
 
 static int mt_index_for(int M) { return M <= 8 ? 0 : (M <= 16 ? 1 : 2); }
-// rows per launch of the mma.sync kernel.  Sub-channel weights at M > 16 (they have no tcgen05 path yet): the MT=4 grouped
+// rows per launch of the mma.sync kernel.  Sub-channel weights at M > 16 (they have no wgmma path yet): the MT=4 grouped
 // variant needs 124 registers (one CTA per SM, 0.05 of HBM at M=32), so they run in passes of 16 rows (MT=2, two CTAs per SM)
 // and stream the weights once per pass.  B2_GEMM_GROUPED_CHUNK=32 restores single-pass MT=4.
 static int rows_per_launch(const b2_gemm_wq* h) {
@@ -1141,7 +1141,7 @@ static bool use_tc(const b2_gemm_wq* h, int M) {
   static const int min_m = env_int("B2_GEMM_TC_MIN_M", 17);
   static const int grouped = env_int("B2_GEMM_TC_GROUPED", 1);
   // int4 / int8 per-channel, dense bf16 (lm_head), and int4 sub-channel (the scale is applied to the weights in the dequant warps)
-  if (h->group_k > 0) return true;  // general group sizes exist on the tcgen05 kernel only
+  if (h->group_k > 0) return true;  // general group sizes exist on the wgmma kernel only
   return M >= min_m && (h->group_tiles == 0 || (grouped && h->d.wbits == 4));
 }
 
@@ -1160,7 +1160,7 @@ static int make_tc_plan(b2_gemm_wq* h) {
   return B2_OK;
 }
 
-// two CTAs per SM on the tcgen05 path: int4 weights with bf16 activations (B2_GEMM_TC_DUAL=0: one 200 KB CTA per SM)
+// two CTAs per SM on the wgmma path: int4 weights with bf16 activations (B2_GEMM_TC_DUAL=0: one 194 KB CTA per SM)
 static bool tc_dual(const b2_gemm_wq* h) {
   static const int on = env_int("B2_GEMM_TC_DUAL", 1);  // 2: every int4 shape, 1: shapes with >= 2 units per SM without split-K
   if (!on || h->d.wbits != 4) return false;
@@ -1296,7 +1296,7 @@ static int run_impl(b2_gemm_wq_t h, const void* A, int64_t lda, void* C, int64_t
   if (workspace_bytes < b2_gemm_wq_workspace_bytes(h, M)) return B2_ERR_PARAM;
   cudaStream_t stream = (cudaStream_t)stream_;
   const bool grouped = h->group_tiles > 0;
-  if (use_tc(h, M) && !comm) {  // decode batches 17..: tcgen05 path, 64 rows per launch
+  if (use_tc(h, M) && !comm) {  // decode batches 17..: wgmma path, 64 rows per launch
     if (int st = make_tc_plan(h)) return st;
     const bool dual = tc_dual(h);
     const int tcs = dual ? h->tc_S2 : h->tc_S;

@@ -1,4 +1,4 @@
-// b200spark — definitions shared by the two weight-only GEMM kernels (mma.sync small-M, tcgen05 medium-M).
+// b200spark — definitions shared by the two weight-only GEMM kernels (mma.sync small-M, wgmma medium-M).
 #pragma once
 #include "b2_common.cuh"
 
@@ -20,7 +20,7 @@ __host__ __device__ __forceinline__ int tile_swz(int wbits, int c) {
   return wbits == 4 ? 4 * (c & 1) : (wbits == 8 ? 2 * (c & 3) : 2 * ((c >> 1) & 3));
 }
 
-// tcgen05 kernel entry (wq_gemm_tc.cu)
+// wgmma kernel entry (wq_gemm_tc.cu)
 struct TcLaunch {
   const uint8_t* packed;
   const float2* sz;
@@ -40,7 +40,7 @@ struct TcLaunch {
   int group_tiles = 0;               // > 0: sub-channel weights, k-tiles per quantization group (sz is [G][Np])
   int group_k = 0, ngroups = 1;      // group_k > 0: group size not a multiple of 64 (a multiple of 8): params per 8-k word
   bool fp16 = false;                 // activations / outputs / bias / residual are fp16 (else bf16)
-  bool dual = false;                 // two CTAs per SM (int4 weights, bf16 activations): half-depth stages, 256 TMEM columns
+  bool dual = false;                 // two CTAs per SM (int4 weights, bf16 activations): half-depth stages
   // RMSNorm hand-off between GEMMs (b2_gemm_fuse, batches >= 17).  Consumer: A holds bf16(x * gamma); the result rows are
   // scaled by rsqrt(sum_p norm_sumsq[p * norm_ld + m] / hidden + eps).  Producer: besides C it writes xg = bf16(C * gamma_out)
   // and, per 128-channel tile, the sum of squares of every stored row.
@@ -74,7 +74,7 @@ struct Gemv2Plan {
 bool gemv2_plan(const Gemv2Launch& a, Gemv2Plan* plan);   // false: use the split-K kernel
 cudaError_t gemv2_launch(const Gemv2Launch& a, const Gemv2Plan& plan, cudaStream_t stream);
 
-constexpr int kTcMaxM = 64;  // batch rows per tcgen05 launch
+constexpr int kTcMaxM = 64;  // batch rows per wgmma launch
 int tc_smem_bytes(int wbits, bool dual);
 cudaError_t tc_configure(int wbits);
 cudaError_t tc_launch(int wbits, const TcLaunch& a, cudaStream_t stream);

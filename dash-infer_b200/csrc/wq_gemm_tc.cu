@@ -1,37 +1,36 @@
-// b200spark — weight-only quantized (int4 / int8) and dense bf16 GEMM for decode batches 17..64 on the 5th-gen tensor
-// cores (tcgen05), sm_100a.
+// b200spark — weight-only quantized (int4 / int8) and dense bf16 GEMM for decode batches 17..64 on the Hopper warpgroup
+// tensor cores (wgmma), sm_90a.
 //
 // Replaces the reference's "dequantize the whole weight to a [K,N] bf16 workspace, then cuBLAS" fallback
 // (csrc/core/operator/general/gemm_lowp/gemm_a16w4_gpu.cpp:193-210, gemm_a16w8_gpu.cpp:210-237): 4.5 B of HBM
 // traffic per weight there, 0.5 B (int4) / 1 B (int8) here.
 //
-//   C^T[128 n x NM m] (fp32, TMEM) += W^T[128 n x 16 k] (bf16, TMEM) * A^T[16 k x NM m] (bf16, shared memory)
+//   C^T[128 n x NM m] (fp32, registers) += W^T[128 n x 16 k] (bf16, registers) * A^T[16 k x NM m] (bf16, shared memory)
 //
-//   warp 0      : TMA producer — int4/int8/bf16 weight tiles (same init-time image as the mma.sync kernel) stream
+//   warps 0..7  : two consumer warpgroups, 64 output channels each.  Every thread dequantizes the weights of its wgmma
+//                 A-operand fragment (rows g and g + 8 of its warp's 16, the k pairs 2t and 2t + 8 of every k16 step):
+//                 LDS.128 of the row's image chunk -> shf/lop3 -> exact bf16 integers (16+q) in registers, which
+//                 wgmma.mma_async reads directly (the dequantized weights never touch shared memory: its bandwidth could
+//                 not carry 2 B/weight at HBM rate).  One commit group per 64-k tile, at most two in flight, so the
+//                 dequantization of tile t+1 overlaps the MMAs of tile t; the accumulators stay in registers.
+//   warp 8      : TMA producer — int4/int8/bf16 weight tiles (same init-time image as the mma.sync kernel) stream
 //                 HBM -> shared memory with cp.async.bulk (16 KB stages), ahead of the previous kernel's completion (PDL)
-//   warps 2..5, : dequant — one thread per output channel: LDS.128 -> lop3/shf -> exact bf16 integers (16+q)
-//   warps 9..12   -> tcgen05.st into the A-operand region of TMEM (the dequantized weights never touch shared
-//                 memory: its bandwidth could not carry 2 B/weight at HBM rate).  Two groups of four warps take
-//                 alternate pipeline stages: one stage is a serial chain of barrier waits, LDS, ALU, tcgen05.st
-//                 and wait::st (~1000 clocks measured), two in flight hide it
-//   warp 8      : activation tiles (64 k x NM m) by TMA tensor-map loads into the 128B-swizzled K-major UMMA
-//                 layout (out-of-range rows/columns are zero-filled by the TMA unit)
-//   warps 6..7  : per-row sums sum_k a[m][k] needed by the zero-point term, read from the landed tiles
-//   warp 1      : one elected thread issues tcgen05.mma (A from TMEM, B from shared memory, D in TMEM) and
-//                 tcgen05.commit's the pipeline barriers
-//   epilogue    : the dequant warps read D with tcgen05.ld, apply s * (acc - (16+z) * sum a) and park the fp32 tile in
-//                 the drained activation ring; then ALL 416 threads do the split-K partial store / last-CTA reduction and
-//                 the final alpha/bias/activation/residual (or SwiGLU) with 16-byte reads and 8-byte bf16x4 stores.
+//   warp 9      : activation tiles (64 k x NM m) by TMA tensor-map loads into the 128B-swizzled K-major layout the wgmma
+//                 B descriptor reads (out-of-range rows/columns are zero-filled by the TMA unit)
+//   warps 10..11: per-row sums sum_k a[m][k] needed by the zero-point term, read from the landed tiles
+//   epilogue    : the consumers apply s * (acc - (16+z) * sum a) to their accumulators and park the fp32 tile in the drained
+//                 activation ring; then ALL 384 threads do the split-K partial store / last-CTA reduction and the final
+//                 alpha/bias/activation/residual (or SwiGLU) with 16-byte reads and 8-byte bf16x4 stores.
 //   persistent  : when there are more (n-group, k-split) units than SMs (gate+up pair, lm_head) one CTA per SM walks
-//                 several units; barriers, TMEM and ring phases carry over and the next unit's first weight stages are
-//                 issued before the epilogue (MULTI instantiation).
+//                 several units; barriers and ring phases carry over and the next unit's first weight stages are issued
+//                 before the epilogue (MULTI instantiation).
 //
-//   variants    : DUAL (two CTAs per SM: half-depth stages, 256 TMEM columns — used where >= 2 units per SM exist without more
-//                 split-K), GROUPED (sub-channel int4: the scale is applied to the weights in the dequant warps; group sizes that
-//                 do not divide the 64-k tile look their params up per 8-k word), A8 (fp8 activations, kind::f8f6f4), H (fp16
+//   variants    : DUAL (two CTAs per SM: half-depth stages — used where >= 2 units per SM exist without more split-K),
+//                 GROUPED (sub-channel int4: the scale is applied to the weights at dequantization; group sizes that do not
+//                 divide the 64-k tile look their params up per 8-k word), A8 (fp8 activations, e4m3 wgmma), H (fp16
 //                 instead of bf16 activations / outputs), the RMSNorm hand-off (row statistics + gamma-scaled copy out, 1/rms in).
 //
-// Roofline: HBM-bound up to M ~ 64 (256 FLOP/B ~ the tensor/HBM ridge); report both.
+// Roofline: HBM-bound up to M ~ 64 (~300 FLOP/B is the H100 tensor/HBM ridge); report both.
 #include <cuda.h>  // CUtensorMap (types only; the encoder is fetched with cudaGetDriverEntryPoint)
 
 #include <cstdlib>
@@ -41,97 +40,96 @@
 
 namespace b2 {
 
-constexpr int kTcThreads = 416;      // warp 0 weights TMA, 1 MMA, 2-5 + 9-12 dequant (two groups, alternate stages), 6-7 row sums,
-                                     // 8 activation TMA; every warp joins the epilogue
-constexpr int kTcNM = 64;            // batch columns per MMA (UMMA N)
-constexpr int kTcNSW = 6;            // weight stages (16 KB each): ~2 us of HBM latency x 44 GB/s/SM needs >= 80 KB in flight
-constexpr int kTcNSX = 3;            // {dequantized-A buffer in TMEM, activation slot in smem} stages (128 columns / 32 or 16 KB each)
+constexpr int kTcThreads = 384;      // warps 0-7 two consumer warpgroups, 8 weights TMA, 9 activation TMA, 10-11 row sums;
+                                     // every warp joins the epilogue
+constexpr int kTcNM = 64;            // batch columns per MMA (wgmma N)
+constexpr int kTcNSW = 6;            // weight stages (16 KB each): ~2 us of HBM latency x 25 GB/s/SM needs >= 50 KB in flight
+constexpr int kTcNSX = 3;            // activation stages (32 or 16 KB each)
 constexpr int kTcXTile = kTcNM * 128;  // bytes: NM rows x 64 k bf16
-constexpr int kTcColsD = 0;          // TMEM columns [0, 64): accumulator
-constexpr int kTcColsA = 64;         // TMEM columns [64, 64 + 128 * NSX): the A stages, 128 columns each
-constexpr int kTcTmemCols = 512;
 
-// ---- tcgen05 wrappers (forms as in cute/arch/{mma_sm100_umma,copy_sm100,tmem_allocator_sm100}.hpp) ----
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+// ---- wgmma wrappers (PTX ISA 8.0, sm_90a): A from registers, B from a shared-memory descriptor, D in registers ----
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator accesses across the asynchronous MMAs
+__device__ __forceinline__ void wg_fence_acc(float (&d)[32]) {
+#pragma unroll
+  for (int i = 0; i < 32; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tc_st8(uint32_t taddr, const uint32_t (&r)[8]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"r"(taddr), "r"(r[0]), "r"(r[1]),
-               "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-               : "memory");
-}
-__device__ __forceinline__ void tc_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,"
-      "%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-        "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem desc]
-__device__ __forceinline__ void tc_mma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, {%5, %5, %5, %5}, p;\n\t}"
-      ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate), "r"(0u)
-      : "memory");
+// K-major operand, 128-byte swizzle, 8-row groups 1024 B apart; a k16 (bf16) or k32 (e4m3) step inside the swizzle atom is
+// +32 B, i.e. +2 in the start-address field
+__device__ __forceinline__ uint64_t wg_desc(uint32_t saddr) {
+  return (uint64_t)((saddr >> 4) & 0x3FFF) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
 }
 
-// fp8 (e4m3 x e4m3 -> fp32), K = 32 per instruction
-__device__ __forceinline__ void tc_mma_ts_f8(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f8f6f4 [%0], [%1], %2, %3, {%5, %5, %5, %5}, p;\n\t}"
-      ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate), "r"(0u)
-      : "memory");
+#define B2_WG_D16 "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}"
+#define B2_WG_D32                                                                                                          \
+  "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}"
+#define B2_WG_ACC16(d)                                                                                                       \
+  "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), \
+      "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+#define B2_WG_ACC32(d)                                                                                                       \
+  B2_WG_ACC16(d), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), \
+      "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+
+// D[64 x NM] += A[64 x k] (registers) * B[k x NM] (smem): KIND 0 = bf16 (k16), 1 = fp16 (k16), 2 = e4m3 (k32).  NM = 32 uses
+// d[0..15] only.
+template <int KIND>
+__device__ __forceinline__ void wg_mma(float (&d)[32], const uint32_t (&a)[4], uint64_t desc, bool n32) {
+  if (n32) {
+    if (KIND == 0)
+      asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
+                   "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 " B2_WG_D16 ", {%16,%17,%18,%19}, %20, p, 1, 1, 0;\n\t}"
+                   : B2_WG_ACC16(d) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc), "r"(1));
+    else if (KIND == 1)
+      asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
+                   "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 " B2_WG_D16 ", {%16,%17,%18,%19}, %20, p, 1, 1, 0;\n\t}"
+                   : B2_WG_ACC16(d) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc), "r"(1));
+    else
+      asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
+                   "wgmma.mma_async.sync.aligned.m64n32k32.f32.e4m3.e4m3 " B2_WG_D16 ", {%16,%17,%18,%19}, %20, p, 1, 1;\n\t}"
+                   : B2_WG_ACC16(d) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc), "r"(1));
+  } else {
+    if (KIND == 0)
+      asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+                   "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 " B2_WG_D32 ", {%32,%33,%34,%35}, %36, p, 1, 1, 0;\n\t}"
+                   : B2_WG_ACC32(d) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc), "r"(1));
+    else if (KIND == 1)
+      asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+                   "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 " B2_WG_D32 ", {%32,%33,%34,%35}, %36, p, 1, 1, 0;\n\t}"
+                   : B2_WG_ACC32(d) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc), "r"(1));
+    else
+      asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+                   "wgmma.mma_async.sync.aligned.m64n64k32.f32.e4m3.e4m3 " B2_WG_D32 ", {%32,%33,%34,%35}, %36, p, 1, 1;\n\t}"
+                   : B2_WG_ACC32(d) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc), "r"(1));
+  }
 }
+
 __device__ __forceinline__ uint32_t tc_prmt(uint32_t a, uint32_t b, uint32_t sel) {
   uint32_t d;
   asm("prmt.b32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(sel));
   return d;
 }
-// 8 int4 codes of one image word -> 8 e4m3 bytes (exact: 0..15 are e4m3 values) in two registers:
-// P = codes of k (0,2,4,6), Q = codes of k (1,3,5,7) of the word's 8 consecutive k — the byte order of the b2 fp8 activation
-// layout (glue.cu quant_fp8_kernel).  Byte-permute look-ups: codes 0..7 from one 8-byte table, 8..15 are 0x50 | (q & 7) from a
-// second one, the choice by a sign-replicating permute of bit 3 of every nibble.  13 ALU ops per 8 weights.
-__device__ __forceinline__ void nib8_to_e4m3(uint32_t w_rot3, uint32_t& P, uint32_t& Q) {
+__device__ __forceinline__ uint32_t lds32(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(addr));
+  return v;
+}
+// 4 of the 8 int4 codes of one image word -> 4 e4m3 bytes (exact: 0..15 are e4m3 values): half 0 = codes of k (0,2,4,6),
+// half 1 = codes of k (1,3,5,7) of the word's 8 consecutive k — the byte order of the b2 fp8 activation layout (glue.cu
+// quant_fp8_kernel).  Byte-permute look-ups: codes 0..7 from one 8-byte table, 8..15 are 0x50 | (q & 7) from a second one,
+// the choice by a sign-replicating permute of bit 3 of every nibble.  qsh = 16 * half, msel = half ? 0xFBEA : 0xD9C8.
+__device__ __forceinline__ uint32_t nib4_to_e4m3(uint32_t w_rot3, uint32_t qsh, uint32_t msel) {
   const uint32_t word = __funnelshift_r(w_rot3, w_rot3, 3);  // the image stores words rotated left by 3 (bf16 path)
-  const uint32_t sel = word & 0x77777777u, selh = sel >> 16;
+  const uint32_t sel = (word & 0x77777777u) >> qsh;
   const uint32_t T0 = 0x44403800u, T1 = 0x4E4C4A48u, H0 = 0x53525150u, H1 = 0x57565554u;
-  const uint32_t plo = tc_prmt(T0, T1, sel), qlo = tc_prmt(T0, T1, selh);
-  const uint32_t phi = tc_prmt(H0, H1, sel), qhi = tc_prmt(H0, H1, selh);
-  const uint32_t ws = word << 4;
-  const uint32_t mp = tc_prmt(ws, word, 0xD9C8u), mq = tc_prmt(ws, word, 0xFBEAu);  // 0xFF where the nibble is >= 8
-  asm("lop3.b32 %0, %1, %2, %3, 0xD8;" : "=r"(P) : "r"(plo), "r"(phi), "r"(mp));   // mp ? phi : plo
-  asm("lop3.b32 %0, %1, %2, %3, 0xD8;" : "=r"(Q) : "r"(qlo), "r"(qhi), "r"(mq));
+  const uint32_t lo = tc_prmt(T0, T1, sel), hi = tc_prmt(H0, H1, sel);
+  const uint32_t m = tc_prmt(word << 4, word, msel);  // 0xFF where the nibble is >= 8
+  uint32_t r;
+  asm("lop3.b32 %0, %1, %2, %3, 0xD8;" : "=r"(r) : "r"(lo), "r"(hi), "r"(m));  // m ? hi : lo
+  return r;
 }
-
-// optional timeline instrumentation (CTA 0 only): compiled in with -DB2_TC_TRACE
-#ifdef B2_TC_TRACE
-__device__ unsigned long long g_tc_trace[16][256];
-__device__ unsigned long long g_tc_gt[64][8];  // per launch (ring): globaltimer + clock at entry / end of CTA 0 and the last CTA
-__device__ __forceinline__ unsigned long long tc_gtime() {
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-  return t;
-}
-#define TC_TRACE(role, idx) do { if (blockIdx.x == 0 && (idx) < 256) g_tc_trace[role][idx] = clock64(); } while (0)
-#define TC_GT(slot) do { if (blockIdx.x == 0 || blockIdx.x == gridDim.x - 1) { \
-    const int b_ = blockIdx.x == 0 ? 0 : 4; \
-    g_tc_gt[p.dbg & 63][b_ + (slot)] = tc_gtime(); } } while (0)
-#else
-#define TC_TRACE(role, idx) do {} while (0)
-#define TC_GT(slot) do {} while (0)
-#endif
 
 struct TcParams {
   const uint8_t* packed;
@@ -162,49 +160,35 @@ struct TcParams {
   int group_tiles;  // GROUPED instantiation: k-tiles per quantization group; sz is [G][Np]
   int group_k, ngroups;  // GROUPED with a group size that is no multiple of 64 (a multiple of 8, >= 32): 8 consecutive k — one
                          // word of the image — never straddle a group, so the params are looked up per word
-  int dbg;  // ablation bitmask, only honoured when compiled with -DB2_TC_ABLATE (tools/tc_ablate.py)
 };
 
-// Timing-only ablations (results are wrong): 1 row sums skip their loads, 2 dequant skips everything, 4 no MMAs,
-// 8 no activation TMA, 16 dequant skips only the tcgen05.st, 32 no weight TMA
-#ifdef B2_TC_ABLATE
-#define TC_ABL(bit) ((p.dbg & (bit)) != 0)
-#else
-#define TC_ABL(bit) false
-#endif
-
 // MULTI: a CTA walks several units (more units than SMs); the single-unit instantiation folds the unit loop away
-// A8: fp8-e4m3 activations (b2_gemm_wq_run_fp8, int4 weights only): the int4 codes go to TMEM as exact e4m3 bytes, the MMAs
-// are kind::f8f6f4 with K = 32 (half the MMAs and half the TMEM stores of the bf16 path), an activation tile is 128 k wide.
+// A8: fp8-e4m3 activations (b2_gemm_wq_run_fp8, int4 weights only): the int4 codes become exact e4m3 bytes, the MMAs are
+// e4m3 x e4m3 with K = 32 (half the MMAs of the bf16 path), an activation tile is 128 k wide.
 // GROUPED: sub-channel weights (GPTQ g128 ...): the (scale, zero) of a channel changes every group_tiles k-tiles, so the affine
-// dequantisation cannot wait for the accumulator.  The dequant warps apply it to the weights instead — exact integer (q - 8)
+// dequantisation cannot wait for the accumulator.  The consumers apply it to the weights instead — exact integer (q - 8)
 // in bf16, then ONE fused multiply-add per two weights: w = (q - 8) * s + (8 - z) * s, rounded to bf16 once — which is what
 // the reference's kernels (dequant in FT, gemm_lowp_utils.cuh:28-47) and its CPU path (weights stored in the model dtype)
 // feed their GEMMs with; the accumulator then needs no zero-point term and no row sums.
-// DUAL: two CTAs per SM (int4, bf16 activations).  A stage is half as deep (k128: 8 KB of weights, 16 KB of activations, 64
-// TMEM columns of dequantized A), so a CTA needs 97 KB of shared memory and 256 TMEM columns; the fixed part of a unit —
-// prologue, pipeline fill, accumulator read-out, split-K hand-off, epilogue (6.4 of 17.6 us on the gate projection,
-// profiles/r2_timelines.md) — overlaps the main loop of the CTA next to it instead of idling the SM.
-// H: fp16 activations / outputs (kind::f16 takes either 16-bit format; the exact-integer constants are 128 + q instead of 16 + q).
+// DUAL: two CTAs per SM (int4, bf16 activations).  A stage is half as deep (k128: 8 KB of weights, 16 KB of activations), so a
+// CTA needs 98 KB of shared memory; the fixed part of a unit — prologue, pipeline fill, split-K hand-off, epilogue — overlaps
+// the main loop of the CTA next to it instead of idling the SM.
+// H: fp16 activations / outputs (the exact-integer constants are 128 + q instead of 16 + q).
 template <int WBITS, bool MULTI, bool A8 = false, bool GROUPED = false, bool DUAL = false, bool H = false>
 __global__ void __launch_bounds__(kTcThreads, DUAL ? 2 : 1) wq_gemm_tc_kernel(const TcParams p, const __grid_constant__ CUtensorMap amap) {
   constexpr int TILE_BYTES = WBITS == 4 ? 4096 : (WBITS == 8 ? 8192 : 16384);
   constexpr int NCH = WBITS == 4 ? 2 : (WBITS == 8 ? 4 : 8);  // 16B chunks per row per k-tile
   constexpr int NSW = WBITS == 16 ? 4 : kTcNSW;               // weight stages (bf16: 32 KB each)
-  // k-tiles per pipeline stage (k256 for W4, k128 for W8): one stage = 16 KB of weights = 16 tcgen05.mma per
-  // commit / barrier round trip of the issuing thread (that round trip costs ~400 clocks, an MMA 45)
+  // k-tiles per pipeline stage (k256 for W4, k128 for W8): one stage = 16 KB of weights per barrier round trip
   constexpr int TPS = WBITS == 4 ? (DUAL ? 2 : 4) : 2;
-  constexpr int TMEM_COLS = DUAL ? 256 : kTcTmemCols;
+  constexpr int KIND = A8 ? 2 : (H ? 1 : 0);
   static_assert(!A8 || WBITS == 4, "fp8 activations: int4 weights only");
   static_assert(!DUAL || (WBITS == 4 && !A8), "two CTAs per SM: int4 weights, 16-bit activations");
   static_assert(!H || !A8, "fp8 activations come with bf16 outputs");
   using F = Ft<H>;
   static_assert(!GROUPED || (!A8 && WBITS != 16), "sub-channel weights: bf16 activations, int4 / int8");
   const int XTILE_LD = p.nm * 128;             // bytes the TMA writes per activation tile (the tile slot stays 64 rows)
-  constexpr int ACOLS = A8 ? 16 : (WBITS == 8 ? 64 : 32);  // TMEM columns of dequantized A per k-tile (int8: lo and hi planes)
   constexpr int XTPS = A8 ? TPS / 2 : TPS;     // activation tiles per stage (fp8: 128 k per 128-byte row)
-  constexpr int ABUF = ACOLS * TPS;            // per stage (128 columns)
-  constexpr int NAB = kTcNSX;                  // A stages in TMEM == activation stages (one 'ready' barrier per stage)
   constexpr int WSTAGE = TPS * TILE_BYTES;     // 16 KB
   constexpr int XSTAGE = XTPS * kTcXTile;      // 32 KB / 16 KB
   extern __shared__ uint8_t smem_raw[];
@@ -214,46 +198,27 @@ __global__ void __launch_bounds__(kTcThreads, DUAL ? 2 : 1) wq_gemm_tc_kernel(co
   float* suma = reinterpret_cast<float*>(wring + NSW * WSTAGE);  // [NM]
   uint64_t* bars = reinterpret_cast<uint64_t*>(suma + kTcNM);
   uint64_t* wfull = bars;                 // [NSW] weights landed (TMA tx)
-  uint64_t* wfree = wfull + kTcNSW;       // [NSW] dequant warps done with the smem stage (4 arrivals)
-  uint64_t* xfull = wfree + kTcNSW;       // [NSX] (reserved; the activation TMA completes on afull)
-  uint64_t* xsum = xfull + kTcNSX;        // [NSX] row sums done with the stage (2 arrivals)
-  uint64_t* afull = xsum + kTcNSX;        // [NAB] stage ready: activation TMA tx + 4 dequant-warp arrivals (A stage in TMEM)
-  uint64_t* mdone = afull + NAB;          // [NSX] tensor core done with stage (tcgen05.commit): frees A buffer + X slot
-  uint64_t* dfull = mdone + kTcNSX;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(dfull + 1);
-  float* ascale = reinterpret_cast<float*>(bars) + 64;  // [NM] per-token activation scales (A8), 256 B into the barrier block
+  uint64_t* wfree = wfull + kTcNSW;       // [NSW] consumer warps done reading the smem stage (8 arrivals)
+  uint64_t* afull = wfree + kTcNSW;       // [NSX] activation tiles landed (TMA tx)
+  uint64_t* xsum = afull + kTcNSX;        // [NSX] row sums done with the stage (2 arrivals)
+  uint64_t* xfree = xsum + kTcNSX;        // [NSX] the MMAs reading the stage completed (8 consumer-warp arrivals)
+  float* ascale = reinterpret_cast<float*>(bars) + 64;  // [NM] per-token activation scales (A8) or 1/rms, 256 B into the barrier block
   __shared__ int s_is_last;
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  if (tid == 0) { TC_GT(0); TC_TRACE(7, 5); }
   const int nunits = p.NG * p.S;
 
   if (tid == 0) {
-    for (int i = 0; i < NSW; ++i) { mbar_init(&wfull[i], 1); mbar_init(&wfree[i], 4); }
-    // afull = stage ready: activation TMA tx + 4 dequant-warp arrivals (the MMA thread and the row-sum warps wait on it)
-    for (int i = 0; i < kTcNSX; ++i) { mbar_init(&xfull[i], 1); mbar_init(&xsum[i], 2); mbar_init(&mdone[i], 1); mbar_init(&afull[i], 5); }
-    mbar_init(dfull, 1);
+    for (int i = 0; i < NSW; ++i) { mbar_init(&wfull[i], 1); mbar_init(&wfree[i], 8); }
+    for (int i = 0; i < kTcNSX; ++i) { mbar_init(&afull[i], 1); mbar_init(&xsum[i], 2); mbar_init(&xfree[i], 8); }
     fence_mbar_init();
   }
-  if (warp == 1) {  // TMEM allocation (this warp also frees it)
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  // warp-uniform for the compiler: tcgen05 operands then live in uniform registers (otherwise every tcgen05.mma is
-  // wrapped in an ELECT / R2UR.BROADCAST waterfall loop, ~70 clocks per MMA instead of the 45-clock hardware floor)
-  const uint32_t tmem = __shfl_sync(0xffffffffu, *tmem_slot, 0);
-  if (tid == 0) TC_TRACE(7, 4);
   pdl_launch_dependents();
 
-  // Persistent over work units (n-group, k-split): unit = blockIdx.x, += gridDim.x.  Barriers, TMEM and the ring phases carry
-  // over; g = gbase + st is the stage index since kernel start.  Stage g uses weight slot g % NSW, X slot g % NSX, A buffer
-  // g % NAB; mdone[g % NSX] is committed once the tensor core has consumed stage g (NSX == NAB, so its phase also tells when
-  // the A buffer is free).
+  // Persistent over work units (n-group, k-split): unit = blockIdx.x, += gridDim.x.  Barriers and the ring phases carry over;
+  // g = gbase + st is the stage index since kernel start.  Stage g uses weight slot g % NSW and X slot g % NSX.
   int w_pre = 0;  // weight stages of the current unit already issued during the previous unit's tail (producer thread only)
-  // (loop control and everything the tcgen05.mma operands derive from must stay provably warp-uniform: see `tmem`)
   const int my_units = !MULTI ? 1 : ((int)blockIdx.x < nunits) ? (nunits - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x : 0;
   for (int uit = 0; uit < my_units; ++uit) {
   const int unit = (int)blockIdx.x + uit * (int)gridDim.x;
@@ -262,24 +227,19 @@ __global__ void __launch_bounds__(kTcThreads, DUAL ? 2 : 1) wq_gemm_tc_kernel(co
   const int kt0 = (int)((int64_t)s * p.KT / p.S), kt1 = (int)((int64_t)(s + 1) * p.KT / p.S);
   const int nt = kt1 - kt0;
   const int nst = (nt + TPS - 1) / TPS;  // pipeline stages of this unit
-  // stages before this unit.  A CTA only walks several units when S == 1, where every unit has the same stage count; a
-  // closed form (not a loop-carried sum) keeps the value provably warp-uniform for the tcgen05.mma operands
+  // stages before this unit.  A CTA only walks several units when S == 1, where every unit has the same stage count
   const int gbase = MULTI ? uit * nst : 0;
-  if (warp == 0) {
+  if (warp == 8) {
     // ===================== weight producer (does not wait for the previous kernel) =====================
     if (lane == 0) {
       auto issue = [&](int g, const uint8_t* src, uint32_t bytes) {
         const int slot = g % NSW;
         if (g >= NSW) mbar_wait_backoff(&wfree[slot], ((g / NSW) & 1) ^ 1);
-        if (TC_ABL(32)) { mbar_arrive(&wfull[slot]); return; }
         mbar_arrive_expect_tx(&wfull[slot], bytes);
         bulk_g2s(wring + slot * WSTAGE, src, bytes, &wfull[slot]);
       };
       const uint8_t* wsrc = p.packed + ((size_t)ng * p.KT + kt0) * TILE_BYTES;
-      for (int st = w_pre; st < nst; ++st) {
-        issue(gbase + st, wsrc + (size_t)st * WSTAGE, min(TPS, nt - st * TPS) * TILE_BYTES);
-        TC_TRACE(0, gbase + st);
-      }
+      for (int st = w_pre; st < nst; ++st) issue(gbase + st, wsrc + (size_t)st * WSTAGE, min(TPS, nt - st * TPS) * TILE_BYTES);
       // head of the next unit: its first stages stream in while this unit drains and runs its epilogue
       w_pre = 0;
       const int nu = unit + gridDim.x;
@@ -293,24 +253,20 @@ __global__ void __launch_bounds__(kTcThreads, DUAL ? 2 : 1) wq_gemm_tc_kernel(co
           issue(gbase + nst + st, wsrc2 + (size_t)st * WSTAGE, min(TPS, nt2 - st * TPS) * TILE_BYTES);
       }
     }
-  } else if (warp == 8) {
+  } else if (warp == 9) {
     // ===================== activation producer: TMA tensor-map loads (zero fill outside [M, K]) =====================
     if (lane == 0) {
       pdl_wait();  // A is the previous kernel's output
-      if (uit == 0) { TC_GT(1); TC_TRACE(7, 6); }
       for (int st = 0; st < nst; ++st) {
         const int g = gbase + st;
         const int slot = g % kTcNSX;
         if (g >= kTcNSX) {
           const uint32_t par = ((g / kTcNSX) & 1) ^ 1;
-          mbar_wait_backoff(&mdone[slot], par);
+          mbar_wait_backoff(&xfree[slot], par);
           mbar_wait_backoff(&xsum[slot], par);
         }
         const int wtiles = min(TPS, nt - st * TPS);
         const int tiles = A8 ? (wtiles + 1) / 2 : wtiles;     // activation tiles (fp8: one per two 64-k weight tiles)
-        // the loads complete on the stage's 'ready' barrier (what the MMA thread waits for, together with the dequant
-        // arrivals); the row-sum warps wait on the same barrier phase
-        if (TC_ABL(8)) { mbar_arrive(&afull[slot]); continue; }
         mbar_arrive_expect_tx(&afull[slot], tiles * XTILE_LD);
         for (int ti = 0; ti < tiles; ++ti)
           asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
@@ -319,73 +275,9 @@ __global__ void __launch_bounds__(kTcThreads, DUAL ? 2 : 1) wq_gemm_tc_kernel(co
                        : "memory");
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer: a single thread =====================
-    // re-broadcast what the tcgen05.mma operands derive from: outer-loop values are not provably warp-uniform for the
-    // compiler, and a non-uniform operand costs an R2UR waterfall per MMA (see `tmem`)
-    const int gb = __shfl_sync(0xffffffffu, gbase, 0);
-    const int nst_u = __shfl_sync(0xffffffffu, nst, 0), nt_u = __shfl_sync(0xffffffffu, nt, 0);
-    const uint32_t nm_u = (uint32_t)__shfl_sync(0xffffffffu, p.nm, 0);
-    if (lane == 0) {
-      // instruction descriptor: D=f32, A=B=bf16, both K-major, N = NM, M = 128 (cute::UMMA::InstrDescriptor)
-      // (fp8: a_format = b_format = 0 = E4M3)
-      const uint32_t idesc = A8 ? ((1u << 4) | ((nm_u >> 3) << 17) | ((uint32_t)(128 >> 4) << 24))
-                                : ((1u << 4) | (H ? 0u : ((1u << 7) | (1u << 10))) | ((nm_u >> 3) << 17) | ((uint32_t)(128 >> 4) << 24));
-      // B smem descriptor (cute::UMMA::SmemDescriptor): K-major, SWIZZLE_128B, SBO = 1024 B (8-row groups), version 1
-      const uint64_t desc_hi = (uint64_t)((1024u >> 4) | (1u << 14) | (2u << 29)) << 32;
-      const uint32_t xbase = smem_u32(xring);
-      for (int st = 0; st < nst_u; ++st) {
-        const int g = gb + st;
-        const int ab = g % NAB, xs = g % kTcNSX;
-        mbar_wait(&afull[ab], (g / NAB) & 1);  // dequantized A stored in TMEM and activations landed
-        tc_fence_after();
-        TC_TRACE(1, g);
-        const int tiles = min(TPS, nt_u - st * TPS);
-        if (A8) {  // an activation tile = 128 k = two weight tiles = four K=32 steps
-#pragma unroll
-          for (int xi = 0; xi < XTPS; ++xi) {
-            if (2 * xi < tiles) {
-              const uint32_t xaddr = xbase + xs * XSTAGE + xi * kTcXTile;
-              const uint64_t bdesc0 = desc_hi | (uint64_t)(((xaddr >> 4) & 0x3FFF) | (1u << 16));
-#pragma unroll
-              for (int kk = 0; kk < 4; ++kk) {
-                const int ti = 2 * xi + (kk >> 1);
-                if (ti < tiles && !TC_ABL(4))
-                  tc_mma_ts_f8(tmem + kTcColsD, tmem + kTcColsA + ab * ABUF + ti * ACOLS + (kk & 1) * 8, bdesc0 + (uint64_t)(2 * kk), idesc,
-                               (st > 0 || xi > 0 || kk > 0) ? 1u : 0u);
-              }
-            }
-          }
-        }
-#pragma unroll
-        for (int ti = 0; ti < TPS; ++ti) {
-          if (!A8 && ti < tiles) {
-            const uint32_t xaddr = xbase + xs * XSTAGE + ti * kTcXTile;
-            // start-address field is (addr >> 4): a k16 step (32 B) inside the swizzle atom is +2
-            const uint64_t bdesc0 = desc_hi | (uint64_t)(((xaddr >> 4) & 0x3FFF) | (1u << 16));
-#pragma unroll
-            for (int kk = 0; kk < 4; ++kk) {
-              const uint64_t bdesc = bdesc0 + (uint64_t)(2 * kk);
-              const uint32_t acc = (st > 0 || ti > 0 || kk > 0) ? 1u : 0u;
-              if (ti * 4 + kk == TPS * 4 - 1) TC_TRACE(15, g);
-              if (TC_ABL(4)) continue;
-              if (WBITS != 8) {
-                tc_mma_ts(tmem + kTcColsD, tmem + kTcColsA + ab * ABUF + ti * ACOLS + kk * 8, bdesc, idesc, acc);
-              } else {  // W8: per k16 step the buffer holds [lo plane | hi plane], 8 columns each
-                tc_mma_ts(tmem + kTcColsD, tmem + kTcColsA + ab * ABUF + ti * ACOLS + kk * 16, bdesc, idesc, acc);
-                tc_mma_ts(tmem + kTcColsD, tmem + kTcColsA + ab * ABUF + ti * ACOLS + kk * 16 + 8, bdesc, idesc, 1u);
-              }
-            }
-          }
-        }
-        tc_commit(&mdone[xs]);
-        if (st == nst_u - 1) tc_commit(dfull);
-        TC_TRACE(2, g);
-      }
-    }
-  } else if (warp == 6 || warp == 7) {
+  } else if (warp >= 10) {
     // ===================== row sums of the landed activation tiles (row = xt) =====================
-    const int xt = tid - 192;  // 0..63
+    const int xt = tid - 320;  // 0..63
     float r0 = 0.f, r1 = 0.f, r2 = 0.f, r3 = 0.f;
     if (A8) {  // the quantizer already summed every 64-k tile of every row: add this unit's tiles; stage the token scales
       pdl_wait();
@@ -407,8 +299,8 @@ __global__ void __launch_bounds__(kTcThreads, DUAL ? 2 : 1) wq_gemm_tc_kernel(co
     for (int st = 0; st < nst; ++st) {
       const int g = gbase + st;
       const int slot = g % kTcNSX;
-      mbar_wait(&afull[slot], (g / kTcNSX) & 1);  // stage ready (implies its activation tiles landed)
-      const int tiles = (TC_ABL(1) || WBITS == 16 || A8 || GROUPED || xt >= p.nm) ? 0 : min(TPS, nt - st * TPS);  // (no zero-point term)
+      mbar_wait(&afull[slot], (g / kTcNSX) & 1);  // activation tiles landed
+      const int tiles = (WBITS == 16 || A8 || GROUPED || xt >= p.nm) ? 0 : min(TPS, nt - st * TPS);  // (no zero-point term)
       for (int ti = 0; ti < tiles; ++ti) {
         const uint32_t rbase = smem_u32(xring + slot * XSTAGE + ti * kTcXTile) + xt * 128;
 #pragma unroll
@@ -423,200 +315,217 @@ __global__ void __launch_bounds__(kTcThreads, DUAL ? 2 : 1) wq_gemm_tc_kernel(co
       }
       __syncwarp();
       if (lane == 0) mbar_arrive(&xsum[slot]);
-      if (xt == 0) TC_TRACE(3, g);
     }
     suma[xt] = (r0 + r1) + (r2 + r3);
-    asm volatile("bar.sync 3, 320;" ::: "memory");  // hand the sums to the dequant/epilogue warps
+    asm volatile("bar.sync 3, 320;" ::: "memory");  // hand the sums to the consumers
   } else {
-    // ===================== dequant (warps 2..5: even stages, warps 9..12: odd stages), then TMEM -> smem =====================
-    const int grp = warp >= 9 ? 1 : 0;
-    const int q = warp & 3;             // TMEM lane quadrant this warp may access
-    const int r = q * 32 + lane;        // output channel (row of the 128-row tile)
-    // per-channel (scale, zero + bias constant): immutable, read before the wait
-    const float2 sz = (WBITS == 16 || GROUPED) ? make_float2(1.f, 0.f) : p.sz[ng * kBN + r];
-    const uint32_t trow = tmem + ((uint32_t)(q * 32) << 16);
-    const uint32_t wring_u = smem_u32(wring);
-    const bool tracer = tid == 64;
-    uint32_t woff[NCH];
+    // ===================== consumers: dequantize into wgmma A fragments, MMA, accumulators -> smem tile =====================
+    const int wg = warp >> 2, g8 = lane >> 2, t4 = lane & 3;
+    const int rr0 = wg * 64 + (warp & 3) * 16 + g8, rr1 = rr0 + 8;  // the two output channels (tile rows) of this thread
+    const bool n32 = p.nm == 32;
+    // per-channel (scale, zero + bias constant): immutable, read before the waits
+    const float2 sz0 = (WBITS == 16 || GROUPED) ? make_float2(1.f, 0.f) : p.sz[ng * kBN + rr0];
+    const float2 sz1 = (WBITS == 16 || GROUPED) ? make_float2(1.f, 0.f) : p.sz[ng * kBN + rr1];
+    const uint32_t wring_u = smem_u32(wring), xring_u = smem_u32(xring);
+    uint32_t off0[NCH], off1[NCH];
 #pragma unroll
-    for (int c = 0; c < NCH; ++c) woff[c] = c * 2048 + ((r ^ tile_swz(WBITS, c)) << 4);
+    for (int c = 0; c < NCH; ++c) {
+      off0[c] = c * 2048 + ((rr0 ^ tile_swz(WBITS, c)) << 4);
+      off1[c] = c * 2048 + ((rr1 ^ tile_swz(WBITS, c)) << 4);
+    }
+    // W4: the nibble of k pair 2t of a word; W8 / A8: which word of a 16-byte chunk, which half of it
+    const uint32_t sh4 = 4 * t4, sh8 = 8 * (t4 & 1), qsh = 16 * (t4 & 1), msel = (t4 & 1) ? 0xFBEAu : 0xD9C8u;
+    const int wa = t4 >> 1;
+    auto word = [](const uint4& v, int j) { return j == 0 ? v.x : (j == 1 ? v.y : (j == 2 ? v.z : v.w)); };
 
-    for (int st = (grp ^ gbase) & 1; st < nst; st += 2) {  // group = parity of the global stage index
+    // fp8 MMAs accumulate with less than fp32 precision on Hopper: A8 runs them into dt and adds dt to the fp32 accumulator
+    // d every 128 k (two weight tiles)
+    float d[32], dt[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) d[i] = dt[i] = 0.f;
+    int prev_xs = -1;
+    for (int st = 0; st < nst; ++st) {
       const int g = gbase + st;
-      const int slot = g % NSW, ab = g % NAB;
+      const int slot = g % NSW, xs = g % kTcNSX;
       // sub-channel weights: this stage's per-(group, channel) params are requested before the wait on the weights
-      uint32_t gs2[TPS], gc2[TPS];
+      uint32_t gs2[TPS][2], gc2[TPS][2];
       if (GROUPED && p.group_k == 0) {
 #pragma unroll
         for (int ti = 0; ti < TPS; ++ti) {
           const int kt = min(kt0 + st * TPS + ti, kt1 - 1);
-          const float2 z = __ldg(p.sz + (size_t)(kt / p.group_tiles) * p.Np + ng * kBN + r);  // (scale, zero + 16)
-          gs2[ti] = F::pack(z.x, z.x);
-          const float c = (F::kBias + 8.f - z.y) * z.x;                                        // (8 - zero) * scale
-          gc2[ti] = F::pack(c, c);
+          const float2 z0 = __ldg(p.sz + (size_t)(kt / p.group_tiles) * p.Np + ng * kBN + rr0);  // (scale, zero + 16)
+          const float2 z1 = __ldg(p.sz + (size_t)(kt / p.group_tiles) * p.Np + ng * kBN + rr1);
+          const float c0 = (F::kBias + 8.f - z0.y) * z0.x, c1 = (F::kBias + 8.f - z1.y) * z1.x;  // (8 - zero) * scale
+          if (DUAL) {  // rows r0 / r1 in the two halves of one register (80-register budget), split at use
+            gs2[ti][0] = F::pack(z0.x, z1.x);
+            gc2[ti][0] = F::pack(c0, c1);
+          } else {
+            gs2[ti][0] = F::pack(z0.x, z0.x); gs2[ti][1] = F::pack(z1.x, z1.x);
+            gc2[ti][0] = F::pack(c0, c0); gc2[ti][1] = F::pack(c1, c1);
+          }
         }
       }
       mbar_wait(&wfull[slot], (g / NSW) & 1);
-      if (tracer) TC_TRACE(4, g);
-      if (g >= NAB) {  // A buffer ab was last read by stage g - NAB, whose commit went to mdone[(g - NAB) % NSX]
-        const int ps = g - NAB;
-        mbar_wait(&mdone[ps % kTcNSX], (ps / kTcNSX) & 1);
-      }
-      tc_fence_after();
-      if (tracer) TC_TRACE(5, g);
-      const int tiles = TC_ABL(2) ? 0 : min(TPS, nt - st * TPS);
+      mbar_wait(&afull[xs], (g / kTcNSX) & 1);
+      const int tiles = min(TPS, nt - st * TPS);
 #pragma unroll
       for (int ti = 0; ti < TPS; ++ti) {
         if (ti < tiles) {
           const uint32_t wt = wring_u + slot * WSTAGE + ti * TILE_BYTES;
-          const uint32_t acol = trow + kTcColsA + ab * ABUF + ti * ACOLS;
-          if (A8) {
+          if (A8) {  // activation tile ti / 2 holds 128 k; this weight tile is its half ti & 1 = two K=32 steps
+            const uint64_t bd = wg_desc(xring_u + xs * XSTAGE + (ti >> 1) * kTcXTile) + (uint64_t)(4 * (ti & 1));
+            uint32_t a[2][4];
 #pragma unroll
             for (int c = 0; c < 2; ++c) {  // chunk c = 32 k = one K=32 step
-              const uint4 wv = lds128(wt + woff[c]);
-              uint32_t a[8];
-              nib8_to_e4m3(wv.x, a[0], a[1]);
-              nib8_to_e4m3(wv.y, a[2], a[3]);
-              nib8_to_e4m3(wv.z, a[4], a[5]);
-              nib8_to_e4m3(wv.w, a[6], a[7]);
-              tc_st8(acol + c * 8, a);
+              const uint4 v0 = lds128(wt + off0[c]), v1 = lds128(wt + off1[c]);
+              a[c][0] = nib4_to_e4m3(word(v0, wa), qsh, msel);
+              a[c][1] = nib4_to_e4m3(word(v1, wa), qsh, msel);
+              a[c][2] = nib4_to_e4m3(word(v0, 2 + wa), qsh, msel);
+              a[c][3] = nib4_to_e4m3(word(v1, 2 + wa), qsh, msel);
             }
-          } else if (WBITS == 4) {
+            wg_fence();
 #pragma unroll
-            for (int c = 0; c < 2; ++c) {
-              const uint4 wv = lds128(wt + woff[c]);
-              const uint32_t ww[4] = {wv.x, wv.y, wv.z, wv.w};
-#pragma unroll
-              for (int h = 0; h < 2; ++h) {  // k16 step kk = 2c + h: words 2h, 2h+1
-                uint32_t a[8];
-#pragma unroll
-                for (int jw = 0; jw < 2; ++jw) {
-                  const uint32_t w = ww[2 * h + jw];
-                  a[4 * jw + 0] = lop3_and_or(w, kMask4, F::kMagic);
-                  a[4 * jw + 1] = lop3_and_or(__funnelshift_r(w, w, 4), kMask4, F::kMagic);
-                  a[4 * jw + 2] = lop3_and_or(__funnelshift_r(w, w, 8), kMask4, F::kMagic);
-                  a[4 * jw + 3] = lop3_and_or(__funnelshift_r(w, w, 12), kMask4, F::kMagic);
-                }
-                if (GROUPED) {  // (16 + q) - 24 = q - 8 exactly, then one fused multiply-add: (q - 8) s + (8 - z) s
-                  uint32_t sw[2] = {gs2[ti], gs2[ti]}, cw[2] = {gc2[ti], gc2[ti]};
-                  if (p.group_k > 0) {  // word j = 2h + jw of chunk c holds k = 64 kt + 32 c + 8 j + (0..7): one group per word
-#pragma unroll
-                    for (int jw = 0; jw < 2; ++jw) {
-                      const int k0 = (kt0 + st * TPS + ti) * kBK + 32 * c + 8 * (2 * h + jw);
-                      const float2 z = __ldg(p.sz + (size_t)min(k0 / p.group_k, p.ngroups - 1) * p.Np + ng * kBN + r);
-                      sw[jw] = F::pack(z.x, z.x);
-                      const float cc = (F::kBias + 8.f - z.y) * z.x;
-                      cw[jw] = F::pack(cc, cc);
-                    }
-                  }
-#pragma unroll
-                  for (int e = 0; e < 8; ++e) {
-                    uint32_t t2;
-                    if (H) {  // (128 + q) - 136
-                      asm("add.rn.f16x2 %0, %1, %2;" : "=r"(t2) : "r"(a[e]), "r"(0xD840D840u));
-                      asm("fma.rn.f16x2 %0, %1, %2, %3;" : "=r"(a[e]) : "r"(t2), "r"(sw[e >> 2]), "r"(cw[e >> 2]));
-                    } else {
-                      asm("add.rn.bf16x2 %0, %1, %2;" : "=r"(t2) : "r"(a[e]), "r"(0xC1C0C1C0u));
-                      asm("fma.rn.bf16x2 %0, %1, %2, %3;" : "=r"(a[e]) : "r"(t2), "r"(sw[e >> 2]), "r"(cw[e >> 2]));
-                    }
-                  }
-                }
-                if (!TC_ABL(16)) tc_st8(acol + (2 * c + h) * 8, a);
-                else if (a[0] + a[3] + a[5] + a[7] == 0x12345u) tc_st8(acol, a);  // keep the ALU work alive
-              }
-            }
-          } else if (WBITS == 16) {  // bf16 weights: a plain copy, k16 step kk = chunks 2kk, 2kk+1
-#pragma unroll
-            for (int kk = 0; kk < 4; ++kk) {
-              const uint4 w0 = lds128(wt + woff[2 * kk]), w1 = lds128(wt + woff[2 * kk + 1]);
-              const uint32_t a[8] = {w0.x, w0.y, w0.z, w0.w, w1.x, w1.y, w1.z, w1.w};
-              tc_st8(acol + kk * 8, a);
-            }
+            for (int c = 0; c < 2; ++c) wg_mma<KIND>(dt, a[c], bd + (uint64_t)(2 * c), n32);
           } else {
+            const uint64_t bd = wg_desc(xring_u + xs * XSTAGE + ti * kTcXTile);
+            if (WBITS == 4) {
+              uint32_t a[4][4];
 #pragma unroll
-            for (int c = 0; c < 4; ++c) {  // chunk c = k16 step kk
-              const uint4 wv = lds128(wt + woff[c]);
-              const uint32_t ww[4] = {wv.x, wv.y, wv.z, wv.w};
-              uint32_t lo[8], hi[8];
+              for (int c = 0; c < 2; ++c) {
+                const uint4 v0 = lds128(wt + off0[c]), v1 = lds128(wt + off1[c]);
 #pragma unroll
-              for (int jw = 0; jw < 4; ++jw) {
-                const uint32_t w = ww[jw];
-                lo[2 * jw + 0] = lop3_and_or(w, kMask4, F::kMagic);
-                hi[2 * jw + 0] = lop3_and_or(__funnelshift_r(w, w, 4), kMask4, F::kMagicHi);
-                lo[2 * jw + 1] = lop3_and_or(__funnelshift_r(w, w, 8), kMask4, F::kMagic);
-                hi[2 * jw + 1] = lop3_and_or(__funnelshift_r(w, w, 12), kMask4, F::kMagicHi);
+                for (int h = 0; h < 2; ++h) {  // k16 step kk = 2c + h: words 2h (k pair 2t), 2h + 1 (k pair 2t + 8)
+                  uint32_t* f = a[2 * c + h];
+                  f[0] = lop3_and_or(__funnelshift_r(word(v0, 2 * h), word(v0, 2 * h), sh4), kMask4, F::kMagic);
+                  f[1] = lop3_and_or(__funnelshift_r(word(v1, 2 * h), word(v1, 2 * h), sh4), kMask4, F::kMagic);
+                  f[2] = lop3_and_or(__funnelshift_r(word(v0, 2 * h + 1), word(v0, 2 * h + 1), sh4), kMask4, F::kMagic);
+                  f[3] = lop3_and_or(__funnelshift_r(word(v1, 2 * h + 1), word(v1, 2 * h + 1), sh4), kMask4, F::kMagic);
+                  if (GROUPED) {  // (16 + q) - 24 = q - 8 exactly, then one fused multiply-add: (q - 8) s + (8 - z) s
+                    uint32_t sw[4], cw[4];  // per fragment register: rows r0, r1, r0, r1
+                    if (p.group_k > 0) {  // word j of chunk c holds k = 64 kt + 32 c + 8 j + (0..7): one group per word
+#pragma unroll
+                      for (int e = 0; e < 4; ++e) {
+                        const int k0 = (kt0 + st * TPS + ti) * kBK + 32 * c + 8 * (2 * h + (e >> 1));
+                        const float2 z = __ldg(p.sz + (size_t)min(k0 / p.group_k, p.ngroups - 1) * p.Np + ng * kBN + ((e & 1) ? rr1 : rr0));
+                        sw[e] = F::pack(z.x, z.x);
+                        const float cc = (F::kBias + 8.f - z.y) * z.x;
+                        cw[e] = F::pack(cc, cc);
+                      }
+                    } else {
+#pragma unroll
+                      for (int e = 0; e < 4; ++e) {
+                        if (DUAL) {
+                          sw[e] = __byte_perm(gs2[ti][0], 0, (e & 1) ? 0x3232 : 0x1010);
+                          cw[e] = __byte_perm(gc2[ti][0], 0, (e & 1) ? 0x3232 : 0x1010);
+                        } else {
+                          sw[e] = gs2[ti][e & 1]; cw[e] = gc2[ti][e & 1];
+                        }
+                      }
+                    }
+#pragma unroll
+                    for (int e = 0; e < 4; ++e) {
+                      uint32_t t2;
+                      if (H) {  // (128 + q) - 136
+                        asm("add.rn.f16x2 %0, %1, %2;" : "=r"(t2) : "r"(f[e]), "r"(0xD840D840u));
+                        asm("fma.rn.f16x2 %0, %1, %2, %3;" : "=r"(f[e]) : "r"(t2), "r"(sw[e]), "r"(cw[e]));
+                      } else {
+                        asm("add.rn.bf16x2 %0, %1, %2;" : "=r"(t2) : "r"(f[e]), "r"(0xC1C0C1C0u));
+                        asm("fma.rn.bf16x2 %0, %1, %2, %3;" : "=r"(f[e]) : "r"(t2), "r"(sw[e]), "r"(cw[e]));
+                      }
+                    }
+                  }
+                }
+                if (DUAL) {  // one commit group per 32-k chunk: half the fragment registers in flight (80-register budget)
+                  wg_fence();
+                  wg_mma<KIND>(d, a[2 * c], bd + (uint64_t)(4 * c), n32);
+                  wg_mma<KIND>(d, a[2 * c + 1], bd + (uint64_t)(4 * c + 2), n32);
+                  wg_commit();
+                  wg_wait<1>();
+                }
               }
-              tc_st8(acol + c * 16, lo);
-              tc_st8(acol + c * 16 + 8, hi);
+              if (!DUAL) {
+                wg_fence();
+#pragma unroll
+                for (int kk = 0; kk < 4; ++kk) wg_mma<KIND>(d, a[kk], bd + (uint64_t)(2 * kk), n32);
+              }
+            } else if (WBITS == 16) {  // bf16 weights: k16 step kk = chunks 2kk (k pair 2t), 2kk + 1 (k pair 2t + 8)
+              uint32_t a[4][4];
+#pragma unroll
+              for (int kk = 0; kk < 4; ++kk) {
+                a[kk][0] = lds32(wt + off0[2 * kk] + 4 * t4);
+                a[kk][1] = lds32(wt + off1[2 * kk] + 4 * t4);
+                a[kk][2] = lds32(wt + off0[2 * kk + 1] + 4 * t4);
+                a[kk][3] = lds32(wt + off1[2 * kk + 1] + 4 * t4);
+              }
+              wg_fence();
+#pragma unroll
+              for (int kk = 0; kk < 4; ++kk) wg_mma<KIND>(d, a[kk], bd + (uint64_t)(2 * kk), n32);
+            } else {  // W8: chunk c = k16 step c; the low and high nibble planes are two MMAs (16 + lo, 16 (16 + hi))
+              uint32_t lo[4][4], hi[4][4];
+#pragma unroll
+              for (int c = 0; c < 4; ++c) {
+                const uint4 v0 = lds128(wt + off0[c]), v1 = lds128(wt + off1[c]);
+                const uint32_t w[4] = {word(v0, wa), word(v1, wa), word(v0, 2 + wa), word(v1, 2 + wa)};
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                  lo[c][e] = lop3_and_or(__funnelshift_r(w[e], w[e], sh8), kMask4, F::kMagic);
+                  hi[c][e] = lop3_and_or(__funnelshift_r(w[e], w[e], sh8 + 4), kMask4, F::kMagicHi);
+                }
+              }
+              wg_fence();
+#pragma unroll
+              for (int c = 0; c < 4; ++c) {
+                wg_mma<KIND>(d, lo[c], bd + (uint64_t)(2 * c), n32);
+                wg_mma<KIND>(d, hi[c], bd + (uint64_t)(2 * c), n32);
+              }
             }
+          }
+          if (!DUAL) {  // (DUAL committed and waited per chunk above)
+            wg_commit();
+            wg_wait<1>();  // the previous tile's MMAs completed (their fragment registers and, at a stage start, X slot are free)
+          }
+          if (ti == 0 && prev_xs >= 0) {
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&xfree[prev_xs]);
+            prev_xs = -1;
+          }
+          if (A8 && ((ti & 1) || ti + 1 == tiles)) {
+            wg_wait<0>();
+            wg_fence_acc(dt);
+#pragma unroll
+            for (int i = 0; i < 32; ++i) { d[i] += dt[i]; dt[i] = 0.f; }
           }
         }
       }
-      tc_wait_st();
-      tc_fence_before();
       __syncwarp();
-      if (tracer) TC_TRACE(6, g);
-      if (lane == 0) {
-        mbar_arrive(&wfree[slot]);
-        mbar_arrive(&afull[ab]);
-      }
+      if (lane == 0) mbar_arrive(&wfree[slot]);  // the weights are in registers: the smem stage is free
+      prev_xs = xs;
     }
+    wg_wait<0>();
+    wg_fence_acc(d);
+    __syncwarp();
+    if (prev_xs >= 0 && lane == 0) mbar_arrive(&xfree[prev_xs]);
 
-    // ---------------- accumulators -> fp32 tile in shared memory (group g takes batch rows [32g, 32g + 32)) ----------------
-    mbar_wait(dfull, uit & 1);
-    if (tracer) TC_TRACE(7, 0);
-    tc_fence_after();
-    asm volatile("bar.sync 3, 320;" ::: "memory");  // row sums ready
-    if (grp * 32 < p.M) {
-      uint32_t d[32];
-      tc_ld32(trow + kTcColsD + grp * 32, d);
-      tc_wait_ld();
-      if (tracer) TC_TRACE(7, 7);
-      // [m][128 n] fp32, over the drained activation ring (all of this unit's MMAs have completed once dfull fired; the
-      // weight ring is already receiving the next unit's first stages)
-      float* fsw = reinterpret_cast<float*>(xring) + (grp * 32) * kBN + r;
-      const float* sm = suma + grp * 32;
-      if (A8) {  // plain codes (no +16 bias in the fp8 operand) and the token's activation scale
-        const float zz = sz.y - 16.f;
-        const float* as = ascale + grp * 32;
+    // ---------------- accumulators -> fp32 tile in shared memory: [m][128 n] over the drained activation ring ----------------
+    asm volatile("bar.sync 3, 320;" ::: "memory");  // row sums ready; every MMA of both warpgroups has completed
+    float* fs = reinterpret_cast<float*>(xring);
 #pragma unroll
-        for (int m4 = 0; m4 < 32; m4 += 4) {
-          const float4 sa = *reinterpret_cast<const float4*>(sm + m4);
-          const float4 sc = *reinterpret_cast<const float4*>(as + m4);
-          fsw[(m4 + 0) * kBN] = sz.x * sc.x * (__uint_as_float(d[m4 + 0]) - zz * sa.x);
-          fsw[(m4 + 1) * kBN] = sz.x * sc.y * (__uint_as_float(d[m4 + 1]) - zz * sa.y);
-          fsw[(m4 + 2) * kBN] = sz.x * sc.z * (__uint_as_float(d[m4 + 2]) - zz * sa.z);
-          fsw[(m4 + 3) * kBN] = sz.x * sc.w * (__uint_as_float(d[m4 + 3]) - zz * sa.w);
-        }
-      } else if (p.norm_sumsq) {  // rows scaled by 1/rms (the activations were bf16(x * gamma))
-        const float* as = ascale + grp * 32;
-#pragma unroll
-        for (int m4 = 0; m4 < 32; m4 += 4) {
-          const float4 sa = *reinterpret_cast<const float4*>(sm + m4);
-          const float4 sc = *reinterpret_cast<const float4*>(as + m4);
-          fsw[(m4 + 0) * kBN] = sz.x * sc.x * (__uint_as_float(d[m4 + 0]) - sz.y * sa.x);
-          fsw[(m4 + 1) * kBN] = sz.x * sc.y * (__uint_as_float(d[m4 + 1]) - sz.y * sa.y);
-          fsw[(m4 + 2) * kBN] = sz.x * sc.z * (__uint_as_float(d[m4 + 2]) - sz.y * sa.z);
-          fsw[(m4 + 3) * kBN] = sz.x * sc.w * (__uint_as_float(d[m4 + 3]) - sz.y * sa.w);
-        }
-      } else {
-#pragma unroll
-      for (int m4 = 0; m4 < 32; m4 += 4) {
-        const float4 sa = *reinterpret_cast<const float4*>(sm + m4);
-        fsw[(m4 + 0) * kBN] = sz.x * (__uint_as_float(d[m4 + 0]) - sz.y * sa.x);
-        fsw[(m4 + 1) * kBN] = sz.x * (__uint_as_float(d[m4 + 1]) - sz.y * sa.y);
-        fsw[(m4 + 2) * kBN] = sz.x * (__uint_as_float(d[m4 + 2]) - sz.y * sa.z);
-        fsw[(m4 + 3) * kBN] = sz.x * (__uint_as_float(d[m4 + 3]) - sz.y * sa.w);
-      }
-      }
+    for (int j = 0; j < 8; ++j) {  // n8 block j of the accumulator: batch rows m = 8j + 2t (+1), channels rr0 / rr1
+      const int m = 8 * j + 2 * t4;
+      float s0 = 1.f, s1 = 1.f;
+      if (A8 || p.norm_sumsq) { s0 = ascale[m]; s1 = ascale[m + 1]; }
+      const float zz0 = A8 ? sz0.y - 16.f : sz0.y, zz1 = A8 ? sz1.y - 16.f : sz1.y;
+      const float sa0 = suma[m], sa1 = suma[m + 1];
+      fs[m * kBN + rr0] = sz0.x * s0 * (d[4 * j + 0] - zz0 * sa0);
+      fs[(m + 1) * kBN + rr0] = sz0.x * s1 * (d[4 * j + 1] - zz0 * sa1);
+      fs[m * kBN + rr1] = sz1.x * s0 * (d[4 * j + 2] - zz1 * sa0);
+      fs[(m + 1) * kBN + rr1] = sz1.x * s1 * (d[4 * j + 3] - zz1 * sa1);
     }
   }
 
   // ======================= epilogue: all threads =======================
   pdl_wait();  // workspace / counters / C belong to the previous kernels until here
-  tc_fence_before();
   __syncthreads();  // tile parked
-  if (tid == 64) TC_TRACE(7, 1);
   {
     constexpr int T = kTcThreads;
     const float4* fs4 = reinterpret_cast<const float4*>(xring);
@@ -667,7 +576,6 @@ __global__ void __launch_bounds__(kTcThreads, DUAL ? 2 : 1) wq_gemm_tc_kernel(co
         __syncthreads();
       }
     }
-    if (tid == 64) TC_TRACE(7, 2);
     if (finalize) {
       const bool vec_ok = (p.ldc & 3) == 0 && (reinterpret_cast<uintptr_t>(p.C) & 7) == 0;
       if (p.act == B2_ACT_SWIGLU) {
@@ -697,7 +605,7 @@ __global__ void __launch_bounds__(kTcThreads, DUAL ? 2 : 1) wq_gemm_tc_kernel(co
                  (!p.residual || (reinterpret_cast<uintptr_t>(p.residual) & 7) == 0) &&
                  (!p.bias || (reinterpret_cast<uintptr_t>(p.bias) & 7) == 0)) {
         // the decode-path case: no activation; all residual loads of a thread are issued before the first use
-        constexpr int UPT = (kTcNM * (kBN / 4) + T - 1) / T;  // units per thread (5)
+        constexpr int UPT = (kTcNM * (kBN / 4) + T - 1) / T;  // units per thread (6)
         uint2 res[UPT];
 #pragma unroll
         for (int j = 0; j < UPT; ++j) {
@@ -729,7 +637,7 @@ __global__ void __launch_bounds__(kTcThreads, DUAL ? 2 : 1) wq_gemm_tc_kernel(co
               ssq = (r0 * r0 + r1 * r1) + (r2 * r2 + r3 * r3);
             }
           }
-          if (p.xg_out) {  // a warp holds the 32 four-column units of one row (416 = 13 x 32): fixed-order lane reduction
+          if (p.xg_out) {  // a warp holds the 32 four-column units of one row (384 = 12 x 32): fixed-order lane reduction
 #pragma unroll
             for (int o = 16; o > 0; o >>= 1) ssq += __shfl_xor_sync(0xffffffffu, ssq, o);
             if (lane == 0 && i < units) p.sumsq_out[(size_t)ng * p.norm_ld + m] = ssq;
@@ -768,35 +676,16 @@ __global__ void __launch_bounds__(kTcThreads, DUAL ? 2 : 1) wq_gemm_tc_kernel(co
     }
   }
 
-  tc_fence_before();
   if (MULTI) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy tile writes before the next unit's TMA writes
-  __syncthreads();  // the tile in the X ring and the accumulator are free again
-  tc_fence_after();
+  __syncthreads();  // the tile in the X ring is free again
   }  // unit loop
-
-  if (tid == 0) { TC_TRACE(7, 3); TC_GT(2); }
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(TMEM_COLS) : "memory");
-  }
 }
-
-#ifdef B2_TC_TRACE
-static unsigned g_tc_host_launches = 0;
-extern "C" int b2_debug_tc_trace(unsigned long long* host_out) {
-  return (int)cudaMemcpyFromSymbol(host_out, g_tc_trace, sizeof(g_tc_trace));
-}
-extern "C" int b2_debug_tc_gt(unsigned long long* host_out, unsigned* launches) {
-  *launches = g_tc_host_launches;
-  return (int)cudaMemcpyFromSymbol(host_out, g_tc_gt, sizeof(g_tc_gt));
-}
-#endif
 
 int tc_smem_bytes(int wbits, bool dual) {
   const int tps = wbits == 4 ? (dual ? 2 : 4) : 2;
   const int wstage = tps * (wbits == 4 ? 4096 : (wbits == 8 ? 8192 : 16384));
   const int nsw = wbits == 16 ? 4 : kTcNSW;
-  return 1024 + kTcNSX * tps * kTcXTile + nsw * wstage + kTcNM * 4 + 96 * 8 + 64;  // barrier block: 25 barriers, TMEM slot, 64 scales
+  return 1024 + kTcNSX * tps * kTcXTile + nsw * wstage + kTcNM * 4 + 96 * 8 + 64;  // barrier block: 21 barriers, 64 scales
 }
 
 cudaError_t tc_configure(int wbits) {
@@ -865,13 +754,6 @@ cudaError_t tc_launch(int wbits, const TcLaunch& a, cudaStream_t stream) {
   p.norm_sumsq = a.norm_sumsq; p.norm_parts = a.norm_parts; p.norm_ld = a.norm_ld; p.norm_inv_hidden = a.norm_inv_hidden;
   p.norm_eps = a.norm_eps; p.sumsq_out = a.sumsq_out; p.xg_out = a.xg_out; p.gamma_out = a.gamma_out; p.ldxg = a.ldxg;
   p.nm = nm; p.group_tiles = a.group_tiles; p.group_k = a.group_k; p.ngroups = a.ngroups;
-  p.dbg = 0;
-#ifdef B2_TC_ABLATE
-  if (const char* e = getenv("B2_TC_ABLATE")) p.dbg = atoi(e);
-#endif
-#ifdef B2_TC_TRACE
-  p.dbg = (int)(g_tc_host_launches++);  // launch id (frozen into a captured graph node)
-#endif
   // persistent: one CTA per SM walks the (n-group, k-split) units; B2_GEMM_TC_PERSIST=0 launches one CTA per unit
   static const int persist = [] { const char* e = getenv("B2_GEMM_TC_PERSIST"); return e ? atoi(e) : 1; }();
   const int units = a.NG * a.S;

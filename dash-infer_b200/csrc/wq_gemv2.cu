@@ -1,10 +1,9 @@
 // b200spark — weight-only quantized GEMV/GEMM for decode batches 1..16 (per-channel and sub-channel) WITHOUT global split-K,
-// sm_100a.  Same weight image, same tensor-core math and the same results (up to fp32 summation order) as wq_gemm.cu.
+// sm_90a.  Same weight image, same tensor-core math and the same results (up to fp32 summation order) as wq_gemm.cu.
 //
-// Why a second decomposition (timeline of the split-K kernel at batch 1, Qwen2-7B qkv, profiles/r2_timelines.md): of the
-// 5.2 us between "previous kernel finished" and "output stored", the weight stream is 0.8 us; 3.2 us are the split-K
-// tail — partials to the workspace, __threadfence, atomic ticket, waiting for the 15 sibling CTAs, re-reading 16 partial
-// tiles from L2.  A 16-way K split across CTAs is what it takes to fill 148 SMs with 128-channel tiles of a 4608-channel
+// Why a second decomposition: at batch 1 most of the split-K kernel's time after the weight stream is its split-K tail —
+// partials to the workspace, __threadfence, atomic ticket, waiting for the sibling CTAs, re-reading the partial tiles from
+// L2.  A 16-way K split across CTAs is what it takes to fill 132 SMs with 128-channel tiles of a 4608-channel
 // projection, so the split has to move INSIDE the CTA:
 //
 //   * a CTA owns CB in {128, 64, 32, 16} output channels of one 128-channel n-group and the FULL K range;
@@ -360,9 +359,9 @@ static int v2_env(const char* name, int dflt) {
 // Channels per CTA: the largest of 128/64/32/16 whose grid still covers the SMs ~twice (more CTAs = more independent TMA
 // rings = more bytes in flight per SM); a pair image needs >= 32 (16 gate + 16 up rows per CTA).
 bool gemv2_plan(const Gemv2Launch& a, Gemv2Plan* pl) {
-  // Measured on B200 (profiles/r2_gemv2.md): with the 128-row tile image a CTA that owns fewer than 128 channels reads
-  // 256..1024-byte row runs at a 2 KB stride and eight CTAs revisit every DRAM page — int4 down_proj drops to 0.13 of HBM
-  // (split-K kernel: 0.36) — while 128-channel blocks of dense bf16 weights (lm_head) reach 0.996 (split-K kernel: 0.94).
+  // With the 128-row tile image a CTA that owns fewer than 128 channels reads 256..1024-byte row runs at a 2 KB stride and
+  // eight CTAs revisit every DRAM page, which starves quantized shapes; 128-channel blocks of dense bf16 weights (lm_head)
+  // stream whole tiles.
   // Default policy (B2_GEMV2=1): dense bf16 weights only; B2_GEMV2=2 takes every shape (tests), 0 none.
   const int mode = v2_env("B2_GEMV2", 1);
   if (mode == 0 || (mode == 1 && a.wbits != 16)) return false;

@@ -1,4 +1,4 @@
-"""b200spark — B200-native quantized decode hot path behind DashInfer's operator API (Python front end).
+"""b200spark — H100-native quantized decode hot path behind DashInfer's operator API (Python front end).
 
 The native library is mandatory: importing this package without `dash-infer_b200/lib/libb200spark.so`
 raises ImportError (no CPU / eager-PyTorch fallback exists on the product path).

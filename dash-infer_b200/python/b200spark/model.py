@@ -137,7 +137,7 @@ class DecodeStack:
         # batches <= 16, else it degrades to "b2"), "b2" = GEMM + b2_allreduce (one-shot over NVLink peer memory, residual
         # fused), "nccl" = torch.distributed all_reduce + copy (the baseline the reference's AllReduceOp amounts to)
         import os
-        self.collective = collective or os.environ.get("B2_TP_COLLECTIVE", "b2")  # measured on 2xB200: b2 946, fused 897 tok/s
+        self.collective = collective or os.environ.get("B2_TP_COLLECTIVE", "b2")
         self.comm = comm
         self.fuse_swiglu = fuse_swiglu
         self.group_size, self.wbits = group, wbits
@@ -202,20 +202,19 @@ class DecodeStack:
         self.set_batch(batch)
         # RMSNorm fusion (decode batches <= 16, TP = 1): the row-parallel GEMVs emit per-tile sums of squares, their
         # consumers normalise while staging activations; only layer 0's first norm stays a stand-alone kernel.
-        # Off by default: measured on B200 it removes 2 launches/layer but lengthens every GEMV's dependent chain
-        # (statistics load + barrier before staging) and loses ~4% at B=1 (438 vs 454 tok/s) — kept for the next round.
+        # Off by default: it removes 2 launches/layer but lengthens every GEMV's dependent chain (statistics load + barrier
+        # before staging).
         self.fuse_norm = fuse_norm and tp == 1 and batch <= 16
         if self.fuse_norm:
             self.ssq_o = torch.zeros(self.layers[0]["o"].op.sumsq_parts(), batch, dtype=torch.float32, device=device)
             self.ssq_d = torch.zeros(self.layers[0]["down"].op.sumsq_parts(), batch, dtype=torch.float32, device=device)
         # Self-contained RMSNorm fusion (any TP): the column-parallel GEMVs (qkv, gate/up) stage bf16(x * gamma), collect
         # sum x^2 in the same pass and scale their reduced tile by 1/rms — two launches per layer disappear.  Every CTA
-        # repeats the normalisation of its k-slice of every live row, so the saving shrinks with the batch: measured on
-        # B200 (Qwen2-7B int4, whole step) batch 1: 445 -> 462 tok/s, batch 8: 3241 -> 3140.  Default: batches <= 2.
+        # repeats the normalisation of its k-slice of every live row, so the saving shrinks with the batch.  Default: batches <= 2.
         self.norm_self = (os.environ.get("B2_NORM_SELF", "1") != "0" and not self.fuse_norm
-                          and (group == -1 or group % 64 == 0))  # other group sizes run on the tcgen05 kernel at every batch
+                          and (group == -1 or group % 64 == 0))  # other group sizes run on the wgmma kernel at every batch
         self.norm_self_max_b = int(os.environ.get("B2_NORM_SELF_MAX_B", "2"))
-        # RMSNorm hand-off between the tcgen05 GEMMs (batches >= 17, TP = 1): o_proj / down_proj also write the next
+        # RMSNorm hand-off between the wgmma GEMMs (batches >= 17, TP = 1): o_proj / down_proj also write the next
         # norm's input scaled by its gamma plus per-tile row statistics; qkv / gate+up / lm_head scale their result rows by
         # 1/rms.  Only layer 0's first norm stays a stand-alone kernel (2 launches per layer fewer).
         self.norm_handoff = (os.environ.get("B2_NORM_HANDOFF", "1") != "0" and tp == 1 and not self.fuse_norm
@@ -368,7 +367,7 @@ class DecodeStack:
             ops.argmax_merge(self.all_val, self.all_ids, out=self.next_ids); n += 1  # lowest rank on ties == lowest vocab id
         ops.lens_add(self.lens_old, 1); n += 1
         ops.lens_add(self.lens_new, 1); n += 1
-        # rows per launch above batch 16: 64 on the tcgen05 path (per-channel int4/int8, bf16 lm_head), 16 for sub-channel
+        # rows per launch above batch 16: 64 on the wgmma path (per-channel int4/int8, bf16 lm_head), 16 for sub-channel
         # weights (mma.sync path); below, one launch takes the whole batch
         hchunks = (self.B + 63) // 64 if self.B > 16 else 1
         qchunks = ((self.B + 15) // 16 if (self.group_size != -1 and self.wbits != 4) else hchunks) if self.B > 16 else 1

@@ -117,7 +117,7 @@ class GemmWQ:
         return out
 
     def run_fp8(self, q8, ws, out=None, act=ACT_NONE, alpha=1.0, residual=None):
-        """fp8-e4m3 activations (a Fp8Act from quant_fp8) x int4 per-channel weights on tcgen05 kind::f8f6f4."""
+        """fp8-e4m3 activations (a Fp8Act from quant_fp8) x int4 per-channel weights on the e4m3 wgmma kernel."""
         if self.pair:
             act = _lib.ACT_SWIGLU
         M = q8.y.shape[0]

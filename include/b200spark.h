@@ -1,5 +1,5 @@
 /*
- * b200spark C ABI — the drop-in boundary for DashInfer's quantized decode hot path on B200 (sm_100a).
+ * b200spark C ABI — the drop-in boundary for DashInfer's quantized decode hot path on H100 (sm_90a).
  *
  * Everything here is `extern "C"`, takes plain pointers / sizes / POD structs and returns an `int`
  * status (b2_status); nothing throws, nothing synchronises the device, every call is ordered on the
@@ -51,7 +51,7 @@ typedef enum {
 const char* b2_status_string(int status);
 /* Last CUDA error text recorded by a failing call on this thread (empty string if none). */
 const char* b2_last_error(void);
-/* "b200spark <ver> sm_100a" */
+/* "b200spark <ver> sm_90a" */
 const char* b2_version(void);
 
 /* ---- allspark.proto wire enums (csrc/proto/allspark.proto:35-76) ---- */
@@ -131,7 +131,7 @@ typedef struct {
   float norm_eps;
   int32_t reserved;
   float* sumsq_out;        /* [b2_gemm_wq_sumsq_parts(handle)][M] or NULL */
-  /* Batches >= 17 (tcgen05 path): the hand-off form.  The producer (o_proj / down_proj with residual) writes, besides C and
+  /* Batches >= 17 (wgmma path): the hand-off form.  The producer (o_proj / down_proj with residual) writes, besides C and
    * sumsq_out, xg_out[m, n] = FT(C[m, n] * gamma_out[n]) — the next RMSNorm's input already scaled by its gamma; the consumer
    * is called with A = xg, norm_sumsq = the producer's sumsq_out, norm_gamma = NULL, and multiplies its fp32 result rows by
    * rsqrt(sum_p norm_sumsq[p][m] / norm_hidden + eps) (the factor is linear in the row).  Two RMSNorm launches per layer
@@ -145,7 +145,7 @@ int b2_gemm_wq_run_fused(b2_gemm_wq_t handle, const void* A, int64_t lda, void* 
                          const void* bias, const void* residual, int activation, float alpha,
                          void* workspace, size_t workspace_bytes, const b2_gemm_fuse* fuse, void* stream);
 /* FP8 activations ("next" row f3; BASELINE config "GPTQ-int4, fp8 activations"): fp8-e4m3 activations x int4 weights on
- * the tcgen05 tensor cores (kind::f8f6f4, K = 32 per MMA).  Beyond the reference (its FP8 operator is per-tensor A8W8 through
+ * the Hopper warpgroup tensor cores (e4m3 wgmma, K = 32 per MMA).  Beyond the reference (its FP8 operator is per-tensor A8W8 through
  * cuBLASLt, csrc/core/operator/general/gemm_lowp/gemm_fp8_a8w8_gpu.cpp:325-395), so the accuracy contract is its own:
  *   C[m,n] = act(alpha * scale_a[m] * s_n * (sum_k a8[m,k] q[k,n] - z_n sum_k a8[m,k]) + bias) (+ residual)
  * exact products (e4m3 x e4m3) and fp32 accumulation: the only loss is the activation quantization itself.

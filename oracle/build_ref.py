@@ -1,9 +1,9 @@
 """Build oracle/_ref/libdashinfer_ref.so — the UNMODIFIED reference GPU code for the KV-cache half of the hot path,
-compiled from the sources where they lie under /root/reference (nothing is copied into the repo).
+compiled from the reference checkout named by B2_REFERENCE (nothing is copied into the repo).
 
-TEST INFRASTRUCTURE: only tests/ and __graft_entry__.build() use this.  The output is git-ignored, but it travels to
-the GPU box with the gpurun snapshot (it is NOT in .gpurunignore), where tests/test_ref_pin_gpu.py uses it to pin
-oracle/kvcache_ref.py and the b200spark kernels to the reference's own results.
+TEST INFRASTRUCTURE: only __graft_entry__.build() and tests/golden/make_ref_pin.py use this.  The output is git-ignored;
+make_ref_pin.py runs it on a GPU and stores its results in tests/golden/ref_pin.npz, against which
+tests/test_ref_pin_gpu.py pins oracle/kvcache_ref.py and the b200spark kernels.
 
 What is compiled (nvcc directly, no cmake; -DNDEBUG like the reference's Release build):
   * span-attention/src/**/*.cu|*.cpp          the span-attention library (span::CreateHandle/Run ...), header-only
@@ -12,7 +12,7 @@ What is compiled (nvcc directly, no cmake; -DNDEBUG like the reference's Release
                                               with three stub headers from oracle/ref_stubs/ standing in for engine
                                               headers that need glog/protobuf/cublas (no kernel code in the stubs)
   * oracle/ref_shim.cu                        extern "C" entry points for ctypes
-Target: sm_100 (plain, the reference has no Blackwell-specific code; its mma.sync kernels run as they are).
+Target: sm_90 (plain, the reference has no Hopper-specific code; its mma.sync kernels run as they are).
 
 The CPU x86 path of the reference cannot be built at all (oneDNN/MKL tarballs are git-LFS stubs) — DESIGN.md §4.
 """
@@ -56,7 +56,7 @@ def build(force=False, verbose=False):
            "-I", os.path.join(sa, "thirdparty", "cutlass", "include"),
            "-I", os.path.join(REF, "csrc", "common"), "-I", os.path.join(REF, "csrc", "core", "kernel"),
            "-I", os.path.join(REF, "csrc", "device"), "-I", os.path.join(REF, "csrc")]        # <cuda/cudabfloat16_impl.hpp>
-    flags = ["-gencode", "arch=compute_100,code=sm_100", "-std=c++17", "-O2", "-DNDEBUG", "-DENABLE_BF16", "-DENABLE_FP16",
+    flags = ["-gencode", "arch=compute_90,code=sm_90", "-std=c++17", "-O2", "-DNDEBUG", "-DENABLE_BF16", "-DENABLE_FP16",
              "-DENABLE_CUDA", "--expt-relaxed-constexpr", "--extended-lambda", "--use_fast_math", "-Xcompiler", "-fPIC",
              "-x", "cu", "-w"]
 
@@ -75,7 +75,7 @@ def build(force=False, verbose=False):
 
     with ThreadPoolExecutor(max_workers=int(os.environ.get("B2_REF_JOBS", "8"))) as ex:
         objs = list(ex.map(one, srcs))
-    r = subprocess.run([NVCC, "-gencode", "arch=compute_100,code=sm_100", "-shared", "-o", SO] + objs,
+    r = subprocess.run([NVCC, "-gencode", "arch=compute_90,code=sm_90", "-shared", "-o", SO] + objs,
                        stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:
         sys.stdout.write(r.stdout)

@@ -4,7 +4,7 @@
 // /root/reference (span-attention/src + csrc/core/kernel/cuda/cache): the span-attention library
 // (span::CreateHandle / Run, span-attention/include/spanattn/span_attn.h:108-175) and the cache writers
 // (DecoderCacheAppendLauncher, ContextSpanCopyLauncher, csrc/core/kernel/cuda/cuda_kernel_span_cache.h:11-27).
-// tests/ use it on the GPU box to pin oracle/kvcache_ref.py and the b200spark kernels against what the reference
+// tests/golden/make_ref_pin.py uses it on a GPU to pin oracle/kvcache_ref.py and the b200spark kernels against what the reference
 // itself computes (append bytes, quant params, attention output).
 #include <cuda_runtime.h>
 #include <span_attn.h>
@@ -103,5 +103,5 @@ int ref_context_span_copy(void* const* spans, const void* src, int n_groups, int
   return 3;
 }
 
-const char* ref_version(void) { return "dash-infer f3cca8e span-attention + cache kernels, built for sm_100 by oracle/build_ref.py"; }
+const char* ref_version(void) { return "dash-infer f3cca8e span-attention + cache kernels, built for sm_90 by oracle/build_ref.py"; }
 }

@@ -9,7 +9,7 @@ sys.path.insert(0, os.path.join(ROOT, "dash-infer_b200", "python"))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100; select with -m gpu)")
 
 
 @pytest.fixture(scope="session")

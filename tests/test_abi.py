@@ -26,7 +26,7 @@ def test_status_strings_and_version():
     from b200spark import lib
     assert lib.b2_status_string(0) == b"B2_OK"
     assert lib.b2_status_string(3) == b"B2_ERR_PARAM"
-    assert b"sm_100a" in lib.b2_version()
+    assert b"sm_90a" in lib.b2_version()
 
 
 def test_param_validation_without_gpu():

@@ -1,4 +1,4 @@
-"""GPU: fp8-e4m3 activations x int4 weights on tcgen05 kind::f8f6f4 (SURVEY.md §8 f3; BASELINE config "GPTQ-int4, fp8
+"""GPU: fp8-e4m3 activations x int4 weights on the e4m3 wgmma kernel (SURVEY.md §8 f3; BASELINE config "GPTQ-int4, fp8
 activations").  Beyond the reference (its FP8 op is per-tensor A8W8 via cuBLASLt, gemm_fp8_a8w8_gpu.cpp:325-395), so the
 contract is stated here:
   * b2_quant_fp8 is checked bit for bit against a torch restatement (per-token scale = amax / 448, round-to-nearest-even e4m3);

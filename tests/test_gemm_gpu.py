@@ -107,7 +107,7 @@ def test_qwen2_7b_w8_and_g128():
 
 
 def test_dense_bf16_tcgen05_multiwave():
-    """bf16 weights on the tcgen05 path (lm_head shape class): more n-groups than SMs, ragged N tail, M 17..64."""
+    """bf16 weights on the wgmma path (lm_head shape class): more n-groups than SMs, ragged N tail, M 17..64."""
     _run(16, 3584, 19000, 64, -1, seed=71)
     _run(16, 1024, 4100, 23, -1, seed=72, use_bias=True, act=5)
 
@@ -296,7 +296,7 @@ def test_tcgen05_rmsnorm_handoff(wbits, group, M):
 @pytest.mark.parametrize("M", [1, 3, 8, 16, 17, 31, 33, 64])
 @pytest.mark.parametrize("wbits,group", [(4, -1), (8, -1), (16, -1), (4, 128), (8, 64)])
 def test_fp16_all_paths(wbits, group, M):
-    """split-K GEMV (M <= 16), tcgen05 (M >= 17; sub-channel int8 stays on the mma.sync kernel), odd N, bias + residual"""
+    """split-K GEMV (M <= 16), wgmma (M >= 17; sub-channel int8 stays on the mma.sync kernel), odd N, bias + residual"""
     _run(wbits, 1024, 1023, M, group, use_bias=True, use_res=True, seed=wbits + M, ft=torch.float16)
 
 
@@ -335,9 +335,17 @@ def test_fp16_swiglu_pair(wbits, group, M):
 @pytest.mark.parametrize("group,K,M", [(32, 1024, 1), (40, 1000, 5), (72, 2048, 16), (200, 1000, 33), (136, 4096, 100), (96, 3584, 64)])
 def test_general_group_sizes_w4(group, K, M, ft):
     """Group sizes that do not divide the 64-k tile (the reference's dequantize + cuBLAS test draws any multiple of 8 in
-    [64, 512]: operator_gemm_lowp_test.cpp:893-903; gemm_a16w4.cpp:57-63 accepts >= 32): int4, on the tcgen05 kernel at
+    [64, 512]: operator_gemm_lowp_test.cpp:893-903; gemm_a16w4.cpp:57-63 accepts >= 32): int4, on the wgmma kernel at
     every batch, the (scale, zero) looked up per 8-k word of the weight image."""
     _run(4, K, 1023, M, group, use_bias=True, use_res=(M > 16), seed=group + M, ft=ft)
+
+
+@pytest.mark.parametrize("group,ft", [(-1, torch.bfloat16), (128, torch.bfloat16), (96, torch.bfloat16), (128, torch.float16)])
+def test_wgmma_two_ctas_per_sm_persistent(group, ft):
+    """More than 2 x (SM count) n-groups: the int4 GEMM of batches >= 17 runs two CTAs per SM, each walking several
+    (n-group, k-split) units — per-channel, sub-channel, a group size that does not divide the 64-k tile, bf16 and fp16."""
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    _run(4, 512, (2 * sms + 6) * 128, 40, group, use_res=True, seed=17, ft=ft)
 
 
 @pytest.mark.parametrize("wbits,group,M,N", [(4, -1, 1, 5117), (4, -1, 7, 5120), (8, -1, 16, 5117), (4, 128, 9, 5118), (16, -1, 3, 5117)])
@@ -407,7 +415,7 @@ def test_self_contained_rmsnorm(wbits, group, M, K, N, pair):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# The launches bench.py actually times (VERDICT r1: "the bench runs it unchecked"): tcgen05 path at M in {17, 32, 64}
+# The launches bench.py actually times (VERDICT r1: "the bench runs it unchecked"): wgmma path at M in {17, 32, 64}
 # on every Qwen2-7B projection shape, int4 and int8, plus the fused gate/up pair and the Qwen2-72B TP=8 shard shapes.
 # ---------------------------------------------------------------------------------------------------------------------
 QWEN7B = [(3584, 4608), (3584, 3584), (3584, 18944), (18944, 3584)]

@@ -117,7 +117,7 @@ def test_glue_ops():
 def test_full_width_qwen2_7b_layer_and_lm_head(B):
     """VERDICT r1 2(ii): model-level parity was only checked on the 512-wide TINY config.  ONE full-width Qwen2-7B layer
     (hidden 3584, 28/4 heads, inter 18944, int4 per-channel — exactly the launches bench.py times at this batch: the
-    mma.sync GEMV family at B=1, the tcgen05 family + persistent gate/up pair at B=64) + final norm + the 152064-wide bf16
+    mma.sync GEMV family at B=1, the wgmma family + persistent gate/up pair at B=64) + final norm + the 152064-wide bf16
     lm_head + argmax, three decode steps from an empty cache, against the reference-CPU-path oracle."""
     from b200spark import model
     steps = 3
@@ -191,7 +191,7 @@ def test_config_c0_qwen2_0p5b_bf16_decode_parity():
 @pytest.mark.parametrize("wbits,group,kv,B", [(4, -1, "none", 2), (8, -1, "i8", 2), (4, 128, "u4", 3), (4, -1, "none", 20)])
 def test_tiny_decoder_fp16(wbits, group, kv, B):
     """The whole decode step in fp16 (activations, scales, unquantized cache, logits) against the oracle rounding to fp16
-    at the same points: split-K GEMV (B <= 16) and the tcgen05 GEMMs with the RMSNorm hand-off (B = 20), eager then a
+    at the same points: split-K GEMV (B <= 16) and the wgmma GEMMs with the RMSNorm hand-off (B = 20), eager then a
     captured graph."""
     from b200spark import model
     steps = 5
