@@ -855,7 +855,7 @@ struct b2_gemm_wq {
   float2* sz = nullptr;
   bool own_sz = false;
   unsigned* counters = nullptr;
-  Plan plans[3];  // MT = 1, 2, 4
+  Plan plans[2];  // MT = 1, 2
   int tc_S = 0;   // split-K of the wgmma path (0 = not planned)
   int tc_S2 = 0;  // same for the two-CTAs-per-SM variant (int4, bf16 activations)
   bool pair = false;  // gate/up pair image (SwiGLU epilogue): physical channels = 2 * N
@@ -868,8 +868,7 @@ template <int WBITS, bool GROUPED, bool H>
 static gemm_kernel_t pick_mt(int mt) {
   switch (mt) {
     case 1: return wq_gemm_kernel<WBITS, 1, GROUPED, H>;
-    case 2: return wq_gemm_kernel<WBITS, 2, GROUPED, H>;
-    default: return wq_gemm_kernel<WBITS, 4, GROUPED, H>;
+    default: return wq_gemm_kernel<WBITS, 2, GROUPED, H>;
   }
 }
 template <bool H>
@@ -889,12 +888,9 @@ static int env_int(const char* name, int dflt) {
   return v ? atoi(v) : dflt;
 }
 
-// The kernel instantiation is shared by every handle with the same (wbits, grouped, MT) while the shared-memory need
-// depends on the handle's group size: the opt-in limit is only ever raised (a later handle with a smaller need must
-// not lower it under an earlier handle's launches).
-static cudaError_t raise_smem_limit(gemm_kernel_t kern, int smem) {
+cudaError_t b2::raise_smem_limit(const void* kern, int smem) {
   static std::mutex mu;
-  static std::map<gemm_kernel_t, int> limit;
+  static std::map<const void*, int> limit;
   std::lock_guard<std::mutex> lk(mu);
   int& cur = limit[kern];
   if (smem <= cur) return cudaSuccess;
@@ -933,7 +929,7 @@ static int make_plan(b2_gemm_wq* h, int mti) {
   };
   // first guess occupancy with the cap, derive S, then shrink xt to what a unit really needs
   int smem = smem_for(xt_cap, nst_log2);
-  B2_CUDA_TRY(raise_smem_limit(kern, smem));
+  B2_CUDA_TRY(raise_smem_limit((const void*)kern, smem));
   int occ = 1;
   B2_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, kThreads, smem));
   if (occ < 1) occ = 1;
@@ -951,18 +947,17 @@ static int make_plan(b2_gemm_wq* h, int mti) {
   if (S > 32) S = 32;  // the reducer reads one k-slice statistic per lane
   // ---- split-K inside thread-block clusters (the default when it keeps enough CTAs in flight): S in {2, 4, 8} slices of a
   // tile form one cluster, the partial tiles meet in distributed shared memory.  Fewer, fatter CTAs than the global
-  // split (<= 8 slices), so the ring grows to keep the same number of weight bytes in flight.
+  // split (<= 8 slices), so the ring grows to keep the same number of weight bytes in flight.  8 is the portable cluster size
+  // limit; the non-portable 16 measured no better (o_proj 7.3 vs 6.4 us).
   bool cluster = false;
   if (env_int("B2_GEMM_CLUSTER", 1) && force <= 0 && S > 1) {
-    const int cmax = env_int("B2_GEMM_CLUSTER_MAX", 8);  // 16 (non-portable, opt-in) measured no better: o_proj 7.3 vs 6.4 us
     int sc = 2;
-    while (sc * 2 <= S && sc * 2 <= cmax) sc *= 2;
-    if (sc > 8) B2_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+    while (sc * 2 <= S && sc * 2 <= 8) sc *= 2;
     while (sc > 1 && !cluster) {
       if (h->NG * sc * 4 < sms * 3) break;  // too few CTAs to pull the HBM bandwidth: keep the wide global split
       const int nl2 = h->NG * sc <= 2 * sms ? log2_stages(env_int("B2_GEMM_CLUSTER_RING_KB", 64)) : nst_log2;
       const int sm_c = smem_for(xt_cap, nl2);
-      B2_CUDA_TRY(raise_smem_limit(kern, sm_c));
+      B2_CUDA_TRY(raise_smem_limit((const void*)kern, sm_c));
       cudaLaunchConfig_t cfg{};
       cfg.gridDim = dim3(h->NG * sc);
       cfg.blockDim = dim3(kThreads);
@@ -1128,26 +1123,20 @@ int b2_gemm_wq_attach_packed(b2_gemm_wq_t h, const void* packed, const void* sca
   return B2_OK;
 }
 
-static int mt_index_for(int M) { return M <= 8 ? 0 : (M <= 16 ? 1 : 2); }
-// rows per launch of the mma.sync kernel.  Sub-channel weights at M > 16 (they have no wgmma path yet): the MT=4 grouped
-// variant needs 124 registers (one CTA per SM, 0.05 of HBM at M=32), so they run in passes of 16 rows (MT=2, two CTAs per SM)
-// and stream the weights once per pass.  B2_GEMM_GROUPED_CHUNK=32 restores single-pass MT=4.
-static int rows_per_launch(const b2_gemm_wq* h) {
-  static const int gc = env_int("B2_GEMM_GROUPED_CHUNK", 16);
-  return (h->group_tiles > 0 && gc == 16) ? 16 : 32;
-}
+static int mt_index_for(int M) { return M <= 8 ? 0 : 1; }
+
+// Batches from kTcMinM up take the wgmma kernel: int4 / int8 per-channel, dense bf16 (lm_head), and int4 sub-channel (the scale
+// is applied to the weights in the dequant warps).  Sub-channel int8 weights have no wgmma path yet: at M > 16 they run on the
+// mma.sync kernel in passes of kGemvMaxM rows (MT = 2, two CTAs per SM) and stream the weights once per pass.
+constexpr int kTcMinM = 17;
 
 static bool use_tc(const b2_gemm_wq* h, int M) {
-  static const int min_m = env_int("B2_GEMM_TC_MIN_M", 17);
-  static const int grouped = env_int("B2_GEMM_TC_GROUPED", 1);
-  // int4 / int8 per-channel, dense bf16 (lm_head), and int4 sub-channel (the scale is applied to the weights in the dequant warps)
   if (h->group_k > 0) return true;  // general group sizes exist on the wgmma kernel only
-  return M >= min_m && (h->group_tiles == 0 || (grouped && h->d.wbits == 4));
+  return M >= kTcMinM && (h->group_tiles == 0 || h->d.wbits == 4);
 }
 
 static int make_tc_plan(b2_gemm_wq* h) {
   if (h->tc_S > 0) return B2_OK;
-  B2_CUDA_TRY(tc_configure(h->d.wbits));
   const int ctas = env_int("B2_GEMM_TC_CTAS_PER_SM", 1);
   auto split_for = [&](int slots, int smax) {
     int S = slots / h->NG;
@@ -1174,8 +1163,7 @@ size_t b2_gemm_wq_workspace_bytes(b2_gemm_wq_t h, int M) {
     const int sm = h->tc_S > h->tc_S2 ? h->tc_S : h->tc_S2;  // the fp8 entry point keeps the one-CTA-per-SM split
     return sm <= 1 ? 16 : (size_t)h->NG * sm * kTcMaxM * kBN * sizeof(float) + 16;
   }
-  const int rpl = rows_per_launch(h);
-  const int mc = M > rpl ? rpl : M;
+  const int mc = M > kGemvMaxM ? kGemvMaxM : M;
   const int mti = mt_index_for(mc);
   if (make_plan(h, mti) != B2_OK) return 0;
   const Plan& pl = h->plans[mti];
@@ -1336,35 +1324,29 @@ static int run_impl(b2_gemm_wq_t h, const void* A, int64_t lda, void* C, int64_t
     }
     return B2_OK;
   }
-  // ---- batches <= 32 without global split-K (wq_gemv2.cu) unless a fusion only the split-K kernel implements is asked for
-  if (!fused && !comm && h->d.ft == B2_DT_BF16) {  // (fp16 handles: the split-K kernel)
-    for (int m0 = 0; m0 < M; m0 += 32) {
-      Gemv2Launch a;
-      a.packed = (const uint8_t*)h->packed; a.sz = h->sz;
-      a.A = (const __nv_bfloat16*)A + (int64_t)m0 * lda; a.lda = lda;
-      a.C = (__nv_bfloat16*)C + (int64_t)m0 * ldc; a.ldc = ldc;
-      a.bias = (const __nv_bfloat16*)bias;
-      a.residual = residual ? (const __nv_bfloat16*)residual + (int64_t)m0 * ldc : nullptr;
-      a.M = (M - m0) > 32 ? 32 : (M - m0);
-      a.N = h->d.N; a.K = h->d.K; a.Np = h->Np; a.KT = h->KT; a.NG = h->NG;
-      a.wbits = h->d.wbits; a.group_tiles = h->group_tiles; a.pair = h->pair; a.act = activation; a.alpha = alpha;
-      Gemv2Plan pl;
-      if (!gemv2_plan(a, &pl)) {
-        if (m0 == 0) goto splitk;  // nothing launched yet: the whole call takes the split-K kernel
-        return B2_ERR_INTERNAL;
-      }
+  // ---- dense bf16 weights at batches <= 16: no global split-K (wq_gemv2.cu), unless a fusion only the split-K kernel
+  //      implements is asked for (fp16 handles: the split-K kernel)
+  if (h->d.wbits == 16 && M <= kGemvMaxM && !fused && !comm && h->d.ft == B2_DT_BF16) {
+    Gemv2Launch a;
+    a.packed = (const uint8_t*)h->packed;
+    a.A = (const __nv_bfloat16*)A; a.lda = lda;
+    a.C = (__nv_bfloat16*)C; a.ldc = ldc;
+    a.bias = (const __nv_bfloat16*)bias;
+    a.residual = (const __nv_bfloat16*)residual;
+    a.M = M; a.N = h->d.N; a.K = h->d.K; a.KT = h->KT; a.NG = h->NG;
+    a.pair = h->pair; a.act = activation; a.alpha = alpha;
+    Gemv2Plan pl;
+    if (gemv2_plan(a, &pl)) {
       cudaError_t e = gemv2_launch(a, pl, stream);
       if (e != cudaSuccess) {
         set_last_error("wq_gemv2 launch", e);
         return B2_ERR_CUDA;
       }
+      return B2_OK;
     }
-    return B2_OK;
   }
-splitk:
-  const int rpl = rows_per_launch(h);
-  for (int m0 = 0; m0 < M; m0 += rpl) {
-    const int mc = (M - m0) > rpl ? rpl : (M - m0);
+  for (int m0 = 0; m0 < M; m0 += kGemvMaxM) {
+    const int mc = (M - m0) > kGemvMaxM ? kGemvMaxM : (M - m0);
     const int mti = mt_index_for(mc);
     if (int st = make_plan(h, mti)) return st;
     const Plan& pl = h->plans[mti];

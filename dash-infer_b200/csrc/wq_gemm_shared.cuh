@@ -1,5 +1,8 @@
-// b200spark — definitions shared by the two weight-only GEMM kernels (mma.sync small-M, wgmma medium-M).
+// b200spark — definitions shared by the weight-only GEMM kernels (mma.sync small-M: wq_gemm.cu, wq_gemv2.cu; wgmma
+// medium-M: wq_gemm_tc.cu).
 #pragma once
+#include <cuda.h>  // CUtensorMap (types only; the encoder is fetched with cudaGetDriverEntryPoint)
+
 #include "b2_common.cuh"
 
 namespace b2 {
@@ -52,31 +55,39 @@ struct TcLaunch {
   const __nv_bfloat16* gamma_out = nullptr;
   int64_t ldxg = 0;
 };
-// GEMV without global split-K (wq_gemv2.cu)
+// GEMV for dense bf16 weights without global split-K (wq_gemv2.cu)
 struct Gemv2Launch {
   const uint8_t* packed;
-  const float2* sz;
   const __nv_bfloat16* A;
   int64_t lda;
   __nv_bfloat16* C;
   int64_t ldc;
   const __nv_bfloat16* bias;
   const __nv_bfloat16* residual;
-  int M, N, K, Np, KT, NG;
-  int wbits, group_tiles;  // group_tiles: k-tiles per quantization group, 0 = per channel
+  int M, N, K, KT, NG;
   bool pair;
   int act;
   float alpha;
 };
 struct Gemv2Plan {
-  int cb_log2, q, xt, nst_log2, mt, grid, smem;
+  int cb_log2, xt, nst_log2, mt, grid, smem;
 };
 bool gemv2_plan(const Gemv2Launch& a, Gemv2Plan* plan);   // false: use the split-K kernel
 cudaError_t gemv2_launch(const Gemv2Launch& a, const Gemv2Plan& plan, cudaStream_t stream);
 
-constexpr int kTcMaxM = 64;  // batch rows per wgmma launch
+constexpr int kGemvMaxM = 16;  // batch rows per launch of the mma.sync GEMV kernels (MT <= 2)
+constexpr int kTcMaxM = 64;    // batch rows per wgmma launch
 int tc_smem_bytes(int wbits, bool dual);
-cudaError_t tc_configure(int wbits);
 cudaError_t tc_launch(int wbits, const TcLaunch& a, cudaStream_t stream);
+
+// Raise a kernel's dynamic shared-memory opt-in to smem, never lower it: an instantiation is shared by handles whose plans
+// need different amounts, and a later handle with a smaller need must not lower the limit under an earlier one's launches.
+cudaError_t raise_smem_limit(const void* kern, int smem);
+
+// cuTensorMapEncodeTiled, fetched from the driver through the runtime (nullptr if unavailable)
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
+                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+EncodeTiledFn encode_tiled();
 
 }  // namespace b2

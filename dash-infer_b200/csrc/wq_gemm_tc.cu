@@ -31,8 +31,6 @@
 //                 instead of bf16 activations / outputs), the RMSNorm hand-off (row statistics + gamma-scaled copy out, 1/rms in).
 //
 // Roofline: HBM-bound up to M ~ 64 (~300 FLOP/B is the H100 tensor/HBM ridge); report both.
-#include <cuda.h>  // CUtensorMap (types only; the encoder is fetched with cudaGetDriverEntryPoint)
-
 #include <cstdlib>
 
 #include "b2_common.cuh"
@@ -688,36 +686,7 @@ int tc_smem_bytes(int wbits, bool dual) {
   return 1024 + kTcNSX * tps * kTcXTile + nsw * wstage + kTcNM * 4 + 96 * 8 + 64;  // barrier block: 21 barriers, 64 scales
 }
 
-cudaError_t tc_configure(int wbits) {
-  cudaError_t e = cudaSuccess;
-  auto cfg = [&](auto kern) { if (e == cudaSuccess) e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, tc_smem_bytes(wbits, false)); };
-  auto cfg2 = [&](auto kern) { if (e == cudaSuccess) e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, tc_smem_bytes(wbits, true)); };
-  if (wbits == 4) {
-    cfg2(wq_gemm_tc_kernel<4, false, false, false, true>); cfg2(wq_gemm_tc_kernel<4, true, false, false, true>);
-    cfg2(wq_gemm_tc_kernel<4, false, false, true, true>); cfg2(wq_gemm_tc_kernel<4, true, false, true, true>);
-    cfg2(wq_gemm_tc_kernel<4, false, false, false, true, true>); cfg2(wq_gemm_tc_kernel<4, true, false, false, true, true>);
-    cfg2(wq_gemm_tc_kernel<4, false, false, true, true, true>); cfg2(wq_gemm_tc_kernel<4, true, false, true, true, true>);
-    cfg(wq_gemm_tc_kernel<4, false>); cfg(wq_gemm_tc_kernel<4, true>); cfg(wq_gemm_tc_kernel<4, false, true>); cfg(wq_gemm_tc_kernel<4, true, true>);
-    cfg(wq_gemm_tc_kernel<4, false, false, true>); cfg(wq_gemm_tc_kernel<4, true, false, true>);
-    cfg(wq_gemm_tc_kernel<4, false, false, false, false, true>); cfg(wq_gemm_tc_kernel<4, true, false, false, false, true>);
-    cfg(wq_gemm_tc_kernel<4, false, false, true, false, true>); cfg(wq_gemm_tc_kernel<4, true, false, true, false, true>);
-  }
-  else if (wbits == 16) {
-    cfg(wq_gemm_tc_kernel<16, false>); cfg(wq_gemm_tc_kernel<16, true>);
-    cfg(wq_gemm_tc_kernel<16, false, false, false, false, true>); cfg(wq_gemm_tc_kernel<16, true, false, false, false, true>);
-  }
-  else {
-    cfg(wq_gemm_tc_kernel<8, false>); cfg(wq_gemm_tc_kernel<8, true>);
-    cfg(wq_gemm_tc_kernel<8, false, false, false, false, true>); cfg(wq_gemm_tc_kernel<8, true, false, false, false, true>);
-  }
-  return e;
-}
-
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static EncodeTiledFn encode_tiled() {
+EncodeTiledFn encode_tiled() {
   static EncodeTiledFn fn = nullptr;
   if (!fn) {
     void* p = nullptr;
@@ -762,7 +731,10 @@ cudaError_t tc_launch(int wbits, const TcLaunch& a, cudaStream_t stream) {
   const int grid = (persist && units > cap) ? cap : units;
   const bool multi = units > grid;
   const size_t smem = (size_t)tc_smem_bytes(wbits, dual);
-  auto go = [&](auto kern) { return launch(kern, dim3(grid), dim3(kTcThreads), smem, stream, true, p, amap); };
+  auto go = [&](auto kern) {
+    const cudaError_t e = raise_smem_limit((const void*)kern, (int)smem);
+    return e != cudaSuccess ? e : launch(kern, dim3(grid), dim3(kTcThreads), smem, stream, true, p, amap);
+  };
   const bool g = a.group_tiles > 0 || a.group_k > 0, h = a.fp16;
   if (a8) {
     if (wbits != 4 || h) return cudaErrorNotSupported;
