@@ -857,7 +857,6 @@ struct b2_gemm_wq {
   unsigned* counters = nullptr;
   Plan plans[2];  // MT = 1, 2
   int tc_S = 0;   // split-K of the wgmma path (0 = not planned)
-  int tc_S2 = 0;  // same for the two-CTAs-per-SM variant (int4, bf16 activations)
   bool pair = false;  // gate/up pair image (SwiGLU epilogue): physical channels = 2 * N
   int device = 0;
 };
@@ -1145,23 +1144,14 @@ static int make_tc_plan(b2_gemm_wq* h) {
     return S < 1 ? 1 : S;
   };
   h->tc_S = split_for(ctas * sm_count(), env_int("B2_GEMM_TC_MAX_SPLIT", 6));
-  h->tc_S2 = split_for(env_int("B2_GEMM_TC_DUAL_SLOTS", 2) * sm_count(), env_int("B2_GEMM_TC_MAX_SPLIT2", 8));
   return B2_OK;
-}
-
-// two CTAs per SM on the wgmma path: int4 weights with bf16 activations (B2_GEMM_TC_DUAL=0: one 194 KB CTA per SM)
-static bool tc_dual(const b2_gemm_wq* h) {
-  static const int on = env_int("B2_GEMM_TC_DUAL", 1);  // 2: every int4 shape, 1: shapes with >= 2 units per SM without split-K
-  if (!on || h->d.wbits != 4) return false;
-  return on >= 2 || h->NG >= 2 * sm_count();
 }
 
 size_t b2_gemm_wq_workspace_bytes(b2_gemm_wq_t h, int M) {
   if (!h || M <= 0) return 0;
   if (use_tc(h, M)) {
     if (make_tc_plan(h) != B2_OK) return 0;
-    const int sm = h->tc_S > h->tc_S2 ? h->tc_S : h->tc_S2;  // the fp8 entry point keeps the one-CTA-per-SM split
-    return sm <= 1 ? 16 : (size_t)h->NG * sm * kTcMaxM * kBN * sizeof(float) + 16;
+    return h->tc_S <= 1 ? 16 : (size_t)h->NG * h->tc_S * kTcMaxM * kBN * sizeof(float) + 16;
   }
   const int mc = M > kGemvMaxM ? kGemvMaxM : M;
   const int mti = mt_index_for(mc);
@@ -1286,12 +1276,10 @@ static int run_impl(b2_gemm_wq_t h, const void* A, int64_t lda, void* C, int64_t
   const bool grouped = h->group_tiles > 0;
   if (use_tc(h, M) && !comm) {  // decode batches 17..: wgmma path, 64 rows per launch
     if (int st = make_tc_plan(h)) return st;
-    const bool dual = tc_dual(h);
-    const int tcs = dual ? h->tc_S2 : h->tc_S;
+    const int tcs = h->tc_S;
     if (tcs > 1 && !workspace) return B2_ERR_PARAM;
     for (int m0 = 0; m0 < M; m0 += kTcMaxM) {
       TcLaunch a;
-      a.dual = dual;
       a.fp16 = h->d.ft == B2_DT_F16;
       a.packed = (const uint8_t*)h->packed; a.sz = h->sz;
       a.A = (const __nv_bfloat16*)A + (int64_t)m0 * lda; a.lda = lda;

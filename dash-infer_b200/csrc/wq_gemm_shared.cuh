@@ -43,7 +43,6 @@ struct TcLaunch {
   int group_tiles = 0;               // > 0: sub-channel weights, k-tiles per quantization group (sz is [G][Np])
   int group_k = 0, ngroups = 1;      // group_k > 0: group size not a multiple of 64 (a multiple of 8): params per 8-k word
   bool fp16 = false;                 // activations / outputs / bias / residual are fp16 (else bf16)
-  bool dual = false;                 // two CTAs per SM (int4 weights, bf16 activations): half-depth stages
   // RMSNorm hand-off between GEMMs (b2_gemm_fuse, batches >= 17).  Consumer: A holds bf16(x * gamma); the result rows are
   // scaled by rsqrt(sum_p norm_sumsq[p * norm_ld + m] / hidden + eps).  Producer: besides C it writes xg = bf16(C * gamma_out)
   // and, per 128-channel tile, the sum of squares of every stored row.
@@ -77,7 +76,7 @@ cudaError_t gemv2_launch(const Gemv2Launch& a, const Gemv2Plan& plan, cudaStream
 
 constexpr int kGemvMaxM = 16;  // batch rows per launch of the mma.sync GEMV kernels (MT <= 2)
 constexpr int kTcMaxM = 64;    // batch rows per wgmma launch
-int tc_smem_bytes(int wbits, bool dual);
+int tc_smem_bytes(int wbits);
 cudaError_t tc_launch(int wbits, const TcLaunch& a, cudaStream_t stream);
 
 // Raise a kernel's dynamic shared-memory opt-in to smem, never lower it: an instantiation is shared by handles whose plans

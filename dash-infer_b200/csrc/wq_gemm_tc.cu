@@ -25,13 +25,13 @@
 //                 several units; barriers and ring phases carry over and the next unit's first weight stages are issued
 //                 before the epilogue (MULTI instantiation).
 //
-//   variants    : DUAL (two CTAs per SM: half-depth stages — used where >= 2 units per SM exist without more split-K),
-//                 GROUPED (sub-channel int4: the scale is applied to the weights at dequantization; group sizes that do not
+//   variants    : GROUPED (sub-channel int4: the scale is applied to the weights at dequantization; group sizes that do not
 //                 divide the 64-k tile look their params up per 8-k word), A8 (fp8 activations, e4m3 wgmma), H (fp16
 //                 instead of bf16 activations / outputs), the RMSNorm hand-off (row statistics + gamma-scaled copy out, 1/rms in).
 //
 // Roofline: HBM-bound up to M ~ 64 (~300 FLOP/B is the H100 tensor/HBM ridge); report both.
 #include <cstdlib>
+#include <type_traits>
 
 #include "b2_common.cuh"
 #include "wq_gemm_shared.cuh"
@@ -72,10 +72,11 @@ __device__ __forceinline__ uint64_t wg_desc(uint32_t saddr) {
       "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
 
 // D[64 x NM] += A[64 x k] (registers) * B[k x NM] (smem): KIND 0 = bf16 (k16), 1 = fp16 (k16), 2 = e4m3 (k32).  NM = 32 uses
-// d[0..15] only.
-template <int KIND>
-__device__ __forceinline__ void wg_mma(float (&d)[32], const uint32_t (&a)[4], uint64_t desc, bool n32) {
-  if (n32) {
+// d[0..15] only.  The width is a template argument: with a runtime choice every MMA is a basic block of its own, and ptxas
+// then fences each one with a warpgroup.arrive and waits for it alone, so no MMA overlaps the next tile's dequantization.
+template <int KIND, bool N32>
+__device__ __forceinline__ void wg_mma(float (&d)[32], const uint32_t (&a)[4], uint64_t desc) {
+  if constexpr (N32) {
     if (KIND == 0)
       asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
                    "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 " B2_WG_D16 ", {%16,%17,%18,%19}, %20, p, 1, 1, 0;\n\t}"
@@ -168,20 +169,16 @@ struct TcParams {
 // in bf16, then ONE fused multiply-add per two weights: w = (q - 8) * s + (8 - z) * s, rounded to bf16 once — which is what
 // the reference's kernels (dequant in FT, gemm_lowp_utils.cuh:28-47) and its CPU path (weights stored in the model dtype)
 // feed their GEMMs with; the accumulator then needs no zero-point term and no row sums.
-// DUAL: two CTAs per SM (int4, bf16 activations).  A stage is half as deep (k128: 8 KB of weights, 16 KB of activations), so a
-// CTA needs 98 KB of shared memory; the fixed part of a unit — prologue, pipeline fill, split-K hand-off, epilogue — overlaps
-// the main loop of the CTA next to it instead of idling the SM.
 // H: fp16 activations / outputs (the exact-integer constants are 128 + q instead of 16 + q).
-template <int WBITS, bool MULTI, bool A8 = false, bool GROUPED = false, bool DUAL = false, bool H = false>
-__global__ void __launch_bounds__(kTcThreads, DUAL ? 2 : 1) wq_gemm_tc_kernel(const TcParams p, const __grid_constant__ CUtensorMap amap) {
+template <int WBITS, bool MULTI, bool A8 = false, bool GROUPED = false, bool H = false>
+__global__ void __launch_bounds__(kTcThreads, 1) wq_gemm_tc_kernel(const TcParams p, const __grid_constant__ CUtensorMap amap) {
   constexpr int TILE_BYTES = WBITS == 4 ? 4096 : (WBITS == 8 ? 8192 : 16384);
   constexpr int NCH = WBITS == 4 ? 2 : (WBITS == 8 ? 4 : 8);  // 16B chunks per row per k-tile
   constexpr int NSW = WBITS == 16 ? 4 : kTcNSW;               // weight stages (bf16: 32 KB each)
   // k-tiles per pipeline stage (k256 for W4, k128 for W8): one stage = 16 KB of weights per barrier round trip
-  constexpr int TPS = WBITS == 4 ? (DUAL ? 2 : 4) : 2;
+  constexpr int TPS = WBITS == 4 ? 4 : 2;
   constexpr int KIND = A8 ? 2 : (H ? 1 : 0);
   static_assert(!A8 || WBITS == 4, "fp8 activations: int4 weights only");
-  static_assert(!DUAL || (WBITS == 4 && !A8), "two CTAs per SM: int4 weights, 16-bit activations");
   static_assert(!H || !A8, "fp8 activations come with bf16 outputs");
   using F = Ft<H>;
   static_assert(!GROUPED || (!A8 && WBITS != 16), "sub-channel weights: bf16 activations, int4 / int8");
@@ -218,6 +215,11 @@ __global__ void __launch_bounds__(kTcThreads, DUAL ? 2 : 1) wq_gemm_tc_kernel(co
   // g = gbase + st is the stage index since kernel start.  Stage g uses weight slot g % NSW and X slot g % NSX.
   int w_pre = 0;  // weight stages of the current unit already issued during the previous unit's tail (producer thread only)
   const int my_units = !MULTI ? 1 : ((int)blockIdx.x < nunits) ? (nunits - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x : 0;
+  // The MMA width (N32: m64n32 for batches <= 32) is fixed once per launch: the whole unit loop is compiled once per width.
+  // A width chosen inside it would leave two main loops in one unit loop, and ptxas then serializes the MMAs of the
+  // persistent instantiations for lack of registers.
+  auto body = [&](auto n32) {
+  constexpr bool N32 = decltype(n32)::value;
   for (int uit = 0; uit < my_units; ++uit) {
   const int unit = (int)blockIdx.x + uit * (int)gridDim.x;
   const int ng = unit / p.S;
@@ -320,7 +322,6 @@ __global__ void __launch_bounds__(kTcThreads, DUAL ? 2 : 1) wq_gemm_tc_kernel(co
     // ===================== consumers: dequantize into wgmma A fragments, MMA, accumulators -> smem tile =====================
     const int wg = warp >> 2, g8 = lane >> 2, t4 = lane & 3;
     const int rr0 = wg * 64 + (warp & 3) * 16 + g8, rr1 = rr0 + 8;  // the two output channels (tile rows) of this thread
-    const bool n32 = p.nm == 32;
     // per-channel (scale, zero + bias constant): immutable, read before the waits
     const float2 sz0 = (WBITS == 16 || GROUPED) ? make_float2(1.f, 0.f) : p.sz[ng * kBN + rr0];
     const float2 sz1 = (WBITS == 16 || GROUPED) ? make_float2(1.f, 0.f) : p.sz[ng * kBN + rr1];
@@ -354,13 +355,8 @@ __global__ void __launch_bounds__(kTcThreads, DUAL ? 2 : 1) wq_gemm_tc_kernel(co
           const float2 z0 = __ldg(p.sz + (size_t)(kt / p.group_tiles) * p.Np + ng * kBN + rr0);  // (scale, zero + 16)
           const float2 z1 = __ldg(p.sz + (size_t)(kt / p.group_tiles) * p.Np + ng * kBN + rr1);
           const float c0 = (F::kBias + 8.f - z0.y) * z0.x, c1 = (F::kBias + 8.f - z1.y) * z1.x;  // (8 - zero) * scale
-          if (DUAL) {  // rows r0 / r1 in the two halves of one register (80-register budget), split at use
-            gs2[ti][0] = F::pack(z0.x, z1.x);
-            gc2[ti][0] = F::pack(c0, c1);
-          } else {
-            gs2[ti][0] = F::pack(z0.x, z0.x); gs2[ti][1] = F::pack(z1.x, z1.x);
-            gc2[ti][0] = F::pack(c0, c0); gc2[ti][1] = F::pack(c1, c1);
-          }
+          gs2[ti][0] = F::pack(z0.x, z0.x); gs2[ti][1] = F::pack(z1.x, z1.x);
+          gc2[ti][0] = F::pack(c0, c0); gc2[ti][1] = F::pack(c1, c1);
         }
       }
       mbar_wait(&wfull[slot], (g / NSW) & 1);
@@ -383,7 +379,7 @@ __global__ void __launch_bounds__(kTcThreads, DUAL ? 2 : 1) wq_gemm_tc_kernel(co
             }
             wg_fence();
 #pragma unroll
-            for (int c = 0; c < 2; ++c) wg_mma<KIND>(dt, a[c], bd + (uint64_t)(2 * c), n32);
+            for (int c = 0; c < 2; ++c) wg_mma<KIND, N32>(dt, a[c], bd + (uint64_t)(2 * c));
           } else {
             const uint64_t bd = wg_desc(xring_u + xs * XSTAGE + ti * kTcXTile);
             if (WBITS == 4) {
@@ -411,14 +407,7 @@ __global__ void __launch_bounds__(kTcThreads, DUAL ? 2 : 1) wq_gemm_tc_kernel(co
                       }
                     } else {
 #pragma unroll
-                      for (int e = 0; e < 4; ++e) {
-                        if (DUAL) {
-                          sw[e] = __byte_perm(gs2[ti][0], 0, (e & 1) ? 0x3232 : 0x1010);
-                          cw[e] = __byte_perm(gc2[ti][0], 0, (e & 1) ? 0x3232 : 0x1010);
-                        } else {
-                          sw[e] = gs2[ti][e & 1]; cw[e] = gc2[ti][e & 1];
-                        }
-                      }
+                      for (int e = 0; e < 4; ++e) { sw[e] = gs2[ti][e & 1]; cw[e] = gc2[ti][e & 1]; }
                     }
 #pragma unroll
                     for (int e = 0; e < 4; ++e) {
@@ -433,19 +422,10 @@ __global__ void __launch_bounds__(kTcThreads, DUAL ? 2 : 1) wq_gemm_tc_kernel(co
                     }
                   }
                 }
-                if (DUAL) {  // one commit group per 32-k chunk: half the fragment registers in flight (80-register budget)
-                  wg_fence();
-                  wg_mma<KIND>(d, a[2 * c], bd + (uint64_t)(4 * c), n32);
-                  wg_mma<KIND>(d, a[2 * c + 1], bd + (uint64_t)(4 * c + 2), n32);
-                  wg_commit();
-                  wg_wait<1>();
-                }
               }
-              if (!DUAL) {
-                wg_fence();
+              wg_fence();
 #pragma unroll
-                for (int kk = 0; kk < 4; ++kk) wg_mma<KIND>(d, a[kk], bd + (uint64_t)(2 * kk), n32);
-              }
+              for (int kk = 0; kk < 4; ++kk) wg_mma<KIND, N32>(d, a[kk], bd + (uint64_t)(2 * kk));
             } else if (WBITS == 16) {  // bf16 weights: k16 step kk = chunks 2kk (k pair 2t), 2kk + 1 (k pair 2t + 8)
               uint32_t a[4][4];
 #pragma unroll
@@ -457,7 +437,7 @@ __global__ void __launch_bounds__(kTcThreads, DUAL ? 2 : 1) wq_gemm_tc_kernel(co
               }
               wg_fence();
 #pragma unroll
-              for (int kk = 0; kk < 4; ++kk) wg_mma<KIND>(d, a[kk], bd + (uint64_t)(2 * kk), n32);
+              for (int kk = 0; kk < 4; ++kk) wg_mma<KIND, N32>(d, a[kk], bd + (uint64_t)(2 * kk));
             } else {  // W8: chunk c = k16 step c; the low and high nibble planes are two MMAs (16 + lo, 16 (16 + hi))
               uint32_t lo[4][4], hi[4][4];
 #pragma unroll
@@ -473,15 +453,13 @@ __global__ void __launch_bounds__(kTcThreads, DUAL ? 2 : 1) wq_gemm_tc_kernel(co
               wg_fence();
 #pragma unroll
               for (int c = 0; c < 4; ++c) {
-                wg_mma<KIND>(d, lo[c], bd + (uint64_t)(2 * c), n32);
-                wg_mma<KIND>(d, hi[c], bd + (uint64_t)(2 * c), n32);
+                wg_mma<KIND, N32>(d, lo[c], bd + (uint64_t)(2 * c));
+                wg_mma<KIND, N32>(d, hi[c], bd + (uint64_t)(2 * c));
               }
             }
           }
-          if (!DUAL) {  // (DUAL committed and waited per chunk above)
-            wg_commit();
-            wg_wait<1>();  // the previous tile's MMAs completed (their fragment registers and, at a stage start, X slot are free)
-          }
+          wg_commit();
+          wg_wait<1>();  // the previous tile's MMAs completed (their fragment registers and, at a stage start, X slot are free)
           if (ti == 0 && prev_xs >= 0) {
             __syncwarp();
             if (lane == 0) mbar_arrive(&xfree[prev_xs]);
@@ -677,10 +655,15 @@ __global__ void __launch_bounds__(kTcThreads, DUAL ? 2 : 1) wq_gemm_tc_kernel(co
   if (MULTI) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy tile writes before the next unit's TMA writes
   __syncthreads();  // the tile in the X ring is free again
   }  // unit loop
+  };
+  if (p.nm == 32)
+    body(std::true_type{});
+  else
+    body(std::false_type{});
 }
 
-int tc_smem_bytes(int wbits, bool dual) {
-  const int tps = wbits == 4 ? (dual ? 2 : 4) : 2;
+int tc_smem_bytes(int wbits) {
+  const int tps = wbits == 4 ? 4 : 2;
   const int wstage = tps * (wbits == 4 ? 4096 : (wbits == 8 ? 8192 : 16384));
   const int nsw = wbits == 16 ? 4 : kTcNSW;
   return 1024 + kTcNSX * tps * kTcXTile + nsw * wstage + kTcNM * 4 + 96 * 8 + 64;  // barrier block: 21 barriers, 64 scales
@@ -726,11 +709,10 @@ cudaError_t tc_launch(int wbits, const TcLaunch& a, cudaStream_t stream) {
   // persistent: one CTA per SM walks the (n-group, k-split) units; B2_GEMM_TC_PERSIST=0 launches one CTA per unit
   static const int persist = [] { const char* e = getenv("B2_GEMM_TC_PERSIST"); return e ? atoi(e) : 1; }();
   const int units = a.NG * a.S;
-  const bool dual = a.dual && wbits == 4 && !a8;
-  const int cap = (dual ? 2 : 1) * sm_count();
+  const int cap = sm_count();
   const int grid = (persist && units > cap) ? cap : units;
   const bool multi = units > grid;
-  const size_t smem = (size_t)tc_smem_bytes(wbits, dual);
+  const size_t smem = (size_t)tc_smem_bytes(wbits);
   auto go = [&](auto kern) {
     const cudaError_t e = raise_smem_limit((const void*)kern, (int)smem);
     return e != cudaSuccess ? e : launch(kern, dim3(grid), dim3(kTcThreads), smem, stream, true, p, amap);
@@ -742,31 +724,23 @@ cudaError_t tc_launch(int wbits, const TcLaunch& a, cudaStream_t stream) {
   }
   if (g && wbits != 4) return cudaErrorNotSupported;
   if (wbits == 4) {
-    // (multi, grouped, dual, fp16)
-    switch ((multi ? 8 : 0) | (g ? 4 : 0) | (dual ? 2 : 0) | (h ? 1 : 0)) {
-      case 0: return go(wq_gemm_tc_kernel<4, false, false, false, false, false>);
-      case 1: return go(wq_gemm_tc_kernel<4, false, false, false, false, true>);
-      case 2: return go(wq_gemm_tc_kernel<4, false, false, false, true, false>);
-      case 3: return go(wq_gemm_tc_kernel<4, false, false, false, true, true>);
-      case 4: return go(wq_gemm_tc_kernel<4, false, false, true, false, false>);
-      case 5: return go(wq_gemm_tc_kernel<4, false, false, true, false, true>);
-      case 6: return go(wq_gemm_tc_kernel<4, false, false, true, true, false>);
-      case 7: return go(wq_gemm_tc_kernel<4, false, false, true, true, true>);
-      case 8: return go(wq_gemm_tc_kernel<4, true, false, false, false, false>);
-      case 9: return go(wq_gemm_tc_kernel<4, true, false, false, false, true>);
-      case 10: return go(wq_gemm_tc_kernel<4, true, false, false, true, false>);
-      case 11: return go(wq_gemm_tc_kernel<4, true, false, false, true, true>);
-      case 12: return go(wq_gemm_tc_kernel<4, true, false, true, false, false>);
-      case 13: return go(wq_gemm_tc_kernel<4, true, false, true, false, true>);
-      case 14: return go(wq_gemm_tc_kernel<4, true, false, true, true, false>);
-      default: return go(wq_gemm_tc_kernel<4, true, false, true, true, true>);
+    // (multi, grouped, fp16)
+    switch ((multi ? 4 : 0) | (g ? 2 : 0) | (h ? 1 : 0)) {
+      case 0: return go(wq_gemm_tc_kernel<4, false, false, false, false>);
+      case 1: return go(wq_gemm_tc_kernel<4, false, false, false, true>);
+      case 2: return go(wq_gemm_tc_kernel<4, false, false, true, false>);
+      case 3: return go(wq_gemm_tc_kernel<4, false, false, true, true>);
+      case 4: return go(wq_gemm_tc_kernel<4, true, false, false, false>);
+      case 5: return go(wq_gemm_tc_kernel<4, true, false, false, true>);
+      case 6: return go(wq_gemm_tc_kernel<4, true, false, true, false>);
+      default: return go(wq_gemm_tc_kernel<4, true, false, true, true>);
     }
   }
   if (wbits == 16) {
-    if (h) return multi ? go(wq_gemm_tc_kernel<16, true, false, false, false, true>) : go(wq_gemm_tc_kernel<16, false, false, false, false, true>);
+    if (h) return multi ? go(wq_gemm_tc_kernel<16, true, false, false, true>) : go(wq_gemm_tc_kernel<16, false, false, false, true>);
     return multi ? go(wq_gemm_tc_kernel<16, true>) : go(wq_gemm_tc_kernel<16, false>);
   }
-  if (h) return multi ? go(wq_gemm_tc_kernel<8, true, false, false, false, true>) : go(wq_gemm_tc_kernel<8, false, false, false, false, true>);
+  if (h) return multi ? go(wq_gemm_tc_kernel<8, true, false, false, true>) : go(wq_gemm_tc_kernel<8, false, false, false, true>);
   return multi ? go(wq_gemm_tc_kernel<8, true>) : go(wq_gemm_tc_kernel<8, false>);
 }
 
