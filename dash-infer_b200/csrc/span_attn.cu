@@ -67,6 +67,8 @@ struct KVTraits<B2_KV_U4> {
   static constexpr int TILE = kTile * ROW;
   static constexpr int PARAM = kTile * 8;
 };
+template <>
+struct KVTraits<B2_KV_FP8> : KVTraits<B2_KV_I8> {};  // the I8 layout: one e4m3 byte per element, {0, scale} per row
 
 // Issue the cp.async copies of one 64-token tile (K and V) of (sequence b, kv-head g) into a stage.
 // Thread tid owns 16-byte chunk column (tid & (CPR-1)) of rows (tid / CPR) + i * (128 / CPR): the swizzled
@@ -208,9 +210,24 @@ __device__ __forceinline__ void tile_compute_bf16(const uint8_t* st, int warp, i
 //   O[h,d]       = sum_tok P'[h,tok]*(BIAS+u[tok,d]) - sum_tok P'[h,tok]*(BIAS + z_v[tok]),   P' = P * s_v[tok]
 // with BIAS = 1024+128 (int8, u = q+128) or 1024 (uint4).  Same math as QuantParam::Dequant
 // (span-attention/src/cache_quant/impl_i8.cuh:66-70, impl_u4.cuh:97-106) without ever rounding a dequantized value.
+// FP8 shares the I8 tile layout and d-order; its codes are converted with cvt (e4m3 -> fp16 exact) and have no zero point.
 __device__ __forceinline__ uint32_t prmt(uint32_t a, uint32_t b, uint32_t sel) {
   uint32_t d;
   asm("prmt.b32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(sel));
+  return d;
+}
+
+// ---- FP8 KV: the e4m3 codes convert EXACTLY to fp16 (one F2FP.F16.E4M3.UNPACK_B per pair), so the same fp16 MMAs run on
+// the codes themselves and only the per-token scale remains (no zero point):
+//   score[h,tok] = s_k[tok] * sum_d Q[h,d] * e4m3(k[tok,d]),   O[h,d] = sum_tok (P[h,tok] * s_v[tok]) * e4m3(v[tok,d])
+// Byte HALF (0: bytes 0,1; 1: bytes 2,3) of w -> fp16x2 {lower byte, upper byte}.
+template <int HALF>
+__device__ __forceinline__ uint32_t e4m3x2_to_f16x2(uint32_t w) {
+  uint32_t d;
+  if (HALF == 0)
+    asm("{\n\t.reg .b16 lo, hi;\n\tmov.b32 {lo, hi}, %1;\n\tcvt.rn.f16x2.e4m3x2 %0, lo;\n\t}" : "=r"(d) : "r"(w));
+  else
+    asm("{\n\t.reg .b16 lo, hi;\n\tmov.b32 {lo, hi}, %1;\n\tcvt.rn.f16x2.e4m3x2 %0, hi;\n\t}" : "=r"(d) : "r"(w));
   return d;
 }
 
@@ -240,6 +257,17 @@ __device__ __forceinline__ void tile_compute_q(const uint8_t* st, int warp, int 
           const int ks = 4 * c2 + j;
           const uint32_t b0 = prmt(kw[j], 0x64646464u, 0x5140u), b1 = prmt(kw[j], 0x64646464u, 0x7362u);
           mma_f16_16816(sc[nt], qa[ks][0], qa[ks][1], qa[ks][2], qa[ks][3], b0, b1);
+        }
+      }
+    } else if (QM == B2_KV_FP8) {  // the I8 d-order: the two halves of a word pair like prmt 0x5140 / 0x7362 above
+#pragma unroll
+      for (int c2 = 0; c2 < 2; ++c2) {
+        const uint4 kv = lds128(kb + row * T::ROW + ((((2 * t + c2) ^ (row & 7))) << 4));
+        const uint32_t kw[4] = {kv.x, kv.y, kv.z, kv.w};
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const int ks = 4 * c2 + j;
+          mma_f16_16816(sc[nt], qa[ks][0], qa[ks][1], qa[ks][2], qa[ks][3], e4m3x2_to_f16x2<0>(kw[j]), e4m3x2_to_f16x2<1>(kw[j]));
         }
       }
     } else {
@@ -275,7 +303,7 @@ __device__ __forceinline__ void tile_compute_q(const uint8_t* st, int warp, int 
     for (int cc = 0; cc < 4; ++cc) {
       const int tok = wtok + nt * 8 + 2 * t + (cc & 1);
       const float kz = (cc & 1) ? kp.z : kp.x, ksc = (cc & 1) ? kp.w : kp.y;
-      const float raw = ksc * (sc[nt][cc] - (BIAS + kz) * sq[cc >> 1]);
+      const float raw = QM == B2_KV_FP8 ? ksc * sc[nt][cc] : ksc * (sc[nt][cc] - (BIAS + kz) * sq[cc >> 1]);
       const float v = tok < tok1 ? raw * scale_log2 : -INFINITY;
       sc[nt][cc] = v;
       mx[cc >> 1] = fmaxf(mx[cc >> 1], v);
@@ -305,17 +333,19 @@ __device__ __forceinline__ void tile_compute_q(const uint8_t* st, int warp, int 
     }
     pa[2 * nt] = pack_f16x2(pq[0], pq[1]);
     pa[2 * nt + 1] = pack_f16x2(pq[2], pq[3]);
-    // zero-point term with the SAME fp16-rounded probabilities the tensor core sees
-    const __half2 h01 = *reinterpret_cast<const __half2*>(&pa[2 * nt]), h23 = *reinterpret_cast<const __half2*>(&pa[2 * nt + 1]);
-    csum[0] += __low2float(h01) * (BIAS + vz[nt][0]) + __high2float(h01) * (BIAS + vz[nt][1]);
-    csum[1] += __low2float(h23) * (BIAS + vz[nt][0]) + __high2float(h23) * (BIAS + vz[nt][1]);
+    if (QM != B2_KV_FP8) {
+      // zero-point term with the SAME fp16-rounded probabilities the tensor core sees
+      const __half2 h01 = *reinterpret_cast<const __half2*>(&pa[2 * nt]), h23 = *reinterpret_cast<const __half2*>(&pa[2 * nt + 1]);
+      csum[0] += __low2float(h01) * (BIAS + vz[nt][0]) + __high2float(h01) * (BIAS + vz[nt][1]);
+      csum[1] += __low2float(h23) * (BIAS + vz[nt][0]) + __high2float(h23) * (BIAS + vz[nt][1]);
+    }
   }
 #pragma unroll
   for (int r2 = 0; r2 < 2; ++r2) {
     psum[r2] += __shfl_xor_sync(0xffffffffu, psum[r2], 1);
     psum[r2] += __shfl_xor_sync(0xffffffffu, psum[r2], 2);
     lrow[r2] = lrow[r2] * corr[r2] + psum[r2];
-    cacc[r2] = cacc[r2] * corr[r2] + csum[r2];  // per-thread partial (its 4 tokens); reduced over the quad at the end
+    if (QM != B2_KV_FP8) cacc[r2] = cacc[r2] * corr[r2] + csum[r2];  // per-thread partial (its 4 tokens); reduced over the quad at the end
   }
   if (corr[0] != 1.f || corr[1] != 1.f) {
 #pragma unroll
@@ -337,6 +367,18 @@ __device__ __forceinline__ void tile_compute_q(const uint8_t* st, int warp, int 
         const uint32_t lo = r[2 * u] ^ 0x80808080u, hi = r[2 * u + 1] ^ 0x80808080u;
         mma_f16_16816(o[2 * (c + u)], pa[0], pa[1], pa[2], pa[3], prmt(lo, 0x64646464u, 0x6240u), prmt(hi, 0x64646464u, 0x6240u));
         mma_f16_16816(o[2 * (c + u) + 1], pa[0], pa[1], pa[2], pa[3], prmt(lo, 0x64646464u, 0x7351u), prmt(hi, 0x64646464u, 0x7351u));
+      }
+    }
+  } else if (QM == B2_KV_FP8) {
+#pragma unroll
+    for (int c = 0; c < 8; c += 2) {
+      uint32_t r[4];
+      ldmatrix_x4_trans(r, vb + vrow * T::ROW + (((c + (mi >> 1)) ^ (vrow & 7)) << 4));
+#pragma unroll
+      for (int u = 0; u < 2; ++u) {  // bytes {V[2t][2g], V[2t][2g+1], V[2t+1][2g], V[2t+1][2g+1]} -> {even d pair, odd d pair}
+        const uint32_t lo = prmt(r[2 * u], 0u, 0x3120u), hi = prmt(r[2 * u + 1], 0u, 0x3120u);
+        mma_f16_16816(o[2 * (c + u)], pa[0], pa[1], pa[2], pa[3], e4m3x2_to_f16x2<0>(lo), e4m3x2_to_f16x2<0>(hi));
+        mma_f16_16816(o[2 * (c + u) + 1], pa[0], pa[1], pa[2], pa[3], e4m3x2_to_f16x2<1>(lo), e4m3x2_to_f16x2<1>(hi));
       }
     }
   } else {
@@ -607,7 +649,7 @@ __global__ void __launch_bounds__(kAttnThreads) span_attn_kernel(const AttnParam
           qa[ks][3] = r1 ? *reinterpret_cast<const uint32_t*>(qb + (gq + 8) * kHead + d0 + 8) : 0u;
         } else {
           int da[2], db[2];  // d of (reg lo, reg hi) for the k-columns (2t,2t+1) and (2t+8,2t+9)
-          if (QM == B2_KV_I8) {
+          if (QM == B2_KV_I8 || QM == B2_KV_FP8) {
             da[0] = 32 * t + 4 * ks; da[1] = da[0] + 1; db[0] = da[0] + 2; db[1] = da[0] + 3;
           } else {
             const int base = 32 * t + 8 * (ks >> 1) + 2 * (ks & 1);
@@ -627,13 +669,13 @@ __global__ void __launch_bounds__(kAttnThreads) span_attn_kernel(const AttnParam
           qa[ks][2] = pack_f16x2(f[0][2], f[0][3]);
           qa[ks][3] = pack_f16x2(f[1][2], f[1][3]);
 #pragma unroll
-          for (int rr = 0; rr < 2; ++rr) {  // sums of exactly the fp16 values the tensor core multiplies
+          for (int rr = 0; rr < 2 && QM != B2_KV_FP8; ++rr) {  // sums of exactly the fp16 values the tensor core multiplies
             const __half2 ha = *reinterpret_cast<const __half2*>(&qa[ks][rr]), hb = *reinterpret_cast<const __half2*>(&qa[ks][2 + rr]);
             sq[rr] += (__low2float(ha) + __high2float(ha)) + (__low2float(hb) + __high2float(hb));
           }
         }
       }
-      if (QM != B2_KV_NONE) {
+      if (QM != B2_KV_NONE && QM != B2_KV_FP8) {
 #pragma unroll
         for (int rr = 0; rr < 2; ++rr) {
           sq[rr] += __shfl_xor_sync(0xffffffffu, sq[rr], 1);
@@ -673,7 +715,7 @@ __global__ void __launch_bounds__(kAttnThreads) span_attn_kernel(const AttnParam
     if (tr0) B2_TR(g_attn_tr, 5);
 
     // ---------------- merge the 4 warps (each saw a disjoint token slice) ----------------
-    if (QM != B2_KV_NONE) {  // subtract the zero-point term (quad-reduced) before leaving registers
+    if (QM != B2_KV_NONE && QM != B2_KV_FP8) {  // subtract the zero-point term (quad-reduced) before leaving registers
 #pragma unroll
       for (int rr = 0; rr < 2; ++rr) {
         cacc[rr] += __shfl_xor_sync(0xffffffffu, cacc[rr], 1);
@@ -695,7 +737,7 @@ __global__ void __launch_bounds__(kAttnThreads) span_attn_kernel(const AttnParam
           *reinterpret_cast<float2*>(m0 + d) = make_float2(o[dt][0], o[dt][1]);
           *reinterpret_cast<float2*>(m1 + d) = make_float2(o[dt][2], o[dt][3]);
         }
-      } else if (QM == B2_KV_I8) {  // o[2c] <-> d = 16c+4t+{0,2}, o[2c+1] <-> d = 16c+4t+{1,3}
+      } else if (QM == B2_KV_I8 || QM == B2_KV_FP8) {  // o[2c] <-> d = 16c+4t+{0,2}, o[2c+1] <-> d = 16c+4t+{1,3}
 #pragma unroll
         for (int c = 0; c < 8; ++c) {
           const int d = 16 * c + 4 * t;
@@ -848,6 +890,21 @@ __device__ __forceinline__ void quant_row(const float (&x)[4], float& qz, float&
   }
 }
 
+// FP8 row quantizer (B2_KV_FP8, the convention of b2_quant_fp8): scale = max(amax, 1e-12) / 448 and r = 1 / scale, both
+// IEEE fp32 (this library is built without fast math), code = e4m3(x * r), round to nearest even, saturating to +-448 —
+// a finite input never becomes 0x7F / 0xFF (the two e4m3fn NaNs).  Returns the lane's 4 codes, element 0 in the low byte.
+__device__ __forceinline__ uint32_t quant_row_fp8(const float (&x)[4], float& qs) {
+  float amax = fmaxf(fmaxf(fabsf(x[0]), fabsf(x[1])), fmaxf(fabsf(x[2]), fabsf(x[3])));
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+  qs = fmaxf(amax, 1e-12f) / 448.f;
+  const float r = 1.f / qs;
+  uint16_t p01, p23;  // cvt puts its FIRST source in the UPPER byte
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(p01) : "f"(x[1] * r), "f"(x[0] * r));
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(p23) : "f"(x[3] * r), "f"(x[2] * r));
+  return (uint32_t)p01 | ((uint32_t)p23 << 16);
+}
+
 // store one (possibly quantized) 128-wide row at row index rowi of a span ([n_rows][row] data, then [n_rows] {zero, scale})
 template <int QM, bool H>
 __device__ __forceinline__ void store_row(uint8_t* span, size_t rowi, int n_rows, int lane, const float (&x)[4]) {
@@ -855,9 +912,15 @@ __device__ __forceinline__ void store_row(uint8_t* span, size_t rowi, int n_rows
     *reinterpret_cast<uint2*>(span + rowi * 256 + lane * 8) = make_uint2(Ft<H>::pack(x[0], x[1]), Ft<H>::pack(x[2], x[3]));
     return;
   }
+  if (QM == B2_KV_FP8) {
+    float s;
+    *reinterpret_cast<uint32_t*>(span + rowi * 128 + lane * 4) = quant_row_fp8(x, s);
+    if (lane == 0) *reinterpret_cast<float2*>(span + (size_t)n_rows * 128 + rowi * 8) = make_float2(0.f, s);
+    return;
+  }
   float qz, qs;
   int qv[4];
-  quant_row<QM == B2_KV_NONE ? B2_KV_I8 : QM>(x, qz, qs, qv);
+  quant_row<QM == B2_KV_NONE || QM == B2_KV_FP8 ? B2_KV_I8 : QM>(x, qz, qs, qv);
   if (QM == B2_KV_I8) {
     const uint32_t w = (qv[0] & 0xff) | ((qv[1] & 0xff) << 8) | ((qv[2] & 0xff) << 16) | ((uint32_t)(qv[3] & 0xff) << 24);
     *reinterpret_cast<uint32_t*>(span + rowi * 128 + lane * 4) = w;
@@ -979,7 +1042,7 @@ static int check_cfg(const b2_span_cfg* c) {
   // 128: the reference GPU library's only head size (span_attention.hpp:203-208).  64: bf16 KV only — the parity anchor C0
   // (Qwen2-0.5B) that the reference runs on its CPU path; span_attn64.cu
   if (c->head_size != kHead && !(c->head_size == 64 && c->quant_mode == B2_KV_NONE)) return B2_ERR_UNSUPPORTED;
-  if (c->quant_mode < B2_KV_NONE || c->quant_mode > B2_KV_U4) return B2_ERR_PARAM;
+  if (c->quant_mode < B2_KV_NONE || c->quant_mode > B2_KV_FP8) return B2_ERR_PARAM;
   if (c->span_len != 16 && c->span_len != 32 && c->span_len != 64 && c->span_len != 128) return B2_ERR_PARAM;
   if (c->n_groups <= 0 || c->n_heads <= 0 || c->n_heads % c->n_groups) return B2_ERR_PARAM;
   if (c->n_heads / c->n_groups > 16) return B2_ERR_UNSUPPORTED;
@@ -1009,12 +1072,14 @@ static attn_kernel_t attn_kernel_for(int qm, bool fp16) {
     switch (qm) {
       case B2_KV_NONE: return span_attn_kernel<B2_KV_NONE, true>;
       case B2_KV_I8: return span_attn_kernel<B2_KV_I8, true>;
+      case B2_KV_FP8: return span_attn_kernel<B2_KV_FP8, true>;
       default: return span_attn_kernel<B2_KV_U4, true>;
     }
   }
   switch (qm) {
     case B2_KV_NONE: return span_attn_kernel<B2_KV_NONE, false>;
     case B2_KV_I8: return span_attn_kernel<B2_KV_I8, false>;
+    case B2_KV_FP8: return span_attn_kernel<B2_KV_FP8, false>;
     default: return span_attn_kernel<B2_KV_U4, false>;
   }
 }
@@ -1026,14 +1091,15 @@ size_t b2_span_bytes(const b2_span_cfg* c) {
   const size_t rows = (size_t)c->span_len * c->n_groups;
   switch (c->quant_mode) {  // csrc/runtime/cache/virtual_cache.cpp:202-232
     case B2_KV_NONE: return rows * c->head_size * 2;
-    case B2_KV_I8: return rows * c->head_size + 2 * rows * 4;
-    default: return rows * c->head_size / 2 + 2 * rows * 4;
+    case B2_KV_I8: case B2_KV_FP8: return rows * c->head_size + 2 * rows * 4;
+    case B2_KV_U4: return rows * c->head_size / 2 + 2 * rows * 4;
+    default: return 0;
   }
 }
 
 size_t b2_span_attn_algo_bytes(const b2_span_cfg* c, int64_t total_tokens) {
   if (check_cfg(c) != B2_OK) return 0;
-  const size_t row = c->quant_mode == B2_KV_NONE ? (size_t)c->head_size * 2 : (c->quant_mode == B2_KV_I8 ? 128 + 8 : 64 + 8);
+  const size_t row = c->quant_mode == B2_KV_NONE ? (size_t)c->head_size * 2 : (c->quant_mode == B2_KV_U4 ? 64 + 8 : 128 + 8);
   return (size_t)total_tokens * 2 * c->n_groups * row;
 }
 
@@ -1046,10 +1112,11 @@ int b2_span_attn_create(b2_span_attn_t* out, const b2_span_cfg* cfg, int max_bat
   h->cfg = *cfg;
   h->max_batch = max_batch;
   attn_kernel_t kern = attn_kernel_for_cfg(cfg);
+  const bool byte_rows = cfg->quant_mode == B2_KV_I8 || cfg->quant_mode == B2_KV_FP8;  // same stage size, same default depth
   const int sb = cfg->quant_mode == B2_KV_NONE ? stage_bytes<B2_KV_NONE>()
-                                                : (cfg->quant_mode == B2_KV_I8 ? stage_bytes<B2_KV_I8>() : stage_bytes<B2_KV_U4>());
+                                                : (byte_rows ? stage_bytes<B2_KV_I8>() : stage_bytes<B2_KV_U4>());
   const char* env = getenv("B2_ATTN_STAGES");
-  h->nstage = env ? atoi(env) : (cfg->quant_mode == B2_KV_NONE ? 2 : (cfg->quant_mode == B2_KV_I8 ? 3 : 4));
+  h->nstage = env ? atoi(env) : (cfg->quant_mode == B2_KV_NONE ? 2 : (byte_rows ? 3 : 4));
   if (h->nstage < 2) h->nstage = 2;
   if (h->nstage > 4) h->nstage = 4;
   const int merge = (4 * 16 * kMergeRS + 4 * 16 * 2) * 4;
@@ -1150,6 +1217,8 @@ int b2_span_context_copy(const b2_span_cfg* cfg, void* const* spans, const void*
                                              : launch(context_span_copy_kernel<B2_KV_NONE, false>, grid, block, 0, stream, true, p);
   else if (cfg->quant_mode == B2_KV_I8) e = h16 ? launch(context_span_copy_kernel<B2_KV_I8, true>, grid, block, 0, stream, true, p)
                                                 : launch(context_span_copy_kernel<B2_KV_I8, false>, grid, block, 0, stream, true, p);
+  else if (cfg->quant_mode == B2_KV_FP8) e = h16 ? launch(context_span_copy_kernel<B2_KV_FP8, true>, grid, block, 0, stream, true, p)
+                                                 : launch(context_span_copy_kernel<B2_KV_FP8, false>, grid, block, 0, stream, true, p);
   else e = h16 ? launch(context_span_copy_kernel<B2_KV_U4, true>, grid, block, 0, stream, true, p)
                : launch(context_span_copy_kernel<B2_KV_U4, false>, grid, block, 0, stream, true, p);
   if (e != cudaSuccess) {
@@ -1182,6 +1251,8 @@ int b2_span_cache_append(const b2_span_cfg* cfg, void* const* k_spans, void* con
                                              : launch(cache_append_kernel<B2_KV_NONE, false>, grid, block, 0, stream, true, p);
   else if (cfg->quant_mode == B2_KV_I8) e = h16 ? launch(cache_append_kernel<B2_KV_I8, true>, grid, block, 0, stream, true, p)
                                                 : launch(cache_append_kernel<B2_KV_I8, false>, grid, block, 0, stream, true, p);
+  else if (cfg->quant_mode == B2_KV_FP8) e = h16 ? launch(cache_append_kernel<B2_KV_FP8, true>, grid, block, 0, stream, true, p)
+                                                 : launch(cache_append_kernel<B2_KV_FP8, false>, grid, block, 0, stream, true, p);
   else e = h16 ? launch(cache_append_kernel<B2_KV_U4, true>, grid, block, 0, stream, true, p)
                : launch(cache_append_kernel<B2_KV_U4, false>, grid, block, 0, stream, true, p);
   if (e != cudaSuccess) {

@@ -42,7 +42,8 @@ enum DeviceType : int { DEVICETYPE_UNDEFINED = 0, CPU = 1, CUDA = 2 };
 enum DataMode : int { DENSE = 0 };
 enum UnaryType : int { UNARYTYPE_UNDEFINED = 0, TANH = 1, GELU_ERF = 2, GELU_TANH = 3, RELU = 4, SILU = 5, SIGMOID = 6 };
 enum BinaryType : int { BINARYTYPE_UNDEFINED = 0, ADD = 1, MUL = 2 };
-enum class AsCacheMode : int { AsCacheDefault = 0, AsCacheQuantI8 = 1, AsCacheQuantU4 = 2 };
+// AsCacheQuantFP8 is an extension (not in the reference's enum): the fp8-e4m3 span cache B2_KV_FP8, head 128 only
+enum class AsCacheMode : int { AsCacheDefault = 0, AsCacheQuantI8 = 1, AsCacheQuantU4 = 2, AsCacheQuantFP8 = 3 };
 
 inline size_t SizeofType(DataType t) {
   switch (t) {

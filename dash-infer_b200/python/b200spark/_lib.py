@@ -48,6 +48,7 @@ ACT_NONE, ACT_TANH, ACT_GELU_ERF, ACT_GELU_TANH, ACT_RELU, ACT_SILU, ACT_SIGMOID
 ACT_SWIGLU = 100
 BIN_ADD, BIN_MUL = 1, 2
 KV_NONE, KV_I8, KV_U4 = 0, 1, 2
+KV_FP8 = 3  # extension (not a span::QuantMode value): fp8-e4m3 KV cache, head 128 only
 COMM_HANDLE_BYTES = 64
 
 

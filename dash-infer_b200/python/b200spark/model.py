@@ -15,7 +15,7 @@ from dataclasses import dataclass
 import torch
 
 from . import ops, quantize as PQ, tp as TP
-from ._lib import ACT_NONE, ACT_SILU, BIN_MUL, KV_I8, KV_NONE, KV_U4
+from ._lib import ACT_NONE, ACT_SILU, BIN_MUL, KV_FP8, KV_I8, KV_NONE, KV_U4
 
 
 @dataclass
@@ -39,7 +39,7 @@ QWEN2_72B = ModelConfig("Qwen2-72B", 8192, 64, 8, 29568, 80, 152064)
 QWEN2_05B = ModelConfig("Qwen2-0.5B", 896, 14, 2, 4864, 24, 151936, head=64)   # config C0: the CPU-parity anchor
 TINY = ModelConfig("tiny-2L", 512, 8, 2, 1024, 2, 1024)
 
-KV_MODES = {"none": KV_NONE, "bf16": KV_NONE, "i8": KV_I8, "u4": KV_U4}
+KV_MODES = {"none": KV_NONE, "bf16": KV_NONE, "i8": KV_I8, "u4": KV_U4, "fp8": KV_FP8}
 
 
 _DT = torch.bfloat16  # the model dtype FT while a DecodeStack is being built (DecodeStack(dtype=...): bf16 or fp16)

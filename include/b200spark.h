@@ -63,6 +63,10 @@ enum { B2_BIN_ADD = 1, B2_BIN_MUL = 2 };
 enum { B2_ACT_SWIGLU = 100 };
 /* span::QuantMode (span_attn.h:41-48) */
 enum { B2_KV_NONE = 0, B2_KV_I8 = 1, B2_KV_U4 = 2 };
+/* extension (not a span::QuantMode value): fp8-e4m3fn KV cache, head 128 only.  Same span layout as B2_KV_I8 (one byte
+ * per element, then {f32 zero, f32 scale} per row) with zero always 0: per (token, kv-head) row
+ * scale = max(max|x|, 1e-12) / 448, code = e4m3(x * (1 / scale)) rounded to nearest even, saturating (IEEE fp32 steps). */
+enum { B2_KV_FP8 = 3 };
 
 /* =====================================================================================
  * Weight-only quantized GEMV/GEMM:  C[M,N] = act(alpha * A[M,K] x dequant(W)[K,N] + bias) (+ residual)
@@ -163,14 +167,14 @@ int b2_gemm_wq_run_fp8(b2_gemm_wq_t handle, const void* A8, int64_t lda_bytes, c
 size_t b2_gemm_wq_algo_bytes(b2_gemm_wq_t handle, int M);
 
 /* =====================================================================================
- * SpanAttention: paged KV cache (spans) append + single-query attention, GQA, KV in FT / int8 / uint4.
+ * SpanAttention: paged KV cache (spans) append + single-query attention, GQA, KV in FT / int8 / uint4 / fp8-e4m3.
  * Span wire format (decoder_cache_append.cuh:33-92): [n_groups, span_len, head_size] of QT followed,
- * for I8/U4, by [n_groups, span_len] of {float zero, float scale}.
+ * for I8/U4/FP8, by [n_groups, span_len] of {float zero, float scale} (FP8: zero = 0).
  * Span tables: device arrays [batch, max_spans_per_seq] of device pointers.
  * ===================================================================================== */
 typedef struct {
   int32_t ft;                /* B2_DT_BF16 or B2_DT_F16: Q, the output, an unquantized cache (head 64: bf16 only) */
-  int32_t quant_mode;        /* B2_KV_NONE / B2_KV_I8 / B2_KV_U4 */
+  int32_t quant_mode;        /* B2_KV_NONE / B2_KV_I8 / B2_KV_U4 / B2_KV_FP8 (head 128 only) */
   int32_t n_heads;           /* query heads on this rank */
   int32_t n_groups;          /* kv heads on this rank; n_heads % n_groups == 0, n_heads/n_groups <= 16 */
   int32_t head_size;         /* 128 */
@@ -187,7 +191,8 @@ size_t b2_span_bytes(const b2_span_cfg* cfg);
  *   old_lens [batch] int32 device: tokens already cached (= write position)
  * rope: optional fused rotary (NeoX rotate-half over rotary_dim, position = old_lens[b]); pass NULL
  * when the graph has a separate Rotary op.  Quantised modes follow QuantParam<I8/U4>::Builder
- * (span-attention/src/cache_quant/impl_i8.cuh:106-140, impl_u4.cuh:146-182) with IEEE division. */
+ * (span-attention/src/cache_quant/impl_i8.cuh:106-140, impl_u4.cuh:146-182) with IEEE division; B2_KV_FP8 quantizes as
+ * described at its enum. */
 typedef struct {
   float base;          /* e.g. 1e6 for Qwen2 */
   int32_t rotary_dim;  /* <= head_size, even */
