@@ -16,6 +16,7 @@ int launch_failed(const char* what);  // returns B2_OK or B2_ERR_CUDA after chec
 bool pdl_enabled();
 int sm_count();
 int max_smem_optin();
+int env_int(const char* name, int dflt);  // integer value of environment variable `name`, dflt if unset
 
 #define B2_CUDA_TRY(expr)                         \
   do {                                            \

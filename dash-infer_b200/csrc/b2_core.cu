@@ -1,5 +1,6 @@
 // b200spark — library plumbing: status strings, last-error text, device queries, PDL switch.
 #include <cstdio>
+#include <cstdlib>
 #include <cstring>
 
 #include "b2_common.cuh"
@@ -40,6 +41,11 @@ int max_smem_optin() {
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&v, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
   return v;
+}
+
+int env_int(const char* name, int dflt) {
+  const char* v = getenv(name);
+  return v ? atoi(v) : dflt;
 }
 
 }  // namespace b2

@@ -47,7 +47,7 @@ __global__ void __launch_bounds__(256) rmsnorm_kernel(__nv_bfloat16* __restrict_
 //   scale[r] = max(|x[r,:]|, tiny) / 448 ;  y = e4m3(x / scale) (round to nearest even, saturating)
 // optional fused RMSNorm (gamma != NULL): x is first normalised exactly like rmsnorm_kernel (result rounded to bf16).
 // Layout of y ("b2 fp8 activation layout"): inside every aligned group of 8 k the bytes hold k = (0,2,4,6,1,3,5,7) — the
-// order in which the int4 weight image yields its nibbles, so the GEMM's dequant needs no final byte shuffle (a dot product
+// order in which the int4 weight image yields its nibbles (the in-word k order, wq_gemm_shared.cuh), so the GEMM's dequant needs no final byte shuffle (a dot product
 // is invariant under a common permutation of k).  tile_sums[r][kt] = sum of the QUANTIZED values of k-tile kt (64 k), the
 // zero-point term of the affine dequantisation (exact in fp32: multiples of 2^-9 below 2^15).
 __global__ void __launch_bounds__(256) quant_fp8_kernel(uint8_t* __restrict__ y, float* __restrict__ scale, float* __restrict__ tile_sums,

@@ -74,9 +74,7 @@ struct GemmParams {
 
 template <int WBITS>
 struct WTraits {
-  static constexpr int LB = WBITS == 4 ? 16 : (WBITS == 8 ? 32 : 64);  // bytes per lane per k-tile
-  static constexpr int NCH = LB / 16;                                   // 16B chunks per lane per k-tile
-  static constexpr int TILE_BYTES = kWarps * 32 * LB;                   // 4K / 8K / 16K
+  static constexpr int TILE_BYTES = Image<WBITS>::kTileBytes;
   static constexpr int TPS = kStageBytes / TILE_BYTES > 0 ? kStageBytes / TILE_BYTES : 1;  // tiles per stage
   static constexpr int STAGE_BYTES = TPS * TILE_BYTES;
 };
@@ -131,7 +129,7 @@ __device__ __forceinline__ void tile_mma(float (&acc)[MT][4], uint32_t wtile, ui
   } else {
 #pragma unroll
     for (int u = 0; u < 2; ++u) {
-      const uint4 w0 = lds128(wtile + woff0 + u * 2048), w1 = lds128(wtile + woff1 + u * 2048);
+      const uint4 w0 = lds128(wtile + woff0 + u * Image<16>::kChunkBytes), w1 = lds128(wtile + woff1 + u * Image<16>::kChunkBytes);
 #pragma unroll
       for (int m = 0; m < MT; ++m) {
         Ft<H>::mma(acc[m], w0.x, w1.x, w0.y, w1.y, xb[m][u].x, xb[m][u].y);
@@ -256,8 +254,8 @@ __global__ void __launch_bounds__(kThreads) wq_gemm_kernel(const GemmParams p) {
   // this thread's rows (16*warp + g, +8) inside the [chunk][row ^ swz][16B] tile image
   const int wc = WBITS == 4 ? (t >> 1) : (WBITS == 8 ? t : 2 * t);
   const int wr = warp * 16 + g;
-  const uint32_t woff0 = wc * 2048 + ((wr ^ tile_swz(WBITS, wc)) << 4) + (WBITS == 4 ? 8 * (t & 1) : 0);
-  const uint32_t woff1 = wc * 2048 + (((wr + 8) ^ tile_swz(WBITS, wc)) << 4) + (WBITS == 4 ? 8 * (t & 1) : 0);
+  const uint32_t woff0 = Image<WBITS>::chunk_offset(wr, wc) + (WBITS == 4 ? 8 * (t & 1) : 0);
+  const uint32_t woff1 = Image<WBITS>::chunk_offset(wr + 8, wc) + (WBITS == 4 ? 8 * (t & 1) : 0);
   const uint32_t x_thr = smem_u32(xs) + g * XS + t * 32;
   const int XS8 = 8 * XS;
   int stage_i = 0;
@@ -734,81 +732,43 @@ __global__ void __launch_bounds__(kThreads) wq_gemm_kernel(const GemmParams p) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// init-time re-layout kernels (reference layouts -> tile image).  One thread per 32-bit word.
+// init-time re-layout (reference layouts -> tile image, wq_gemm_shared.cuh).  One thread per 32-bit word of the image:
+// word index -> (tile, chunk, stored row, word j) -> logical row / k run.  Sources: int4 [K, ceil(N/2)] (low nibble = even
+// column), int8 / uint8 [K, N] (int8 stored with the sign bit flipped: 128 + q), bf16 [K, N]; k >= K and n >= N pack as 0.
+// pair != 0: rows 0..63 of every 128-row tile come from q (gate), rows 64..127 from q2 (up).
 // ------------------------------------------------------------------------------------------------
-// One thread per 32-bit word of the image: word index -> (tile, chunk, stored row, word j) -> logical row/k.
-// pair != 0: rows 0..63 of every 128-row tile come from q (gate), rows 64..127 from q2 (up), both [K, N]
-__global__ void pack_w4_kernel(uint32_t* __restrict__ dst, const uint8_t* __restrict__ q, const uint8_t* __restrict__ q2, int pair,
-                               int K, int N, int KT, int NG) {
-  const int64_t total = (int64_t)NG * KT * 1024;
-  const int npack = (N + 1) / 2;
+template <int WBITS>
+__global__ void pack_image_kernel(uint32_t* __restrict__ dst, const void* __restrict__ q, const void* __restrict__ q2, int pair, int K,
+                                  int N, int KT, int NG, int is_signed) {
+  using I = Image<WBITS>;
+  const int64_t total = (int64_t)NG * KT * I::kTileWords;
+  const uint32_t flip = (WBITS == 8 && is_signed) ? 0x80u : 0u;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
     const int j = i & 3;
-    const int rs = (i >> 2) & 127;
-    const int c = (i >> 9) & 1;
-    const int64_t tile = i >> 10;
+    const int rs = (i >> 2) & (kBN - 1);
+    const int c = (i / (4 * kBN)) & (I::kChunks - 1);
+    const int64_t tile = i / I::kTileWords;
     const int kt = tile % KT, ng = tile / KT;
-    const int r = rs ^ tile_swz(4, c);
+    const int r = rs ^ I::swz(c);
     const int n = pair ? ng * 64 + (r & 63) : ng * kBN + r;
-    const uint8_t* qs = (pair && r >= 64) ? q2 : q;
+    const void* src = (pair && r >= 64) ? q2 : q;
     uint32_t word = 0;
-    for (int nb = 0; nb < 8; ++nb) {
-      const int k = kt * kBK + 32 * c + 8 * j + 2 * (nb & 3) + (nb >> 2);
+    for (int e = 0; e < I::kKPerWord; ++e) {  // k run of the word: even k in the low half, odd k in the high half
+      const int k = kt * kBK + I::kKPerChunk * c + I::kKPerWord * j + e;
       uint32_t v = 0;
       if (n < N && k < K) {
-        const uint8_t b = qs[(int64_t)k * npack + (n >> 1)];
-        v = (n & 1) ? (b >> 4) : (b & 0xF);
+        if (WBITS == 4) {
+          const uint8_t b = static_cast<const uint8_t*>(src)[(int64_t)k * ((N + 1) / 2) + (n >> 1)];
+          v = (n & 1) ? (b >> 4) : (b & 0xF);
+        } else if (WBITS == 8) {
+          v = static_cast<const uint8_t*>(src)[(int64_t)k * N + n];
+        } else {
+          v = static_cast<const uint16_t*>(src)[(int64_t)k * N + n];
+        }
       }
-      word |= v << (4 * nb);
+      word |= (v ^ flip) << (WBITS * ((e >> 1) + (e & 1) * I::kKPerWord / 2));
     }
-    dst[i] = (word << 3) | (word >> 29);
-  }
-}
-
-__global__ void pack_w8_kernel(uint32_t* __restrict__ dst, const uint8_t* __restrict__ q, const uint8_t* __restrict__ q2, int pair,
-                               int K, int N, int KT, int NG, int is_signed) {
-  const int64_t total = (int64_t)NG * KT * 2048;
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
-    const int j = i & 3;
-    const int rs = (i >> 2) & 127;
-    const int c = (i >> 9) & 3;
-    const int64_t tile = i >> 11;
-    const int kt = tile % KT, ng = tile / KT;
-    const int r = rs ^ tile_swz(8, c);
-    const int n = pair ? ng * 64 + (r & 63) : ng * kBN + r;
-    const uint8_t* qs = (pair && r >= 64) ? q2 : q;
-    uint32_t word = 0;
-    for (int b = 0; b < 4; ++b) {
-      const int kk = (b == 0) ? 0 : (b == 2 ? 1 : (b == 1 ? 2 : 3));  // bytes (b0,b2,b1,b3) hold k+0,1,2,3
-      const int k = kt * kBK + 16 * c + 4 * j + kk;
-      uint32_t v = is_signed ? 0x80u : 0u;
-      if (n < N && k < K) v = qs[(int64_t)k * N + n] ^ (is_signed ? 0x80u : 0u);
-      word |= v << (8 * b);
-    }
-    dst[i] = (word << 3) | (word >> 29);
-  }
-}
-
-__global__ void pack_w16_kernel(uint32_t* __restrict__ dst, const uint16_t* __restrict__ wsrc, const uint16_t* __restrict__ wsrc2,
-                                int pair, int K, int N, int KT, int NG) {
-  const int64_t total = (int64_t)NG * KT * 4096;
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
-    const int j = i & 3;
-    const int rs = (i >> 2) & 127;
-    const int c = (i >> 9) & 7;
-    const int64_t tile = i >> 12;
-    const int kt = tile % KT, ng = tile / KT;
-    const int r = rs ^ tile_swz(16, c);
-    const int n = pair ? ng * 64 + (r & 63) : ng * kBN + r;
-    const uint16_t* ws = (pair && r >= 64) ? wsrc2 : wsrc;
-    uint32_t word = 0;
-    for (int e = 0; e < 2; ++e) {
-      const int k = kt * kBK + 8 * c + 2 * j + e;
-      uint32_t v = 0;
-      if (n < N && k < K) v = ws[(int64_t)k * N + n];
-      word |= v << (16 * e);
-    }
-    dst[i] = word;
+    dst[i] = I::kRotated ? (word << 3) | (word >> 29) : word;
   }
 }
 
@@ -849,7 +809,7 @@ struct b2_gemm_wq {
   b2_gemm_wq_desc d;
   int Kp = 0, Np = 0, KT = 0, NG = 0, G = 1, group_tiles = 0;
   int group_k = 0;  // > 0: quantization group size that is not a multiple of 64 (params looked up per 8-k word)
-  size_t tile_bytes = 0, packed_bytes = 0;
+  size_t packed_bytes = 0;
   void* packed = nullptr;
   bool own_packed = false;
   float2* sz = nullptr;
@@ -863,29 +823,17 @@ struct b2_gemm_wq {
 
 typedef void (*gemm_kernel_t)(const GemmParams);
 
-template <int WBITS, bool GROUPED, bool H>
-static gemm_kernel_t pick_mt(int mt) {
-  switch (mt) {
-    case 1: return wq_gemm_kernel<WBITS, 1, GROUPED, H>;
-    default: return wq_gemm_kernel<WBITS, 2, GROUPED, H>;
-  }
-}
-template <bool H>
-static gemm_kernel_t pick_kernel_ft(int wbits, bool grouped, int mt) {
-  if (wbits == 4) return grouped ? pick_mt<4, true, H>(mt) : pick_mt<4, false, H>(mt);
-  if (wbits == 8) return grouped ? pick_mt<8, true, H>(mt) : pick_mt<8, false, H>(mt);
-  return pick_mt<16, false, H>(mt);
-}
+// bf16 weights carry no sub-channel params: one instantiation whatever `grouped` says
 static gemm_kernel_t pick_kernel(int wbits, bool grouped, int mt, bool fp16) {
-  return fp16 ? pick_kernel_ft<true>(wbits, grouped, mt) : pick_kernel_ft<false>(wbits, grouped, mt);
+  return with_wbits(wbits, [&](auto W) {
+    return with_flag(grouped, [&](auto G) {
+      return with_flag(mt == 1, [&](auto MT1) {
+        return with_flag(fp16, [&](auto H) { return wq_gemm_kernel<W, MT1 ? 1 : 2, G && W != 16, H>; });
+      });
+    });
+  });
 }
-static int stage_bytes_of(int wbits) { return wbits == 16 ? WTraits<16>::STAGE_BYTES : kStageBytes; }
-static int tile_bytes_of(int wbits) { return wbits == 4 ? WTraits<4>::TILE_BYTES : (wbits == 8 ? WTraits<8>::TILE_BYTES : WTraits<16>::TILE_BYTES); }
-
-static int env_int(const char* name, int dflt) {
-  const char* v = getenv(name);
-  return v ? atoi(v) : dflt;
-}
+static int stage_bytes_of(int wbits) { return with_wbits(wbits, [](auto W) { return WTraits<W>::STAGE_BYTES; }); }
 
 cudaError_t b2::raise_smem_limit(const void* kern, int smem) {
   static std::mutex mu;
@@ -914,7 +862,7 @@ static int make_plan(b2_gemm_wq* h, int mti) {
     return l;
   };
   int nst_log2 = log2_stages(ring_kb);
-  const int tps = kStageBytes / tile_bytes_of(h->d.wbits) > 0 ? kStageBytes / tile_bytes_of(h->d.wbits) : 1;
+  const int tps = with_wbits(h->d.wbits, [](auto W) { return WTraits<W>::TPS; });
   const int xq = gt > tps ? gt : tps;  // chunk granularity (gt and tps are powers of two)
   const int x_budget = env_int("B2_GEMM_XBYTES", 20 * 1024);
   // activation chunk: as many k-tiles as fit the budget, a multiple of the quant group
@@ -1024,8 +972,7 @@ int b2_gemm_wq_create(b2_gemm_wq_t* out, const b2_gemm_wq_desc* d) {
   h->group_tiles = (grouped && !general_groups) ? d->group_size / kBK : 0;
   h->group_k = general_groups ? d->group_size : 0;
   h->G = grouped ? (general_groups ? (d->K + d->group_size - 1) / d->group_size : h->Kp / d->group_size) : 1;
-  h->tile_bytes = tile_bytes_of(d->wbits);
-  h->packed_bytes = (size_t)h->NG * h->KT * h->tile_bytes;
+  h->packed_bytes = (size_t)h->NG * h->KT * with_wbits(d->wbits, [](auto W) { return Image<W>::kTileBytes; });
   cudaGetDevice(&h->device);
   cudaError_t e = cudaMalloc(&h->counters, sizeof(unsigned) * h->NG);
   if (e == cudaSuccess) e = cudaMemset(h->counters, 0, sizeof(unsigned) * h->NG);
@@ -1068,15 +1015,10 @@ static int prepare_impl(b2_gemm_wq_t h, const void* qdata, const void* scales, c
   const int threads = 256;
   const int64_t words = (int64_t)h->packed_bytes / 4;
   const int blocks = (int)((words + threads - 1) / threads > 65535 * 8 ? 65535 * 8 : (words + threads - 1) / threads);
-  if (d.wbits == 4)
-    pack_w4_kernel<<<blocks, threads, 0, stream>>>((uint32_t*)h->packed, (const uint8_t*)qdata, (const uint8_t*)qdata2, pair, d.K, d.N,
-                                                   h->KT, h->NG);
-  else if (d.wbits == 8)
-    pack_w8_kernel<<<blocks, threads, 0, stream>>>((uint32_t*)h->packed, (const uint8_t*)qdata, (const uint8_t*)qdata2, pair, d.K, d.N,
-                                                   h->KT, h->NG, d.qtype == B2_DT_I8);
-  else
-    pack_w16_kernel<<<blocks, threads, 0, stream>>>((uint32_t*)h->packed, (const uint16_t*)qdata, (const uint16_t*)qdata2, pair, d.K,
-                                                    d.N, h->KT, h->NG);
+  with_wbits(d.wbits, [&](auto W) {
+    pack_image_kernel<W><<<blocks, threads, 0, stream>>>((uint32_t*)h->packed, qdata, qdata2, pair, d.K, d.N, h->KT, h->NG,
+                                                         d.qtype == B2_DT_I8);
+  });
   if (int st = launch_failed("pack_weights")) return st;
   if (d.wbits != 16) {
     if (!h->sz || !h->own_sz) {
@@ -1134,8 +1076,8 @@ static bool use_tc(const b2_gemm_wq* h, int M) {
   return M >= kTcMinM && (h->group_tiles == 0 || h->d.wbits == 4);
 }
 
-static int make_tc_plan(b2_gemm_wq* h) {
-  if (h->tc_S > 0) return B2_OK;
+static void make_tc_plan(b2_gemm_wq* h) {
+  if (h->tc_S > 0) return;
   const int ctas = env_int("B2_GEMM_TC_CTAS_PER_SM", 1);
   auto split_for = [&](int slots, int smax) {
     int S = slots / h->NG;
@@ -1144,15 +1086,49 @@ static int make_tc_plan(b2_gemm_wq* h) {
     return S < 1 ? 1 : S;
   };
   h->tc_S = split_for(ctas * sm_count(), env_int("B2_GEMM_TC_MAX_SPLIT", 6));
+}
+
+// workspace of the wgmma path: the split-K partial tiles of one launch (kTcMaxM rows)
+static size_t tc_workspace_bytes(b2_gemm_wq* h) {
+  make_tc_plan(h);
+  return h->tc_S <= 1 ? 16 : (size_t)h->NG * h->tc_S * kTcMaxM * kBN * sizeof(float) + 16;
+}
+
+// The wgmma kernel over M rows, kTcMaxM per launch.  p holds the caller's operands for row 0 (A, C, residual and the per-row
+// fp8 / RMSNorm arrays, offset here for every launch); the image, its params and the split-K plan come from the handle.
+static int run_tc(b2_gemm_wq* h, TcParams p, int M, cudaStream_t stream) {
+  make_tc_plan(h);
+  if (h->tc_S > 1 && !p.ws) return B2_ERR_PARAM;
+  p.packed = (const uint8_t*)h->packed; p.sz = h->sz; p.counters = h->counters;
+  p.N = h->d.N; p.K = h->d.K; p.Np = h->Np; p.KT = h->KT; p.NG = h->NG; p.S = h->tc_S;
+  const int64_t a_row = p.a_scale ? p.lda : 2 * p.lda;  // bytes per activation row (fp8: lda counts bytes)
+  for (int m0 = 0; m0 < M; m0 += kTcMaxM) {
+    TcParams q = p;
+    q.M = (M - m0) > kTcMaxM ? kTcMaxM : (M - m0);
+    q.A = reinterpret_cast<const __nv_bfloat16*>(reinterpret_cast<const uint8_t*>(p.A) + m0 * a_row);
+    q.C = p.C + (int64_t)m0 * p.ldc;
+    if (p.residual) q.residual = p.residual + (int64_t)m0 * p.ldc;
+    if (p.a_scale) {
+      q.a_scale = p.a_scale + m0;
+      q.tile_sums = p.tile_sums + (size_t)m0 * p.KT;
+    }
+    if (p.norm_sumsq) q.norm_sumsq = p.norm_sumsq + m0;
+    if (p.xg_out) {
+      q.sumsq_out = p.sumsq_out + m0;
+      q.xg_out = p.xg_out + (int64_t)m0 * p.ldxg;
+    }
+    cudaError_t e = tc_launch(h->d.wbits, h->d.ft == B2_DT_F16, q, stream);
+    if (e != cudaSuccess) {
+      set_last_error(p.a_scale ? "wq_gemm_tc (fp8) launch" : "wq_gemm_tc launch", e);
+      return B2_ERR_CUDA;
+    }
+  }
   return B2_OK;
 }
 
 size_t b2_gemm_wq_workspace_bytes(b2_gemm_wq_t h, int M) {
   if (!h || M <= 0) return 0;
-  if (use_tc(h, M)) {
-    if (make_tc_plan(h) != B2_OK) return 0;
-    return h->tc_S <= 1 ? 16 : (size_t)h->NG * h->tc_S * kTcMaxM * kBN * sizeof(float) + 16;
-  }
+  if (use_tc(h, M)) return tc_workspace_bytes(h);
   const int mc = M > kGemvMaxM ? kGemvMaxM : M;
   const int mti = mt_index_for(mc);
   if (make_plan(h, mti) != B2_OK) return 0;
@@ -1201,28 +1177,16 @@ int b2_gemm_wq_run_fp8(b2_gemm_wq_t h, const void* A8, int64_t lda_bytes, const 
   if (activation != B2_ACT_SWIGLU && (activation < 0 || activation > B2_ACT_SIGMOID)) return B2_ERR_PARAM;
   if (h->pair && (bias || residual)) return B2_ERR_UNSUPPORTED;
   if ((reinterpret_cast<uintptr_t>(A8) & 15) || (lda_bytes % 16) != 0 || lda_bytes < h->d.K) return B2_ERR_UNSUPPORTED;
-  if (int st = make_tc_plan(h)) return st;
-  const size_t need = h->tc_S <= 1 ? 16 : (size_t)h->NG * h->tc_S * kTcMaxM * kBN * sizeof(float) + 16;
-  if (workspace_bytes < need || (h->tc_S > 1 && !workspace)) return B2_ERR_PARAM;
-  for (int m0 = 0; m0 < M; m0 += kTcMaxM) {
-    TcLaunch a;
-    a.packed = (const uint8_t*)h->packed; a.sz = h->sz;
-    a.A = reinterpret_cast<const __nv_bfloat16*>((const uint8_t*)A8 + (int64_t)m0 * lda_bytes); a.lda = lda_bytes;
-    a.C = (__nv_bfloat16*)C + (int64_t)m0 * ldc; a.ldc = ldc;
-    a.bias = (const __nv_bfloat16*)bias;
-    a.residual = residual ? (const __nv_bfloat16*)residual + (int64_t)m0 * ldc : nullptr;
-    a.ws = (float*)workspace; a.counters = h->counters;
-    a.M = (M - m0) > kTcMaxM ? kTcMaxM : (M - m0);
-    a.N = h->d.N; a.K = h->d.K; a.Np = h->Np; a.KT = h->KT; a.NG = h->NG; a.S = h->tc_S;
-    a.act = activation; a.alpha = alpha;
-    a.a_scale = a_scale + m0; a.tile_sums = tile_sums + (size_t)m0 * h->KT;
-    cudaError_t e = tc_launch(4, a, (cudaStream_t)stream_);
-    if (e != cudaSuccess) {
-      set_last_error("wq_gemm_tc (fp8) launch", e);
-      return B2_ERR_CUDA;
-    }
-  }
-  return B2_OK;
+  if (workspace_bytes < tc_workspace_bytes(h)) return B2_ERR_PARAM;
+  TcParams p;
+  p.A = (const __nv_bfloat16*)A8; p.lda = lda_bytes;
+  p.C = (__nv_bfloat16*)C; p.ldc = ldc;
+  p.bias = (const __nv_bfloat16*)bias;
+  p.residual = (const __nv_bfloat16*)residual;
+  p.ws = (float*)workspace;
+  p.act = activation; p.alpha = alpha;
+  p.a_scale = a_scale; p.tile_sums = tile_sums;
+  return run_tc(h, p, M, (cudaStream_t)stream_);
 }
 
 int b2_gemm_wq_run_allreduce(b2_gemm_wq_t h, const void* A, int64_t lda, void* C, int64_t ldc, int M, const void* bias,
@@ -1275,57 +1239,43 @@ static int run_impl(b2_gemm_wq_t h, const void* A, int64_t lda, void* C, int64_t
   cudaStream_t stream = (cudaStream_t)stream_;
   const bool grouped = h->group_tiles > 0;
   if (use_tc(h, M) && !comm) {  // decode batches 17..: wgmma path, 64 rows per launch
-    if (int st = make_tc_plan(h)) return st;
-    const int tcs = h->tc_S;
-    if (tcs > 1 && !workspace) return B2_ERR_PARAM;
-    for (int m0 = 0; m0 < M; m0 += kTcMaxM) {
-      TcLaunch a;
-      a.fp16 = h->d.ft == B2_DT_F16;
-      a.packed = (const uint8_t*)h->packed; a.sz = h->sz;
-      a.A = (const __nv_bfloat16*)A + (int64_t)m0 * lda; a.lda = lda;
-      a.C = (__nv_bfloat16*)C + (int64_t)m0 * ldc; a.ldc = ldc;
-      a.bias = (const __nv_bfloat16*)bias;
-      a.residual = residual ? (const __nv_bfloat16*)residual + (int64_t)m0 * ldc : nullptr;
-      a.ws = (float*)workspace; a.counters = h->counters;
-      a.M = (M - m0) > kTcMaxM ? kTcMaxM : (M - m0);
-      a.N = h->d.N; a.K = h->d.K; a.Np = h->Np; a.KT = h->KT; a.NG = h->NG; a.S = tcs;
-      a.act = activation; a.alpha = alpha;
-      a.group_tiles = h->group_tiles;
-      a.group_k = h->group_k; a.ngroups = h->G;
-      if (fused) {
-        a.norm_ld = M;
-        if (fuse->norm_sumsq) {
-          a.norm_sumsq = fuse->norm_sumsq + m0; a.norm_parts = fuse->norm_parts;
-          a.norm_inv_hidden = 1.0f / (float)fuse->norm_hidden; a.norm_eps = fuse->norm_eps;
-        }
-        if (fuse->xg_out) {
-          a.sumsq_out = fuse->sumsq_out + m0;
-          a.xg_out = (__nv_bfloat16*)fuse->xg_out + (int64_t)m0 * fuse->ldxg;
-          a.gamma_out = (const __nv_bfloat16*)fuse->gamma_out; a.ldxg = fuse->ldxg;
-        }
+    TcParams p;
+    p.A = (const __nv_bfloat16*)A; p.lda = lda;
+    p.C = (__nv_bfloat16*)C; p.ldc = ldc;
+    p.bias = (const __nv_bfloat16*)bias;
+    p.residual = (const __nv_bfloat16*)residual;
+    p.ws = (float*)workspace;
+    p.act = activation; p.alpha = alpha;
+    p.group_tiles = h->group_tiles;
+    p.group_k = h->group_k; p.ngroups = h->G;
+    if (fused) {
+      p.norm_ld = M;
+      if (fuse->norm_sumsq) {
+        p.norm_sumsq = fuse->norm_sumsq; p.norm_parts = fuse->norm_parts;
+        p.norm_inv_hidden = 1.0f / (float)fuse->norm_hidden; p.norm_eps = fuse->norm_eps;
       }
-      cudaError_t e = tc_launch(h->d.wbits, a, stream);
-      if (e != cudaSuccess) {
-        set_last_error("wq_gemm_tc launch", e);
-        return B2_ERR_CUDA;
+      if (fuse->xg_out) {
+        p.sumsq_out = fuse->sumsq_out;
+        p.xg_out = (__nv_bfloat16*)fuse->xg_out;
+        p.gamma_out = (const __nv_bfloat16*)fuse->gamma_out; p.ldxg = fuse->ldxg;
       }
     }
-    return B2_OK;
+    return run_tc(h, p, M, stream);
   }
   // ---- dense bf16 weights at batches <= 16: no global split-K (wq_gemv2.cu), unless a fusion only the split-K kernel
   //      implements is asked for (fp16 handles: the split-K kernel)
   if (h->d.wbits == 16 && M <= kGemvMaxM && !fused && !comm && h->d.ft == B2_DT_BF16) {
-    Gemv2Launch a;
-    a.packed = (const uint8_t*)h->packed;
-    a.A = (const __nv_bfloat16*)A; a.lda = lda;
-    a.C = (__nv_bfloat16*)C; a.ldc = ldc;
-    a.bias = (const __nv_bfloat16*)bias;
-    a.residual = (const __nv_bfloat16*)residual;
-    a.M = M; a.N = h->d.N; a.K = h->d.K; a.KT = h->KT; a.NG = h->NG;
-    a.pair = h->pair; a.act = activation; a.alpha = alpha;
+    Gemv2Params p;
+    p.packed = (const uint8_t*)h->packed;
+    p.A = (const __nv_bfloat16*)A; p.lda = lda;
+    p.C = (__nv_bfloat16*)C; p.ldc = ldc;
+    p.bias = (const __nv_bfloat16*)bias;
+    p.residual = (const __nv_bfloat16*)residual;
+    p.M = M; p.N = h->d.N; p.K = h->d.K; p.KT = h->KT; p.NG = h->NG;
+    p.pair = h->pair ? 1 : 0; p.act = activation; p.alpha = alpha;
     Gemv2Plan pl;
-    if (gemv2_plan(a, &pl)) {
-      cudaError_t e = gemv2_launch(a, pl, stream);
+    if (gemv2_plan(p, &pl)) {
+      cudaError_t e = gemv2_launch(p, pl, stream);
       if (e != cudaSuccess) {
         set_last_error("wq_gemv2 launch", e);
         return B2_ERR_CUDA;

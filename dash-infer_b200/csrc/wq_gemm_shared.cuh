@@ -3,6 +3,8 @@
 #pragma once
 #include <cuda.h>  // CUtensorMap (types only; the encoder is fetched with cudaGetDriverEntryPoint)
 
+#include <type_traits>
+
 #include "b2_common.cuh"
 
 namespace b2 {
@@ -13,18 +15,47 @@ constexpr uint32_t kMask4 = 0x00780078u;   // nibble at mantissa bits 3..6 of ea
 constexpr uint32_t kMagic = 0x41804180u;   // bf16 16.0 in both halves: 16 + q exactly
 constexpr uint32_t kMagicHi = 0x43804380u; // bf16 256.0: 16 * (16 + q) exactly (hi nibble plane of W8)
 
-// ---- weight image layout (one image serves both kernels) ----
-// tile(ng, kt) = 128 output channels x 64 k, stored as [chunk c][row r ^ swz(c)][16 bytes]:
+// ---- weight image layout (one image serves every weight-only GEMM kernel) ----
+// image[n_group][k_tile] = tile of 128 output channels x 64 k, stored as [chunk c][row r ^ swz(c)][16 bytes]:
 //   W4 : 2 chunks, chunk = 32 k of one row as 4 words; word j nibble i <-> k = 32c+8j+2i, nibble i+4 <-> k+1
 //   W8 : 4 chunks, chunk = 16 k of one row as 4 words; word j bytes (b0,b2,b1,b3) <-> k = 16c+4j+(0,1,2,3)
-//   W16: 8 chunks, chunk = 8 k of one row, natural order
-// every word of W4/W8 is rotated left by 3 so that (w >> 4i) & 0x00780078 | magic yields two exact bf16 integers.
-__host__ __device__ __forceinline__ int tile_swz(int wbits, int c) {
-  return wbits == 4 ? 4 * (c & 1) : (wbits == 8 ? 2 * (c & 3) : 2 * ((c >> 1) & 3));
+//   W16: 8 chunks, chunk = 8 k of one row as 4 words; word j halves (h0,h1) <-> k = 8c+2j+(0,1)
+// i.e. the even k of a word fill its low half and the odd k its high half, each in k order.  Every word of W4/W8 is rotated
+// left by 3 so that (w >> 4i) & 0x00780078 | magic yields two exact bf16 integers.  A gate/up pair image (SwiGLU) takes rows
+// 0..63 of every tile from the gate weights and rows 64..127 from the up weights.
+template <int WBITS>
+struct Image {
+  static constexpr int kChunks = WBITS == 4 ? 2 : (WBITS == 8 ? 4 : 8);  // 16-byte chunks per tile row
+  static constexpr int kKPerChunk = kBK / kChunks;                       // 32 / 16 / 8
+  static constexpr int kKPerWord = kKPerChunk / 4;                       // 8 / 4 / 2
+  static constexpr int kChunkBytes = kBN * 16;                           // 2048
+  static constexpr int kTileBytes = kChunks * kChunkBytes;               // 4096 / 8192 / 16384
+  static constexpr int kTileWords = kTileBytes / 4;
+  static constexpr bool kRotated = WBITS != 16;                          // words stored rotated left by 3
+  __host__ __device__ __forceinline__ static int swz(int c) {
+    return WBITS == 4 ? 4 * (c & 1) : (WBITS == 8 ? 2 * (c & 3) : 2 * ((c >> 1) & 3));
+  }
+  // byte offset of (row, chunk c) inside a chunk of rows / inside a tile.  chunk_offset takes the row by reference: by value
+  // it is an argument when the helper is simplified on its own, the XOR's operands come out swapped, and ptxas schedules the
+  // mma.sync GEMV kernel's address arithmetic differently.
+  __host__ __device__ __forceinline__ static int row_offset(int row, int c) { return (row ^ swz(c)) << 4; }
+  __host__ __device__ __forceinline__ static int chunk_offset(const int& row, int c) { return c * kChunkBytes + ((row ^ swz(c)) << 4); }
+};
+
+// Runtime weight width / flag -> template argument: f(std::integral_constant<int, WBITS>) / f(std::bool_constant<b>)
+template <typename F>
+inline auto with_wbits(int wbits, F&& f) {
+  if (wbits == 4) return f(std::integral_constant<int, 4>{});
+  if (wbits == 8) return f(std::integral_constant<int, 8>{});
+  return f(std::integral_constant<int, 16>{});
+}
+template <typename F>
+inline auto with_flag(bool b, F&& f) {
+  return b ? f(std::true_type{}) : f(std::false_type{});
 }
 
 // wgmma kernel entry (wq_gemm_tc.cu)
-struct TcLaunch {
+struct TcParams {
   const uint8_t* packed;
   const float2* sz;
   const __nv_bfloat16* A;
@@ -38,11 +69,10 @@ struct TcLaunch {
   int M, N, K, Np, KT, NG, S;
   int act;
   float alpha;
-  const float* a_scale = nullptr;    // != NULL: A is fp8-e4m3 in the b2 fp8 activation layout (lda in bytes)
-  const float* tile_sums = nullptr;  // [M][KT] sums of the quantized activations per 64-k tile
-  int group_tiles = 0;               // > 0: sub-channel weights, k-tiles per quantization group (sz is [G][Np])
-  int group_k = 0, ngroups = 1;      // group_k > 0: group size not a multiple of 64 (a multiple of 8): params per 8-k word
-  bool fp16 = false;                 // activations / outputs / bias / residual are fp16 (else bf16)
+  // fp8 activations (A8 instantiation): A is fp8-e4m3 in the b2 fp8 activation layout (lda in bytes), per-token scale [M] and
+  // per-(row, 64-k tile) sums of the quantized values [M][KT]
+  const float* a_scale = nullptr;
+  const float* tile_sums = nullptr;
   // RMSNorm hand-off between GEMMs (b2_gemm_fuse, batches >= 17).  Consumer: A holds bf16(x * gamma); the result rows are
   // scaled by rsqrt(sum_p norm_sumsq[p * norm_ld + m] / hidden + eps).  Producer: besides C it writes xg = bf16(C * gamma_out)
   // and, per 128-channel tile, the sum of squares of every stored row.
@@ -53,9 +83,14 @@ struct TcLaunch {
   __nv_bfloat16* xg_out = nullptr;   // [M, ldxg]
   const __nv_bfloat16* gamma_out = nullptr;
   int64_t ldxg = 0;
+  int nm;                 // MMA N (batch columns): 64, or 32 when M <= 32 (half the tensor-pipe time and activation traffic)
+  int group_tiles = 0;    // > 0: sub-channel weights (GROUPED instantiation), k-tiles per quantization group; sz is [G][Np]
+  int group_k = 0, ngroups = 1;  // group_k > 0: a group size that is no multiple of 64 (a multiple of 8, >= 32): 8 consecutive
+                                 // k — one word of the image — never straddle a group, so the params are looked up per word
 };
+
 // GEMV for dense bf16 weights without global split-K (wq_gemv2.cu)
-struct Gemv2Launch {
+struct Gemv2Params {
   const uint8_t* packed;
   const __nv_bfloat16* A;
   int64_t lda;
@@ -64,20 +99,23 @@ struct Gemv2Launch {
   const __nv_bfloat16* bias;
   const __nv_bfloat16* residual;
   int M, N, K, KT, NG;
-  bool pair;
+  int cb_log2;      // log2(CB)
+  int xt;           // k-tiles per activation chunk (multiple of the stage: WK * kV2Q)
+  int nst_log2;     // log2(pipeline stages)
+  int pair;         // gate/up pair image (SwiGLU epilogue)
   int act;
   float alpha;
 };
 struct Gemv2Plan {
-  int cb_log2, xt, nst_log2, mt, grid, smem;
+  int mt, grid, smem;
 };
-bool gemv2_plan(const Gemv2Launch& a, Gemv2Plan* plan);   // false: use the split-K kernel
-cudaError_t gemv2_launch(const Gemv2Launch& a, const Gemv2Plan& plan, cudaStream_t stream);
+bool gemv2_plan(Gemv2Params& p, Gemv2Plan* plan);   // fills cb_log2, xt, nst_log2; false: use the split-K kernel
+cudaError_t gemv2_launch(const Gemv2Params& p, const Gemv2Plan& plan, cudaStream_t stream);
 
 constexpr int kGemvMaxM = 16;  // batch rows per launch of the mma.sync GEMV kernels (MT <= 2)
 constexpr int kTcMaxM = 64;    // batch rows per wgmma launch
-int tc_smem_bytes(int wbits);
-cudaError_t tc_launch(int wbits, const TcLaunch& a, cudaStream_t stream);
+// sets p.nm; fp16: activations / outputs / bias / residual are fp16 (else bf16)
+cudaError_t tc_launch(int wbits, bool fp16, TcParams p, cudaStream_t stream);
 
 // Raise a kernel's dynamic shared-memory opt-in to smem, never lower it: an instantiation is shared by handles whose plans
 // need different amounts, and a later handle with a smaller need must not lower the limit under an earlier one's launches.

@@ -30,7 +30,6 @@
 //                 instead of bf16 activations / outputs), the RMSNorm hand-off (row statistics + gamma-scaled copy out, 1/rms in).
 //
 // Roofline: HBM-bound up to M ~ 64 (~300 FLOP/B is the H100 tensor/HBM ridge); report both.
-#include <cstdlib>
 #include <type_traits>
 
 #include "b2_common.cuh"
@@ -116,9 +115,10 @@ __device__ __forceinline__ uint32_t lds32(uint32_t addr) {
   return v;
 }
 // 4 of the 8 int4 codes of one image word -> 4 e4m3 bytes (exact: 0..15 are e4m3 values): half 0 = codes of k (0,2,4,6),
-// half 1 = codes of k (1,3,5,7) of the word's 8 consecutive k — the byte order of the b2 fp8 activation layout (glue.cu
-// quant_fp8_kernel).  Byte-permute look-ups: codes 0..7 from one 8-byte table, 8..15 are 0x50 | (q & 7) from a second one,
-// the choice by a sign-replicating permute of bit 3 of every nibble.  qsh = 16 * half, msel = half ? 0xFBEA : 0xD9C8.
+// half 1 = codes of k (1,3,5,7) of the word's 8 consecutive k (the in-word k order of the image, wq_gemm_shared.cuh) — the
+// byte order of the b2 fp8 activation layout (glue.cu quant_fp8_kernel).  Byte-permute look-ups: codes 0..7 from one 8-byte
+// table, 8..15 are 0x50 | (q & 7) from a second one, the choice by a sign-replicating permute of bit 3 of every nibble.
+// qsh = 16 * half, msel = half ? 0xFBEA : 0xD9C8.
 __device__ __forceinline__ uint32_t nib4_to_e4m3(uint32_t w_rot3, uint32_t qsh, uint32_t msel) {
   const uint32_t word = __funnelshift_r(w_rot3, w_rot3, 3);  // the image stores words rotated left by 3 (bf16 path)
   const uint32_t sel = (word & 0x77777777u) >> qsh;
@@ -129,37 +129,6 @@ __device__ __forceinline__ uint32_t nib4_to_e4m3(uint32_t w_rot3, uint32_t qsh, 
   asm("lop3.b32 %0, %1, %2, %3, 0xD8;" : "=r"(r) : "r"(lo), "r"(hi), "r"(m));  // m ? hi : lo
   return r;
 }
-
-struct TcParams {
-  const uint8_t* packed;
-  const float2* sz;
-  const __nv_bfloat16* A;
-  int64_t lda;
-  __nv_bfloat16* C;
-  int64_t ldc;
-  const __nv_bfloat16* bias;
-  const __nv_bfloat16* residual;
-  float* ws;
-  unsigned* counters;
-  int M, N, K, Np, KT, NG, S;
-  int act;
-  float alpha;
-  // fp8 activations (A8 instantiation): per-token scale [M] and per-(row, 64-k tile) sums of the quantized values [M][KT]
-  const float* a_scale;
-  const float* tile_sums;
-  // RMSNorm hand-off (see TcLaunch)
-  const float* norm_sumsq;
-  int norm_parts, norm_ld;
-  float norm_inv_hidden, norm_eps;
-  float* sumsq_out;
-  __nv_bfloat16* xg_out;
-  const __nv_bfloat16* gamma_out;
-  int64_t ldxg;
-  int nm;           // MMA N (batch columns): 64, or 32 when M <= 32 (half the tensor-pipe time and activation traffic)
-  int group_tiles;  // GROUPED instantiation: k-tiles per quantization group; sz is [G][Np]
-  int group_k, ngroups;  // GROUPED with a group size that is no multiple of 64 (a multiple of 8, >= 32): 8 consecutive k — one
-                         // word of the image — never straddle a group, so the params are looked up per word
-};
 
 // MULTI: a CTA walks several units (more units than SMs); the single-unit instantiation folds the unit loop away
 // A8: fp8-e4m3 activations (b2_gemm_wq_run_fp8, int4 weights only): the int4 codes become exact e4m3 bytes, the MMAs are
@@ -172,8 +141,8 @@ struct TcParams {
 // H: fp16 activations / outputs (the exact-integer constants are 128 + q instead of 16 + q).
 template <int WBITS, bool MULTI, bool A8 = false, bool GROUPED = false, bool H = false>
 __global__ void __launch_bounds__(kTcThreads, 1) wq_gemm_tc_kernel(const TcParams p, const __grid_constant__ CUtensorMap amap) {
-  constexpr int TILE_BYTES = WBITS == 4 ? 4096 : (WBITS == 8 ? 8192 : 16384);
-  constexpr int NCH = WBITS == 4 ? 2 : (WBITS == 8 ? 4 : 8);  // 16B chunks per row per k-tile
+  using I = Image<WBITS>;
+  constexpr int TILE_BYTES = I::kTileBytes;
   constexpr int NSW = WBITS == 16 ? 4 : kTcNSW;               // weight stages (bf16: 32 KB each)
   // k-tiles per pipeline stage (k256 for W4, k128 for W8): one stage = 16 KB of weights per barrier round trip
   constexpr int TPS = WBITS == 4 ? 4 : 2;
@@ -326,11 +295,11 @@ __global__ void __launch_bounds__(kTcThreads, 1) wq_gemm_tc_kernel(const TcParam
     const float2 sz0 = (WBITS == 16 || GROUPED) ? make_float2(1.f, 0.f) : p.sz[ng * kBN + rr0];
     const float2 sz1 = (WBITS == 16 || GROUPED) ? make_float2(1.f, 0.f) : p.sz[ng * kBN + rr1];
     const uint32_t wring_u = smem_u32(wring), xring_u = smem_u32(xring);
-    uint32_t off0[NCH], off1[NCH];
+    uint32_t off0[I::kChunks], off1[I::kChunks];
 #pragma unroll
-    for (int c = 0; c < NCH; ++c) {
-      off0[c] = c * 2048 + ((rr0 ^ tile_swz(WBITS, c)) << 4);
-      off1[c] = c * 2048 + ((rr1 ^ tile_swz(WBITS, c)) << 4);
+    for (int c = 0; c < I::kChunks; ++c) {
+      off0[c] = I::chunk_offset(rr0, c);
+      off1[c] = I::chunk_offset(rr1, c);
     }
     // W4: the nibble of k pair 2t of a word; W8 / A8: which word of a 16-byte chunk, which half of it
     const uint32_t sh4 = 4 * t4, sh8 = 8 * (t4 & 1), qsh = 16 * (t4 & 1), msel = (t4 & 1) ? 0xFBEAu : 0xD9C8u;
@@ -662,10 +631,11 @@ __global__ void __launch_bounds__(kTcThreads, 1) wq_gemm_tc_kernel(const TcParam
     body(std::false_type{});
 }
 
-int tc_smem_bytes(int wbits) {
-  const int tps = wbits == 4 ? 4 : 2;
-  const int wstage = tps * (wbits == 4 ? 4096 : (wbits == 8 ? 8192 : 16384));
-  const int nsw = wbits == 16 ? 4 : kTcNSW;
+template <int WBITS>
+static int tc_smem_bytes() {
+  const int tps = WBITS == 4 ? 4 : 2;
+  const int wstage = tps * Image<WBITS>::kTileBytes;
+  const int nsw = WBITS == 16 ? 4 : kTcNSW;
   return 1024 + kTcNSX * tps * kTcXTile + nsw * wstage + kTcNM * 4 + 96 * 8 + 64;  // barrier block: 21 barriers, 64 scales
 }
 
@@ -680,68 +650,47 @@ EncodeTiledFn encode_tiled() {
   return fn;
 }
 
-cudaError_t tc_launch(int wbits, const TcLaunch& a, cudaStream_t stream) {
+cudaError_t tc_launch(int wbits, bool fp16, TcParams p, cudaStream_t stream) {
   EncodeTiledFn enc = encode_tiled();
   if (!enc) return cudaErrorNotSupported;
   // activations A[M, K] bf16, row stride lda: box = 64 k x 64 rows, 128B swizzle, zero fill outside [M, K]
   alignas(64) CUtensorMap amap;
-  const bool a8 = a.a_scale != nullptr;  // fp8 activations: bytes, 128 k per 128-byte swizzle row
-  const cuuint64_t gdim[2] = {(cuuint64_t)a.K, (cuuint64_t)a.M};
-  const cuuint64_t gstride[1] = {(cuuint64_t)a.lda * (a8 ? 1 : 2)};
+  const bool a8 = p.a_scale != nullptr;  // fp8 activations: bytes, 128 k per 128-byte swizzle row
+  const cuuint64_t gdim[2] = {(cuuint64_t)p.K, (cuuint64_t)p.M};
+  const cuuint64_t gstride[1] = {(cuuint64_t)p.lda * (a8 ? 1 : 2)};
   // batches <= 32 run the MMAs with N = 32 and load 32-row activation tiles (B2_GEMM_TC_N32=0: always 64)
-  static const int n32 = [] { const char* e = getenv("B2_GEMM_TC_N32"); return e ? atoi(e) : 1; }();
-  const int nm = (n32 && a.M <= 32) ? 32 : kTcNM;
-  const cuuint32_t box[2] = {(cuuint32_t)(a8 ? 2 * kBK : kBK), (cuuint32_t)nm};
+  static const int n32 = env_int("B2_GEMM_TC_N32", 1);
+  p.nm = (n32 && p.M <= 32) ? 32 : kTcNM;
+  const cuuint32_t box[2] = {(cuuint32_t)(a8 ? 2 * kBK : kBK), (cuuint32_t)p.nm};
   const cuuint32_t estr[2] = {1, 1};
-  if (enc(&amap, a8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<__nv_bfloat16*>(a.A), gdim, gstride, box, estr,
+  if (enc(&amap, a8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<__nv_bfloat16*>(p.A), gdim, gstride, box, estr,
           CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
           CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
     return cudaErrorInvalidValue;
 
-  TcParams p;
-  p.packed = a.packed; p.sz = a.sz; p.A = a.A; p.lda = a.lda; p.C = a.C; p.ldc = a.ldc; p.bias = a.bias; p.residual = a.residual;
-  p.ws = a.ws; p.counters = a.counters; p.M = a.M; p.N = a.N; p.K = a.K; p.Np = a.Np; p.KT = a.KT; p.NG = a.NG; p.S = a.S;
-  p.act = a.act; p.alpha = a.alpha;
-  p.a_scale = a.a_scale; p.tile_sums = a.tile_sums;
-  p.norm_sumsq = a.norm_sumsq; p.norm_parts = a.norm_parts; p.norm_ld = a.norm_ld; p.norm_inv_hidden = a.norm_inv_hidden;
-  p.norm_eps = a.norm_eps; p.sumsq_out = a.sumsq_out; p.xg_out = a.xg_out; p.gamma_out = a.gamma_out; p.ldxg = a.ldxg;
-  p.nm = nm; p.group_tiles = a.group_tiles; p.group_k = a.group_k; p.ngroups = a.ngroups;
   // persistent: one CTA per SM walks the (n-group, k-split) units; B2_GEMM_TC_PERSIST=0 launches one CTA per unit
-  static const int persist = [] { const char* e = getenv("B2_GEMM_TC_PERSIST"); return e ? atoi(e) : 1; }();
-  const int units = a.NG * a.S;
+  static const int persist = env_int("B2_GEMM_TC_PERSIST", 1);
+  const int units = p.NG * p.S;
   const int cap = sm_count();
   const int grid = (persist && units > cap) ? cap : units;
-  const bool multi = units > grid;
-  const size_t smem = (size_t)tc_smem_bytes(wbits);
-  auto go = [&](auto kern) {
-    const cudaError_t e = raise_smem_limit((const void*)kern, (int)smem);
-    return e != cudaSuccess ? e : launch(kern, dim3(grid), dim3(kTcThreads), smem, stream, true, p, amap);
-  };
-  const bool g = a.group_tiles > 0 || a.group_k > 0, h = a.fp16;
-  if (a8) {
-    if (wbits != 4 || h) return cudaErrorNotSupported;
-    return multi ? go(wq_gemm_tc_kernel<4, true, true>) : go(wq_gemm_tc_kernel<4, false, true>);
-  }
-  if (g && wbits != 4) return cudaErrorNotSupported;
-  if (wbits == 4) {
-    // (multi, grouped, fp16)
-    switch ((multi ? 4 : 0) | (g ? 2 : 0) | (h ? 1 : 0)) {
-      case 0: return go(wq_gemm_tc_kernel<4, false, false, false, false>);
-      case 1: return go(wq_gemm_tc_kernel<4, false, false, false, true>);
-      case 2: return go(wq_gemm_tc_kernel<4, false, false, true, false>);
-      case 3: return go(wq_gemm_tc_kernel<4, false, false, true, true>);
-      case 4: return go(wq_gemm_tc_kernel<4, true, false, false, false>);
-      case 5: return go(wq_gemm_tc_kernel<4, true, false, false, true>);
-      case 6: return go(wq_gemm_tc_kernel<4, true, false, true, false>);
-      default: return go(wq_gemm_tc_kernel<4, true, false, true, true>);
-    }
-  }
-  if (wbits == 16) {
-    if (h) return multi ? go(wq_gemm_tc_kernel<16, true, false, false, true>) : go(wq_gemm_tc_kernel<16, false, false, false, true>);
-    return multi ? go(wq_gemm_tc_kernel<16, true>) : go(wq_gemm_tc_kernel<16, false>);
-  }
-  if (h) return multi ? go(wq_gemm_tc_kernel<8, true, false, false, true>) : go(wq_gemm_tc_kernel<8, false, false, false, true>);
-  return multi ? go(wq_gemm_tc_kernel<8, true>) : go(wq_gemm_tc_kernel<8, false>);
+  const bool grouped = p.group_tiles > 0 || p.group_k > 0;
+  // instantiations: fp8 activations with int4 weights and bf16 outputs; sub-channel weights with int4 only
+  if ((a8 && (wbits != 4 || fp16)) || (grouped && !a8 && wbits != 4)) return cudaErrorNotSupported;
+  return with_wbits(wbits, [&](auto W) {
+    const size_t smem = (size_t)tc_smem_bytes<W>();
+    auto go = [&](auto kern) {
+      const cudaError_t e = raise_smem_limit((const void*)kern, (int)smem);
+      return e != cudaSuccess ? e : launch(kern, dim3(grid), dim3(kTcThreads), smem, stream, true, p, amap);
+    };
+    return with_flag(units > grid, [&](auto MULTI) {
+      if constexpr (W == 4) {
+        if (a8) return go(wq_gemm_tc_kernel<4, MULTI, true>);
+      }
+      return with_flag(grouped, [&](auto G) {
+        return with_flag(fp16, [&](auto H) { return go(wq_gemm_tc_kernel<W, MULTI, false, G && W == 4, H>); });
+      });
+    });
+  });
 }
 
 }  // namespace b2

@@ -24,35 +24,15 @@
 // 128-channel blocks of dense bf16 weights (lm_head) stream whole tiles.
 //
 // Roofline: HBM-bound; algorithmic bytes/launch = 2*K*N + 2*M*(K+N).
-#include <cstdlib>
-
 #include "b2_common.cuh"
 #include "wq_gemm_shared.cuh"
 
 namespace b2 {
 
+using V2Image = Image<16>;
 constexpr int kV2Warps = 8;
 constexpr int kV2Threads = kV2Warps * 32 + 32;  // + producer warp
 constexpr int kV2Q = 2;                         // k-tiles per quantum (= per warp per stage)
-constexpr int kV2Chunks = 8;                    // 16-byte chunks per row per k-tile (8 k of bf16 each)
-constexpr int kV2TileBytes = kBN * kV2Chunks * 16;  // one (128 n x 64 k) tile of the image
-
-struct Gemv2Params {
-  const uint8_t* packed;
-  const __nv_bfloat16* A;
-  int64_t lda;
-  __nv_bfloat16* C;
-  int64_t ldc;
-  const __nv_bfloat16* bias;
-  const __nv_bfloat16* residual;
-  int M, N, K, KT, NG;
-  int cb_log2;      // log2(CB)
-  int xt;           // k-tiles per activation chunk (multiple of the stage: WK * kV2Q)
-  int nst_log2;     // log2(pipeline stages)
-  int pair;         // gate/up pair image (SwiGLU epilogue)
-  int act;
-  float alpha;
-};
 
 __device__ __forceinline__ void v2_bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 
@@ -91,9 +71,9 @@ __global__ void __launch_bounds__(kV2Threads) wq_gemv2_kernel(const Gemv2Params 
   const int SUBS = kBN >> p.cb_log2;                                // CTAs per n-group == k-slices per CTA (WK)
   const int WK = SUBS, WN = CB >> 4;
   const uint32_t CS = (uint32_t)CB * 16u;                           // bytes per chunk of the CTA's sub-tile
-  const int sub_tile_bytes = kV2Chunks * (int)CS;                   // bytes per k-tile in shared memory
+  const int sub_tile_bytes = V2Image::kChunks * (int)CS;            // bytes per k-tile in shared memory
   const int stage_tiles = WK * kV2Q;
-  const int stage_bytes = stage_tiles * sub_tile_bytes;             // == kV2Q * kV2TileBytes
+  const int stage_bytes = stage_tiles * sub_tile_bytes;             // == kV2Q * V2Image::kTileBytes
   extern __shared__ __align__(128) uint8_t smem[];
   const int tid = threadIdx.x;
   const int warp = tid >> 5, lane = tid & 31;
@@ -164,8 +144,8 @@ __global__ void __launch_bounds__(kV2Threads) wq_gemv2_kernel(const Gemv2Params 
   const uint32_t w_ring = smem_u32(ring);
   const int wc = 2 * t;
   // the image stores row r of chunk c at r ^ swz(c): swz < 8 and the CTA's row runs are 16-aligned, so the XOR stays local
-  const uint32_t woff0 = wc * CS + ((lr0 ^ tile_swz(16, wc)) << 4);
-  const uint32_t woff1 = wc * CS + ((lr1 ^ tile_swz(16, wc)) << 4);
+  const uint32_t woff0 = wc * CS + V2Image::row_offset(lr0, wc);
+  const uint32_t woff1 = wc * CS + V2Image::row_offset(lr1, wc);
   const uint32_t x_thr = smem_u32(xs) + g * XS + t * 32;
   const int XS8 = 8 * XS;
   int stage_i = 0;
@@ -250,71 +230,62 @@ __global__ void __launch_bounds__(kV2Threads) wq_gemv2_kernel(const Gemv2Params 
   }
 }
 
-static int v2_env(const char* name, int dflt) {
-  const char* v = getenv(name);
-  return v ? atoi(v) : dflt;
-}
-
 // Channels per CTA: the largest of 128/64/32/16 whose grid still covers the SMs ~twice (more CTAs = more independent TMA
 // rings = more bytes in flight per SM); a pair image needs >= 32 (16 gate + 16 up rows per CTA).  B2_GEMV2=0: never.
-bool gemv2_plan(const Gemv2Launch& a, Gemv2Plan* pl) {
-  if (!v2_env("B2_GEMV2", 1) || a.M > kGemvMaxM) return false;
+bool gemv2_plan(Gemv2Params& p, Gemv2Plan* pl) {
+  if (!env_int("B2_GEMV2", 1) || p.M > kGemvMaxM) return false;
   const int sms = sm_count();
-  const int rows = a.NG * kBN;
-  const int want = v2_env("B2_GEMV2_MIN_CTAS", 2 * sms);
+  const int rows = p.NG * kBN;
+  const int want = env_int("B2_GEMV2_MIN_CTAS", 2 * sms);
   int cb = 128;
-  const int cb_min = a.pair ? 32 : 16;
-  const int forced = v2_env("B2_GEMV2_CB", 0);
+  const int cb_min = p.pair ? 32 : 16;
+  const int forced = env_int("B2_GEMV2_CB", 0);
   if (forced) cb = forced;
   else
     while (cb > cb_min && rows / cb < want) cb >>= 1;
   if (cb < cb_min || cb > 128 || (cb & (cb - 1))) return false;
-  if (!forced && rows / cb < v2_env("B2_GEMV2_FLOOR_CTAS", sms / 2)) return false;  // too small even at 16 channels: split-K kernel
+  if (!forced && rows / cb < env_int("B2_GEMV2_FLOOR_CTAS", sms / 2)) return false;  // too small even at 16 channels: split-K kernel
   const int wk = kBN / cb;
   const int stage_tiles = wk * kV2Q;
-  const int stage_bytes = kV2Q * kV2TileBytes;
-  const int ring_kb = v2_env("B2_GEMV2_RING_KB", 32);
+  const int stage_bytes = kV2Q * V2Image::kTileBytes;
+  const int ring_kb = env_int("B2_GEMV2_RING_KB", 32);
   int nst_log2 = 1;
   while ((2 << nst_log2) * stage_bytes <= ring_kb * 1024) ++nst_log2;
-  const int mt = a.M <= 8 ? 1 : 2;
+  const int mt = p.M <= 8 ? 1 : 2;
   const int MP = 8 * mt;
-  const int x_budget = v2_env("B2_GEMV2_XBYTES", 24 * 1024);
+  const int x_budget = env_int("B2_GEMV2_XBYTES", 24 * 1024);
   int xt = (x_budget / MP - 16) / 128;
   xt = xt / stage_tiles * stage_tiles;
   if (xt < stage_tiles) xt = stage_tiles;
-  const int kt_round = (a.KT + stage_tiles - 1) / stage_tiles * stage_tiles;
+  const int kt_round = (p.KT + stage_tiles - 1) / stage_tiles * stage_tiles;
   if (xt > kt_round) xt = kt_round;
-  pl->cb_log2 = cb == 128 ? 7 : (cb == 64 ? 6 : (cb == 32 ? 5 : 4));
-  pl->xt = xt;
-  pl->nst_log2 = nst_log2;
+  p.cb_log2 = cb == 128 ? 7 : (cb == 64 ? 6 : (cb == 32 ? 5 : 4));
+  p.xt = xt;
+  p.nst_log2 = nst_log2;
   pl->mt = mt;
-  pl->grid = a.NG * wk;
+  pl->grid = p.NG * wk;
   pl->smem = (1 << nst_log2) * stage_bytes + wk * MP * cb * 4 + MP * (xt * 128 + 16) + 16 + 8 + (1 << nst_log2) * 16 + 64;
   return pl->smem <= 200 * 1024;
 }
 
-cudaError_t gemv2_launch(const Gemv2Launch& a, const Gemv2Plan& pl, cudaStream_t stream) {
+cudaError_t gemv2_launch(const Gemv2Params& p, const Gemv2Plan& pl, cudaStream_t stream) {
   auto kern = pl.mt == 1 ? wq_gemv2_kernel<1> : wq_gemv2_kernel<2>;
   cudaError_t e = raise_smem_limit((const void*)kern, pl.smem);
   if (e != cudaSuccess) return e;
   // the tile image as a 4-D tensor of 8-byte elements: [tile (NG*KT)][chunk][half: rows 0-63 | 64-127][64 rows x 16 B = 128 el]
   EncodeTiledFn enc = encode_tiled();
   if (!enc) return cudaErrorNotSupported;
-  const int cb = 1 << pl.cb_log2, wk = kBN / cb;
-  const int run_rows = a.pair ? cb / 2 : (cb < 64 ? cb : 64);
+  const int cb = 1 << p.cb_log2, wk = kBN / cb;
+  const int run_rows = p.pair ? cb / 2 : (cb < 64 ? cb : 64);
   alignas(64) CUtensorMap wmap;
-  const cuuint64_t gdim[4] = {128, 2, (cuuint64_t)kV2Chunks, (cuuint64_t)a.NG * a.KT};
-  const cuuint64_t gstride[3] = {1024, 2048, (cuuint64_t)kV2Chunks * 2048};
-  const cuuint32_t box[4] = {(cuuint32_t)run_rows * 2, (cuuint32_t)((a.pair || cb == 128) ? 2 : 1), (cuuint32_t)kV2Chunks, (cuuint32_t)(wk * kV2Q)};
+  const cuuint64_t gdim[4] = {V2Image::kChunkBytes / 16, 2, (cuuint64_t)V2Image::kChunks, (cuuint64_t)p.NG * p.KT};
+  const cuuint64_t gstride[3] = {V2Image::kChunkBytes / 2, V2Image::kChunkBytes, V2Image::kTileBytes};
+  const cuuint32_t box[4] = {(cuuint32_t)run_rows * 2, (cuuint32_t)((p.pair || cb == 128) ? 2 : 1), (cuuint32_t)V2Image::kChunks,
+                             (cuuint32_t)(wk * kV2Q)};
   const cuuint32_t estr[4] = {1, 1, 1, 1};
-  if (enc(&wmap, CU_TENSOR_MAP_DATA_TYPE_UINT64, 4, const_cast<uint8_t*>(a.packed), gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+  if (enc(&wmap, CU_TENSOR_MAP_DATA_TYPE_UINT64, 4, const_cast<uint8_t*>(p.packed), gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
           CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
     return cudaErrorInvalidValue;
-  Gemv2Params p;
-  p.packed = a.packed; p.A = a.A; p.lda = a.lda; p.C = a.C; p.ldc = a.ldc; p.bias = a.bias; p.residual = a.residual;
-  p.M = a.M; p.N = a.N; p.K = a.K; p.KT = a.KT; p.NG = a.NG;
-  p.cb_log2 = pl.cb_log2; p.xt = pl.xt; p.nst_log2 = pl.nst_log2;
-  p.pair = a.pair ? 1 : 0; p.act = a.act; p.alpha = a.alpha;
   return launch(kern, dim3(pl.grid), dim3(kV2Threads), (size_t)pl.smem, stream, true, p, wmap);
 }
 
