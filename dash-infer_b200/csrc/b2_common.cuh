@@ -6,6 +6,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 #include "../../include/b200spark.h"
 
 namespace b2 {
@@ -17,6 +19,26 @@ bool pdl_enabled();
 int sm_count();
 int max_smem_optin();
 int env_int(const char* name, int dflt);  // integer value of environment variable `name`, dflt if unset
+
+inline int ilog2(int x) {  // ceil(log2(x)); the shift of a power-of-two span length
+  int s = 0;
+  while ((1 << s) < x) ++s;
+  return s;
+}
+
+// Runtime flag / KV-cache mode -> template argument: f(std::bool_constant<b>) / f(std::integral_constant<int, QM>).
+// Modes above B2_KV_FP8 are rejected before dispatch; they would run as B2_KV_U4.
+template <typename F>
+inline auto with_flag(bool b, F&& f) {
+  return b ? f(std::true_type{}) : f(std::false_type{});
+}
+template <typename F>
+inline auto with_kv_mode(int qm, F&& f) {
+  if (qm == B2_KV_NONE) return f(std::integral_constant<int, B2_KV_NONE>{});
+  if (qm == B2_KV_I8) return f(std::integral_constant<int, B2_KV_I8>{});
+  if (qm == B2_KV_FP8) return f(std::integral_constant<int, B2_KV_FP8>{});
+  return f(std::integral_constant<int, B2_KV_U4>{});
+}
 
 #define B2_CUDA_TRY(expr)                         \
   do {                                            \

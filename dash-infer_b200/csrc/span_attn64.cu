@@ -133,18 +133,12 @@ __global__ void __launch_bounds__(128) cache_append64_kernel(const Append64Param
   *reinterpret_cast<uint32_t*>(span + ((size_t)g * p.span_len + (pos & (p.span_len - 1))) * 64 + lane * 2) = pk;
 }
 
-static int ilog2_64(int x) {
-  int s = 0;
-  while ((1 << s) < x) ++s;
-  return s;
-}
-
 int span_attn64_run(const b2_span_cfg* c, void* out, const void* q, const void* const* k_spans, const void* const* v_spans,
                     const int32_t* lens, int batch, float qk_scale, cudaStream_t stream) {
   Attn64Params p;
   p.out = (__nv_bfloat16*)out; p.q = (const __nv_bfloat16*)q; p.k_spans = k_spans; p.v_spans = v_spans; p.lens = lens;
   p.n_heads = c->n_heads; p.n_groups = c->n_groups; p.hpg = c->n_heads / c->n_groups;
-  p.span_len = c->span_len; p.span_shift = ilog2_64(c->span_len); p.max_spans = c->max_spans_per_seq;
+  p.span_len = c->span_len; p.span_shift = ilog2(c->span_len); p.max_spans = c->max_spans_per_seq;
   p.scale_log2 = qk_scale * 1.4426950408889634f;
   cudaError_t e = launch(span_attn64_kernel, dim3(batch * c->n_groups), dim3(128), 0, stream, true, p);
   if (e != cudaSuccess) {
@@ -159,7 +153,7 @@ int span_append64_run(const b2_span_cfg* c, void* const* k_spans, void* const* v
   if (rope && rope->rotary_dim != 64 && rope->rotary_dim != 32) return B2_ERR_UNSUPPORTED;
   Append64Params p;
   p.k_spans = k_spans; p.v_spans = v_spans; p.q_out = (__nv_bfloat16*)q_out; p.qkv = (const __nv_bfloat16*)qkv; p.old_lens = old_lens;
-  p.batch = batch; p.n_heads = c->n_heads; p.n_groups = c->n_groups; p.span_len = c->span_len; p.span_shift = ilog2_64(c->span_len);
+  p.batch = batch; p.n_heads = c->n_heads; p.n_groups = c->n_groups; p.span_len = c->span_len; p.span_shift = ilog2(c->span_len);
   p.max_spans = c->max_spans_per_seq;
   p.rope = rope ? 1 : 0; p.rotary_dim = rope ? rope->rotary_dim : 0; p.log2_base = rope ? log2f(rope->base) : 0.f;
   const int warps = batch * (c->n_heads + 2 * c->n_groups);

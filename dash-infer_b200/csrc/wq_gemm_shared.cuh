@@ -42,16 +42,12 @@ struct Image {
   __host__ __device__ __forceinline__ static int chunk_offset(const int& row, int c) { return c * kChunkBytes + ((row ^ swz(c)) << 4); }
 };
 
-// Runtime weight width / flag -> template argument: f(std::integral_constant<int, WBITS>) / f(std::bool_constant<b>)
+// Runtime weight width -> template argument: f(std::integral_constant<int, WBITS>)  (flags: with_flag, b2_common.cuh)
 template <typename F>
 inline auto with_wbits(int wbits, F&& f) {
   if (wbits == 4) return f(std::integral_constant<int, 4>{});
   if (wbits == 8) return f(std::integral_constant<int, 8>{});
   return f(std::integral_constant<int, 16>{});
-}
-template <typename F>
-inline auto with_flag(bool b, F&& f) {
-  return b ? f(std::true_type{}) : f(std::false_type{});
 }
 
 // wgmma kernel entry (wq_gemm_tc.cu)

@@ -84,6 +84,15 @@ def test_span_bytes_equal_i8():
             assert lib.b2_span_attn_algo_bytes(C.byref(f8), 1000) == lib.b2_span_attn_algo_bytes(C.byref(i8), 1000) == 1000 * 2 * nG * 136
     f16 = _lib.SpanCfg(_lib.DT_F16, _lib.KV_FP8, 28, 4, 128, 128, 16, 0)
     assert lib.b2_span_bytes(C.byref(f16)) == F8.span_bytes(128, 4)
+    # every mode: span bytes against the oracles; attention reads each token row of a span once (2 = K and V)
+    oracle = {_lib.KV_NONE: lambda s, g: KV.span_bytes(KV.QUANT_NONE, s, g), _lib.KV_I8: lambda s, g: KV.span_bytes(KV.QUANT_I8, s, g),
+              _lib.KV_U4: lambda s, g: KV.span_bytes(KV.QUANT_U4, s, g), _lib.KV_FP8: F8.span_bytes}
+    for mode, ref in oracle.items():
+        for span in (16, 32, 64, 128):
+            for nG in (1, 2, 4, 8):
+                cfg = _lib.SpanCfg(_lib.DT_BF16, mode, 8 * nG, nG, 128, span, 16, 0)
+                assert lib.b2_span_bytes(C.byref(cfg)) == ref(span, nG)
+                assert lib.b2_span_attn_algo_bytes(C.byref(cfg), 1000) == 1000 * 2 * ref(span, nG) // span
 
 
 def test_header_value_matches_python(tmp_path):
