@@ -264,6 +264,27 @@ __global__ void lens_add_kernel(int32_t* lens, int batch, int delta) {
   if (i < batch) lens[i] += delta;
 }
 
+// greedy verification of a multi-token step: row t of sequence b predicted pred[b][t] after tokens[b][0..t]; the drafts
+// tokens[b][1..] are accepted while each equals the prediction before it
+__global__ void spec_accept_kernel(int32_t* accepted, int64_t* next_ids, int32_t* old_lens, int32_t* new_lens, int64_t* tokens,
+                                   const int64_t* pred, int batch, int q_len) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= batch) return;
+  const int64_t* tk = tokens + (size_t)b * q_len;
+  const int64_t* pr = pred + (size_t)b * q_len;
+  int n = 1;
+  while (n < q_len && tk[n] == pr[n - 1]) ++n;
+  const int64_t next = pr[n - 1];
+  accepted[b] = n;
+  if (next_ids) next_ids[b] = next;
+  tokens[(size_t)b * q_len] = next;  // the last emitted token of the next step
+  const int ol = old_lens[b] + n;
+  old_lens[b] = ol;
+  new_lens[b] = ol + q_len;
+}
+
 // vocab-split lm_head: pick the global winner among the ranks' (max, argmax) pairs; ties -> lowest rank == lowest vocab id
 __global__ void argmax_merge_kernel(int64_t* ids_out, const float* vals, const int64_t* ids, int nranks, int batch) {
   pdl_wait();
@@ -386,6 +407,15 @@ int b2_lens_add(int32_t* lens, int batch, int delta, void* stream) {
   if (!lens || batch <= 0) return B2_ERR_PARAM;
   B2_LAUNCH_CHECK("lens_add", launch(lens_add_kernel, dim3((batch + 127) / 128), dim3(128), 0, (cudaStream_t)stream, true, lens,
                                      batch, delta));
+  return B2_OK;
+}
+
+int b2_spec_accept(int32_t* accepted, int64_t* next_ids, int32_t* old_lens, int32_t* new_lens, int64_t* tokens, const int64_t* pred,
+                   int batch, int q_len, void* stream) {
+  if (!accepted || !old_lens || !new_lens || !tokens || !pred || batch <= 0) return B2_ERR_PARAM;
+  if (q_len < 1 || q_len > 16) return B2_ERR_LIMIT;
+  B2_LAUNCH_CHECK("spec_accept", launch(spec_accept_kernel, dim3((batch + 127) / 128), dim3(128), 0, (cudaStream_t)stream, true,
+                                        accepted, next_ids, old_lens, new_lens, tokens, pred, batch, q_len));
   return B2_OK;
 }
 

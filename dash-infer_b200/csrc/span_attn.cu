@@ -46,6 +46,15 @@ struct AttnParams {
   int nstage;
   float scale_log2;
 };
+// The multi-token form (span_attn_kernel<..., MT = true>) takes these fields on top.  They are not members of AttnParams
+// because a kernel parameter larger than 128 bytes changes the code of the single-token kernels.
+// q / out rows b*q_len + t; the 16 MMA rows hold the heads of one kv-group for tpb consecutive tokens of one sequence (a
+// row block), nrb row blocks per sequence; partial slots hold rstride = tpb * hpg rows.
+struct AttnTokParams : AttnParams {
+  int q_len, tpb, nrb, rstride;
+};
+template <bool MT>
+using AttnArgs = std::conditional_t<MT, AttnTokParams, AttnParams>;
 
 // ---- span format (one description for the writers, the tile loader, the tile math and the host sizes) ----
 // A span holds span_len tokens of one sequence for all n_groups kv-heads (the wire format of decoder_cache_append.cuh:33-92):
@@ -151,14 +160,19 @@ __device__ __forceinline__ void quad_sum(float& x) {
   x += __shfl_xor_sync(0xffffffffu, x, 1);
   x += __shfl_xor_sync(0xffffffffu, x, 2);
 }
-// running max of both rows after this tile (mx: the thread's tile max); corr rescales what was summed under the old max
-__device__ __forceinline__ void softmax_max(float (&mx)[2], float (&mrow)[2], float (&corr)[2]) {
+// running max of both rows after this tile (mx: the thread's tile max); corr rescales what was summed under the old max;
+// msub is what the tile's scores are reduced by before exp2
+template <bool MT>
+__device__ __forceinline__ void softmax_max(float (&mx)[2], float (&mrow)[2], float (&corr)[2], float (&msub)[2]) {
 #pragma unroll
   for (int r2 = 0; r2 < 2; ++r2) quad_max(mx[r2]);
 #pragma unroll
   for (int r2 = 0; r2 < 2; ++r2) {
-    const float mnew = fmaxf(mrow[r2], mx[r2]);  // finite: the warp's first token is always live
-    corr[r2] = exp2f(mrow[r2] - mnew);
+    // single token: finite, the warp's first token is always live.  Multi-token: a row whose limit lies before this
+    // warp's slice has seen no live token yet (mnew = -inf); it subtracts 0 so that corr and its probabilities are 0, not NaN
+    const float mnew = fmaxf(mrow[r2], mx[r2]);
+    msub[r2] = MT && mnew == -INFINITY ? 0.f : mnew;
+    corr[r2] = exp2f(mrow[r2] - msub[r2]);
     mrow[r2] = mnew;
   }
 }
@@ -179,10 +193,11 @@ __device__ __forceinline__ void softmax_sum(float (&psum)[2], float (&lrow)[2], 
 }
 
 // One 64-token tile of attention math for this warp's 16-token slice (cache in the 16-bit type FT: bf16, or fp16 when H).
-template <bool H>
-__device__ __forceinline__ void tile_compute_bf16(const uint8_t* st, int warp, int lane, int wtok, int tok1, float scale_log2,
-                                                  const uint32_t (&qa)[8][4], float (&o)[16][4], float (&mrow)[2],
-                                                  float (&lrow)[2]) {
+// Tokens >= tok1 are masked; multi-token (MT): rows gq and gq+8 are masked at their own limits lim[0] and lim[1] (<= tok1).
+template <bool H, bool MT>
+__device__ __forceinline__ void tile_compute_bf16(const uint8_t* st, int warp, int lane, int wtok, int tok1, const int (&lim)[2],
+                                                  float scale_log2, const uint32_t (&qa)[8][4], float (&o)[16][4],
+                                                  float (&mrow)[2], float (&lrow)[2]) {
   using T = KVTraits<B2_KV_NONE>;
   const int t = lane & 3;
   const uint32_t kb = smem_u32(st), vb = kb + T::TILE;
@@ -209,17 +224,17 @@ __device__ __forceinline__ void tile_compute_bf16(const uint8_t* st, int warp, i
 #pragma unroll
     for (int cc = 0; cc < 4; ++cc) {
       const int tok = wtok + nt * 8 + 2 * t + (cc & 1);
-      const float v = tok < tok1 ? sc[nt][cc] * scale_log2 : -INFINITY;
+      const float v = tok < (MT ? lim[cc >> 1] : tok1) ? sc[nt][cc] * scale_log2 : -INFINITY;
       sc[nt][cc] = v;
       mx[cc >> 1] = fmaxf(mx[cc >> 1], v);
     }
-  float corr[2], psum[2] = {0.f, 0.f};
-  softmax_max(mx, mrow, corr);
+  float corr[2], psum[2] = {0.f, 0.f}, msub[2];
+  softmax_max<MT>(mx, mrow, corr, msub);
 #pragma unroll
   for (int nt = 0; nt < 2; ++nt)
 #pragma unroll
     for (int cc = 0; cc < 4; ++cc) {
-      const float pv = exp2f(sc[nt][cc] - mrow[cc >> 1]);
+      const float pv = exp2f(sc[nt][cc] - msub[cc >> 1]);
       sc[nt][cc] = pv;
       psum[cc >> 1] += pv;
     }
@@ -266,10 +281,10 @@ __device__ __forceinline__ uint32_t e4m3x2_to_f16x2(uint32_t w) {
   return d;
 }
 
-template <int QM>
-__device__ __forceinline__ void tile_compute_q(const uint8_t* st, int warp, int lane, int wtok, int tok1, float scale_log2,
-                                               const uint32_t (&qa)[8][4], const float (&sq)[2], float (&o)[16][4],
-                                               float (&mrow)[2], float (&lrow)[2], float (&cacc)[2]) {
+template <int QM, bool MT>
+__device__ __forceinline__ void tile_compute_q(const uint8_t* st, int warp, int lane, int wtok, int tok1, const int (&lim)[2],
+                                               float scale_log2, const uint32_t (&qa)[8][4], const float (&sq)[2],
+                                               float (&o)[16][4], float (&mrow)[2], float (&lrow)[2], float (&cacc)[2]) {
   using T = KVTraits<QM>;
   constexpr float BIAS = QM == B2_KV_I8 ? 1152.f : 1024.f;
   const int gq = lane >> 2, t = lane & 3;
@@ -331,20 +346,20 @@ __device__ __forceinline__ void tile_compute_q(const uint8_t* st, int warp, int 
       const int tok = wtok + nt * 8 + 2 * t + (cc & 1);
       const float kz = (cc & 1) ? kp.z : kp.x, ksc = (cc & 1) ? kp.w : kp.y;
       const float raw = T::kZeroPoint ? ksc * (sc[nt][cc] - (BIAS + kz) * sq[cc >> 1]) : ksc * sc[nt][cc];
-      const float v = tok < tok1 ? raw * scale_log2 : -INFINITY;
+      const float v = tok < (MT ? lim[cc >> 1] : tok1) ? raw * scale_log2 : -INFINITY;
       sc[nt][cc] = v;
       mx[cc >> 1] = fmaxf(mx[cc >> 1], v);
     }
   }
-  float corr[2], psum[2] = {0.f, 0.f}, csum[2] = {0.f, 0.f};
-  softmax_max(mx, mrow, corr);
+  float corr[2], psum[2] = {0.f, 0.f}, csum[2] = {0.f, 0.f}, msub[2];
+  softmax_max<MT>(mx, mrow, corr, msub);
   uint32_t pa[4];
 #pragma unroll
   for (int nt = 0; nt < 2; ++nt) {
     float pq[4];
 #pragma unroll
     for (int cc = 0; cc < 4; ++cc) {
-      const float pv = exp2f(sc[nt][cc] - mrow[cc >> 1]);
+      const float pv = exp2f(sc[nt][cc] - msub[cc >> 1]);
       psum[cc >> 1] += pv;
       pq[cc] = pv * vs[nt][cc & 1];  // fold the V scale into the probability
     }
@@ -398,14 +413,18 @@ __device__ __forceinline__ void tile_compute_q(const uint8_t* st, int warp, int 
 // merge of up to 8 sources (every level-1 group, most final merges) is ONE round trip; longer lists take one more per 8.
 // FINAL writes softmax-normalised bf16 rows of `out`; otherwise the merged, still unnormalised partial goes to slot
 // `dst_slot` of (dst_o, dst_ml).  s_w: shared scratch [kMergeMaxSrc][16] floats (weights), s_ML: [16][2].
+// A slot holds `hpg` rows.  Multi-token (MT): a slot holds `hpg` = rstride rows of which the first `rows` are live, and
+// row r of the output is head r % qh of token r / qh, tokens tok_stride elements apart.
 constexpr int kMergeMaxSrc = 96;  // sources of one merge call (final level: ceil(pieces / kMergeFan)); more -> looped M pass
-template <bool FINAL, bool H>
+template <bool FINAL, bool H, bool MT = false>
 __device__ __forceinline__ void merge_partials(const float* src_o, const float* src_ml, int slot0, int stride2, int par0, int n,
                                                int hpg, __nv_bfloat16* out_rows, float* dst_o, float* dst_ml, int dst_slot,
-                                               float* s_w, float* s_ML) {
+                                               float* s_w, float* s_ML, int rows = 0, int qh = 0, int tok_stride = 0) {
   const int tid = threadIdx.x;
   auto slot_of = [&](int i) { return slot0 + i * stride2 + (i == 0 ? par0 : 0); };
-  const int nunits = hpg * 32;  // (row, float4) units
+  int R = hpg;  // rows merged
+  if constexpr (MT) R = rows;
+  const int nunits = R * 32;  // (row, float4) units
   // ---- request the first batch of rows and every (m, l) pair before waiting for anything
   float4 v[2][8];
 #pragma unroll
@@ -416,14 +435,14 @@ __device__ __forceinline__ void merge_partials(const float* src_o, const float* 
       v[uu][i] = (u < nunits && i < n) ? __ldcg(reinterpret_cast<const float4*>(src_o + ((size_t)slot_of(i) * hpg + (u >> 5)) * kHead) + (u & 31))
                                        : make_float4(0.f, 0.f, 0.f, 0.f);
   }
-  for (int k = tid; k < n * hpg; k += kAttnThreads) {  // k = i * hpg + r
-    const int i = k / hpg, r = k - i * hpg;
+  for (int k = tid; k < n * R; k += kAttnThreads) {  // k = i * R + r
+    const int i = k / R, r = k - i * R;
     const float2 ml = __ldcg(reinterpret_cast<const float2*>(src_ml + ((size_t)slot_of(i) * hpg + r) * 2));
     if (i < kMergeMaxSrc) { s_w[i * 16 + r] = ml.x; s_w[(kMergeMaxSrc + i) * 16 + r] = ml.y; }
   }
   __syncthreads();
   const int nn = min(n, kMergeMaxSrc);  // (n > kMergeMaxSrc cannot happen: pieces <= grid, fan-in 8, grid <= 8 * kMergeMaxSrc)
-  if (tid < hpg) {  // per row: global max, weights, denominator (fixed source order)
+  if (tid < R) {  // per row: global max, weights, denominator (fixed source order)
     float M = -INFINITY;
     for (int i = 0; i < nn; ++i) M = fmaxf(M, s_w[i * 16 + tid]);
     float L = 0.f;
@@ -444,7 +463,7 @@ __device__ __forceinline__ void merge_partials(const float* src_o, const float* 
     acc[uu] = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
-      const float w = (i < nn && r < hpg) ? s_w[i * 16 + r] : 0.f;
+      const float w = (i < nn && r < R) ? s_w[i * 16 + r] : 0.f;
       acc[uu].x += w * v[uu][i].x; acc[uu].y += w * v[uu][i].y; acc[uu].z += w * v[uu][i].z; acc[uu].w += w * v[uu][i].w;
     }
   }
@@ -462,15 +481,15 @@ __device__ __forceinline__ void merge_partials(const float* src_o, const float* 
       const int r = (tid + uu * kAttnThreads) >> 5;
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
-        const float w = (i0 + i < nn && r < hpg) ? s_w[(i0 + i) * 16 + r] : 0.f;
+        const float w = (i0 + i < nn && r < R) ? s_w[(i0 + i) * 16 + r] : 0.f;
         acc[uu].x += w * v[uu][i].x; acc[uu].y += w * v[uu][i].y; acc[uu].z += w * v[uu][i].z; acc[uu].w += w * v[uu][i].w;
       }
     }
   }
-  // hpg <= 16: up to 512 units, two per thread cover 8 rows; the remaining rows (hpg > 8) take a second sweep
+  // R <= 16: up to 512 units, two per thread cover 8 rows; the remaining rows (R > 8) take a second sweep
   for (int sweep = 0; sweep < 2; ++sweep) {
     if (sweep == 1) {
-      if (hpg <= 8) break;
+      if (R <= 8) break;
 #pragma unroll
       for (int uu = 0; uu < 2; ++uu) {
         const int u = tid + (uu + 2) * kAttnThreads;
@@ -491,8 +510,12 @@ __device__ __forceinline__ void merge_partials(const float* src_o, const float* 
       const int r = u >> 5, c4 = u & 31;
       if (FINAL) {
         const float inv = 1.f / s_ML[r * 2 + 1];
-        *reinterpret_cast<uint2*>(out_rows + (size_t)r * kHead + c4 * 4) =
-            make_uint2(Ft<H>::pack(acc[uu].x * inv, acc[uu].y * inv), Ft<H>::pack(acc[uu].z * inv, acc[uu].w * inv));
+        if constexpr (MT)
+          *reinterpret_cast<uint2*>(out_rows + (size_t)(r / qh) * tok_stride + (size_t)(r % qh) * kHead + c4 * 4) =
+              make_uint2(Ft<H>::pack(acc[uu].x * inv, acc[uu].y * inv), Ft<H>::pack(acc[uu].z * inv, acc[uu].w * inv));
+        else
+          *reinterpret_cast<uint2*>(out_rows + (size_t)r * kHead + c4 * 4) =
+              make_uint2(Ft<H>::pack(acc[uu].x * inv, acc[uu].y * inv), Ft<H>::pack(acc[uu].z * inv, acc[uu].w * inv));
       } else {
         const size_t row = (size_t)dst_slot * hpg + r;
         *(reinterpret_cast<float4*>(dst_o + row * kHead) + c4) = acc[uu];
@@ -511,8 +534,25 @@ B2_TRACE_DECL(g_attn_tr)
 extern "C" int b2_debug_trace_attn(unsigned long long* host_out) { return (int)cudaMemcpyFromSymbol(host_out, g_attn_tr, sizeof(g_attn_tr)); }
 #endif
 
-template <int QM, bool H>
-__global__ void __launch_bounds__(kAttnThreads) span_attn_kernel(const AttnParams p) {
+// Multi-token form (MT): the work items are (sequence, row block, kv-head, tile).  Row block rb of sequence b holds
+// tokens rb*tpb .. min(q_len, (rb+1)*tpb) - 1; token t attends to the first lens[b] - q_len + t + 1 tokens, so the block
+// streams the tiles its last token sees and masks each row at its own limit.  The scheduler below treats each
+// (sequence, row block) as one item of length block_len: counters and partials are per (item, kv-head).
+// (Overloads rather than `MT ? :` expressions: the single-token kernels then compile to the code they had before.)
+__device__ __forceinline__ int n_items(const AttnParams& p) { return p.batch; }
+__device__ __forceinline__ int n_items(const AttnTokParams& p) { return p.batch * p.nrb; }
+__device__ __forceinline__ int item_len(const AttnParams& p, int b) { return p.lens[b]; }
+__device__ __forceinline__ int item_len(const AttnTokParams& p, int v) {
+  const int b = v / p.nrb, rb = v - b * p.nrb;
+  return p.lens[b] - p.q_len + min(p.q_len, (rb + 1) * p.tpb);
+}
+// offset of MMA row r of the row block starting at token qt0 of sequence b, kv-head g, in q and out
+__device__ __forceinline__ size_t tok_row(const AttnTokParams& p, int b, int qt0, int g, int r) {
+  return ((size_t)b * p.q_len + qt0 + r / p.hpg) * p.n_heads * kHead + ((size_t)g * p.hpg + r % p.hpg) * kHead;
+}
+
+template <int QM, bool H, bool MT = false>
+__global__ void __launch_bounds__(kAttnThreads) span_attn_kernel(const AttnArgs<MT> p) {
   using F = Ft<H>;  // the 16-bit type of Q, the output and an unquantized cache
   using T = KVTraits<QM>;
   extern __shared__ __align__(128) uint8_t smem[];
@@ -530,10 +570,11 @@ __global__ void __launch_bounds__(kAttnThreads) span_attn_kernel(const AttnParam
   if (tr0) B2_TR(g_attn_tr, 1);
 
   // ---------------- device-side work decomposition (ONE global round trip: the lengths) ----------------
+  // items: sequences, or (sequence, row block)s
   {
     int my_tiles = 0, my_max = 0;
-    for (int b = tid; b < p.batch; b += kAttnThreads) {
-      const int tl = (p.lens[b] + kTile - 1) / kTile;
+    for (int b = tid; b < n_items(p); b += kAttnThreads) {
+      const int tl = (item_len(p, b) + kTile - 1) / kTile;
       s_prefix[b] = tl;  // tile count for now; warp 0 turns it into the exclusive scan below
       my_tiles += tl;
       my_max = max(my_max, tl);
@@ -555,18 +596,18 @@ __global__ void __launch_bounds__(kAttnThreads) span_attn_kernel(const AttnParam
   if (lo >= hi) return;
   if (warp == 0) {  // exclusive scan of tiles*n_groups per sequence
     int carry = 0;
-    for (int b0 = 0; b0 < p.batch; b0 += 32) {
+    for (int b0 = 0; b0 < n_items(p); b0 += 32) {
       const int b = b0 + lane;
-      int v = b < p.batch ? s_prefix[b] * p.n_groups : 0, x = v;
+      int v = b < n_items(p) ? s_prefix[b] * p.n_groups : 0, x = v;
 #pragma unroll
       for (int o = 1; o < 32; o <<= 1) {
         const int y = __shfl_up_sync(0xffffffffu, x, o);
         if (lane >= o) x += y;
       }
-      if (b < p.batch) s_prefix[b] = carry + x - v;
+      if (b < n_items(p)) s_prefix[b] = carry + x - v;
       carry += __shfl_sync(0xffffffffu, x, 31);
     }
-    if (lane == 0) s_prefix[p.batch] = carry;
+    if (lane == 0) s_prefix[n_items(p)] = carry;
   }
   __syncthreads();
 
@@ -581,17 +622,19 @@ __global__ void __launch_bounds__(kAttnThreads) span_attn_kernel(const AttnParam
   int pos = lo;
   while (pos < hi) {
     // ---- locate (b, g, first tile) of the piece starting at flat index pos
-    int blo = 0, bhi = p.batch - 1;
+    int blo = 0, bhi = n_items(p) - 1;
     while (blo < bhi) {
       const int mid = (blo + bhi + 1) >> 1;
       if (s_prefix[mid] <= pos) blo = mid; else bhi = mid - 1;
     }
-    const int b = blo;
-    const int len = p.lens[b];
+    const int item = blo;
+    int b, len;  // the sequence, the tokens the item attends to
+    if constexpr (MT) { b = item / p.nrb; len = item_len(p, item); }
+    else { b = blo; len = p.lens[b]; }
     const int tiles_b = (len + kTile - 1) / kTile;
-    const int within = pos - s_prefix[b];
+    const int within = pos - s_prefix[item];
     const int g = within / tiles_b, t0 = within - g * tiles_b;
-    const int bg_start = s_prefix[b] + g * tiles_b, bg_end = bg_start + tiles_b;
+    const int bg_start = s_prefix[item] + g * tiles_b, bg_end = bg_start + tiles_b;
     const int pend = min(hi, bg_end);
     const int ntiles = pend - pos;
     const int tok0 = t0 * kTile;
@@ -600,6 +643,10 @@ __global__ void __launch_bounds__(kAttnThreads) span_attn_kernel(const AttnParam
     const int npieces = (bg_end - 1) / Tc - k0 + 1;
     const void* const* ktab = p.k_spans + (size_t)b * p.max_spans;
     const void* const* vtab = p.v_spans + (size_t)b * p.max_spans;
+    // multi-token: this row block's tokens qt0 .. qt0+ntok-1 sit in MMA rows 0 .. nrows-1 (row r: token qt0 + r / hpg,
+    // head r % hpg).  Row r sees the tokens before len - ntok + 1 + r / hpg (lim[] for the thread's rows gq and gq+8).
+    int nrows, rstride, qt0;  // live rows, rows of a partial slot (set below, next to the single-token kernel's first use of hpg)
+    int lim[2];
 
     // ---- start streaming: the piece's first nstage-1 tiles are requested NOW (span-table lookups + cp.async), so their
     //      HBM latency overlaps the load of the query rows below
@@ -619,23 +666,48 @@ __global__ void __launch_bounds__(kAttnThreads) span_attn_kernel(const AttnParam
       // [16][128] in the LAST ring stage: the only one the prefetch above does not write (it is first filled at iteration 0)
       __nv_bfloat16* qs = reinterpret_cast<__nv_bfloat16*>(smem + (p.nstage - 1) * T::STAGE);
       const __nv_bfloat16* qb = p.q + ((size_t)b * p.n_heads + (size_t)g * p.hpg) * kHead;
+      if constexpr (MT) {
+        qt0 = (item - b * p.nrb) * p.tpb;
+        const int ntok = min(p.tpb, p.q_len - qt0);
+        nrows = ntok * p.hpg;
+        rstride = p.rstride;
+#pragma unroll
+        for (int rr = 0; rr < 2; ++rr) {
+          const int r = gq + 8 * rr;
+          lim[rr] = r < nrows ? len - ntok + 1 + r / p.hpg : len;
+        }
+      } else {
+        nrows = rstride = p.hpg;
+      }
       if (QM != B2_KV_NONE) {
         for (int i = tid; i < 16 * (kHead / 8); i += kAttnThreads) {
           const int row = i >> 4;
-          *reinterpret_cast<uint4*>(qs + row * kHead + (i & 15) * 8) =
-              row < p.hpg ? *reinterpret_cast<const uint4*>(qb + row * kHead + (i & 15) * 8) : make_uint4(0, 0, 0, 0);
+          if constexpr (MT)
+            *reinterpret_cast<uint4*>(qs + row * kHead + (i & 15) * 8) =
+                row < nrows ? *reinterpret_cast<const uint4*>(p.q + tok_row(p, b, qt0, g, row) + (i & 15) * 8) : make_uint4(0, 0, 0, 0);
+          else
+            *reinterpret_cast<uint4*>(qs + row * kHead + (i & 15) * 8) =
+                row < p.hpg ? *reinterpret_cast<const uint4*>(qb + row * kHead + (i & 15) * 8) : make_uint4(0, 0, 0, 0);
         }
         __syncthreads();
       }
-      const bool r0 = gq < p.hpg, r1 = (gq + 8) < p.hpg;
+      const bool r0 = gq < nrows, r1 = (gq + 8) < nrows;
 #pragma unroll
       for (int ks = 0; ks < 8; ++ks) {
         if (QM == B2_KV_NONE) {  // natural d order: 32 independent 4-byte loads per thread straight from global memory
           const int d0 = 16 * ks + 2 * t;
-          qa[ks][0] = r0 ? *reinterpret_cast<const uint32_t*>(qb + gq * kHead + d0) : 0u;
-          qa[ks][1] = r1 ? *reinterpret_cast<const uint32_t*>(qb + (gq + 8) * kHead + d0) : 0u;
-          qa[ks][2] = r0 ? *reinterpret_cast<const uint32_t*>(qb + gq * kHead + d0 + 8) : 0u;
-          qa[ks][3] = r1 ? *reinterpret_cast<const uint32_t*>(qb + (gq + 8) * kHead + d0 + 8) : 0u;
+          if constexpr (MT) {
+            const __nv_bfloat16 *q0 = p.q + tok_row(p, b, qt0, g, gq), *q1 = p.q + tok_row(p, b, qt0, g, gq + 8);
+            qa[ks][0] = r0 ? *reinterpret_cast<const uint32_t*>(q0 + d0) : 0u;
+            qa[ks][1] = r1 ? *reinterpret_cast<const uint32_t*>(q1 + d0) : 0u;
+            qa[ks][2] = r0 ? *reinterpret_cast<const uint32_t*>(q0 + d0 + 8) : 0u;
+            qa[ks][3] = r1 ? *reinterpret_cast<const uint32_t*>(q1 + d0 + 8) : 0u;
+          } else {
+            qa[ks][0] = r0 ? *reinterpret_cast<const uint32_t*>(qb + gq * kHead + d0) : 0u;
+            qa[ks][1] = r1 ? *reinterpret_cast<const uint32_t*>(qb + (gq + 8) * kHead + d0) : 0u;
+            qa[ks][2] = r0 ? *reinterpret_cast<const uint32_t*>(qb + gq * kHead + d0 + 8) : 0u;
+            qa[ks][3] = r1 ? *reinterpret_cast<const uint32_t*>(qb + (gq + 8) * kHead + d0 + 8) : 0u;
+          }
         } else {
           float f[2][4];
 #pragma unroll
@@ -681,8 +753,8 @@ __global__ void __launch_bounds__(kAttnThreads) span_attn_kernel(const AttnParam
       if (tr0 && i == 0) B2_TR(g_attn_tr, 4);
       const int wtok = tok0 + i * kTile + warp * 16;  // first token of this warp's slice
       if (wtok < tok1) {
-        if constexpr (!T::kCodesF16) tile_compute_bf16<H>(smem + slot * T::STAGE, warp, lane, wtok, tok1, p.scale_log2, qa, o, mrow, lrow);
-        else tile_compute_q<QM>(smem + slot * T::STAGE, warp, lane, wtok, tok1, p.scale_log2, qa, sq, o, mrow, lrow, cacc);
+        if constexpr (!T::kCodesF16) tile_compute_bf16<H, MT>(smem + slot * T::STAGE, warp, lane, wtok, tok1, lim, p.scale_log2, qa, o, mrow, lrow);
+        else tile_compute_q<QM, MT>(smem + slot * T::STAGE, warp, lane, wtok, tok1, lim, p.scale_log2, qa, sq, o, mrow, lrow, cacc);
       }
       __syncthreads();  // this stage may be refilled by the next iteration's prefetch
       slot = slot + 1 == p.nstage ? 0 : slot + 1;
@@ -740,9 +812,9 @@ __global__ void __launch_bounds__(kAttnThreads) span_attn_kernel(const AttnParam
     }
     __syncthreads();
     // thread d = tid handles column d of every head row
-    const int cnt_idx = b * p.n_groups + g;
+    const int cnt_idx = item * p.n_groups + g;
     const int my_slot = 2 * blockIdx.x + (pos != lo ? 1 : 0);
-    for (int r = 0; r < p.hpg; ++r) {
+    for (int r = 0; r < nrows; ++r) {
       float M = -INFINITY;
 #pragma unroll
       for (int w = 0; w < 4; ++w) M = fmaxf(M, mrg_ml[(w * 16 + r) * 2]);
@@ -755,12 +827,13 @@ __global__ void __launch_bounds__(kAttnThreads) span_attn_kernel(const AttnParam
         acc += f * mrg[(w * 16 + r) * kMergeRS + tid];
       }
       if (npieces == 1) {
-        p.out[((size_t)b * p.n_heads + (size_t)g * p.hpg + r) * kHead + tid] = F::from_f(acc / L);
+        if constexpr (MT) p.out[tok_row(p, b, qt0, g, r) + tid] = F::from_f(acc / L);
+        else p.out[((size_t)b * p.n_heads + (size_t)g * p.hpg + r) * kHead + tid] = F::from_f(acc / L);
       } else {
-        p.ws_o[((size_t)my_slot * p.hpg + r) * kHead + tid] = acc;
+        p.ws_o[((size_t)my_slot * rstride + r) * kHead + tid] = acc;
         if (tid == 0) {
-          p.ws_ml[((size_t)my_slot * p.hpg + r) * 2] = M;
-          p.ws_ml[((size_t)my_slot * p.hpg + r) * 2 + 1] = L;
+          p.ws_ml[((size_t)my_slot * rstride + r) * 2] = M;
+          p.ws_ml[((size_t)my_slot * rstride + r) * 2 + 1] = L;
         }
       }
     }
@@ -772,14 +845,17 @@ __global__ void __launch_bounds__(kAttnThreads) span_attn_kernel(const AttnParam
       // pieces of this (sequence, kv-head) come from CTAs k0 .. k0+npieces-1 (one each); only CTA k0's piece can start
       // inside its range (slot parity 1)
       const int first_par = bg_start > k0 * Tc ? 1 : 0;
-      __nv_bfloat16* out_rows = p.out + ((size_t)b * p.n_heads + (size_t)g * p.hpg) * kHead;
+      __nv_bfloat16* out_rows;
+      if constexpr (MT) out_rows = p.out + tok_row(p, b, qt0, g, 0);
+      else out_rows = p.out + ((size_t)b * p.n_heads + (size_t)g * p.hpg) * kHead;
       if (npieces <= kMergeDirect) {
         if (tid == 0) s_is_last = atomicAdd(&p.counters[cnt_idx], 1u) == (unsigned)(npieces - 1);
         __syncthreads();
         if (s_is_last) {
           __threadfence();
           if (tid == 0 && cnt_idx == 0) B2_TR(g_attn_tr, 10);
-          merge_partials<true, H>(p.ws_o, p.ws_ml, 2 * k0, 2, first_par, npieces, p.hpg, out_rows, nullptr, nullptr, 0, s_w, s_ML);
+          merge_partials<true, H, MT>(p.ws_o, p.ws_ml, 2 * k0, 2, first_par, npieces, rstride, out_rows, nullptr, nullptr, 0, s_w, s_ML,
+                                      nrows, p.hpg, p.n_heads * kHead);
           if (tid == 0) p.counters[cnt_idx] = 0;  // re-arm
           if (tid == 0 && cnt_idx == 0) B2_TR(g_attn_tr, 11);
         }
@@ -797,8 +873,8 @@ __global__ void __launch_bounds__(kAttnThreads) span_attn_kernel(const AttnParam
         if (s_is_last) {
           __threadfence();
           if (tid == 0 && cnt_idx == 0 && q == 0) B2_TR(g_attn_tr, 8);
-          merge_partials<false, H>(p.ws_o, p.ws_ml, 2 * (k0 + q * kMergeFan), 2, q == 0 ? first_par : 0, gsize, p.hpg, nullptr,
-                                p.ws2_o, p.ws2_ml, lead, s_w, s_ML);
+          merge_partials<false, H, MT>(p.ws_o, p.ws_ml, 2 * (k0 + q * kMergeFan), 2, q == 0 ? first_par : 0, gsize, rstride, nullptr,
+                                       p.ws2_o, p.ws2_ml, lead, s_w, s_ML, nrows, p.hpg, p.n_heads * kHead);
           if (tid == 0 && cnt_idx == 0 && q == 0) B2_TR(g_attn_tr, 9);
           if (tid == 0) p.counters1[lead] = 0;
           __threadfence();
@@ -808,7 +884,8 @@ __global__ void __launch_bounds__(kAttnThreads) span_attn_kernel(const AttnParam
           if (s_is_last) {
             __threadfence();
             if (tid == 0 && cnt_idx == 0) B2_TR(g_attn_tr, 10);
-            merge_partials<true, H>(p.ws2_o, p.ws2_ml, 2 * k0, 2 * kMergeFan, first_par, ngroups, p.hpg, out_rows, nullptr, nullptr, 0, s_w, s_ML);
+            merge_partials<true, H, MT>(p.ws2_o, p.ws2_ml, 2 * k0, 2 * kMergeFan, first_par, ngroups, rstride, out_rows, nullptr, nullptr, 0,
+                                        s_w, s_ML, nrows, p.hpg, p.n_heads * kHead);
             if (tid == 0) p.counters[cnt_idx] = 0;
             if (tid == 0 && cnt_idx == 0) B2_TR(g_attn_tr, 11);
           }
@@ -946,9 +1023,12 @@ struct AppendParams {
   int rope;        // 0/1
   int rotary_dim;
   float log2_base;
+  int q_len;       // multi-token form: rows per sequence
 };
 
-template <int QM, bool H>
+// MT = false: row b of qkv / q_out is sequence b, written at position old_lens[b].  MT = true: row b*q_len + t is token t of
+// sequence b, written at position old_lens[b] + t.
+template <int QM, bool H, bool MT = false>
 __global__ void __launch_bounds__(128) cache_append_kernel(const AppendParams p) {
   using F = Ft<H>;
   pdl_wait();
@@ -956,12 +1036,13 @@ __global__ void __launch_bounds__(128) cache_append_kernel(const AppendParams p)
   const int lane = threadIdx.x & 31;
   const int slots = p.n_heads + 2 * p.n_groups;
   const int wid = blockIdx.x * 4 + (threadIdx.x >> 5);
-  if (wid >= p.batch * slots) return;
-  const int b = wid / slots, slot = wid - b * slots;
-  const __nv_bfloat16* src = p.qkv + ((size_t)b * slots + slot) * kHead + lane * 4;
+  if (wid >= (MT ? p.batch * p.q_len : p.batch) * slots) return;
+  const int row = wid / slots, slot = wid - row * slots;
+  const int b = MT ? row / p.q_len : row;
+  const __nv_bfloat16* src = p.qkv + ((size_t)row * slots + slot) * kHead + lane * 4;
   const uint2 raw = *reinterpret_cast<const uint2*>(src);
   float x[4] = {F::lo(raw.x), F::hi(raw.x), F::lo(raw.y), F::hi(raw.y)};
-  const int pos = p.old_lens[b];
+  const int pos = MT ? p.old_lens[b] + (row - b * p.q_len) : p.old_lens[b];
   const bool is_v = slot >= p.n_heads + p.n_groups;
 
   if (p.rope && !is_v) {
@@ -987,7 +1068,7 @@ __global__ void __launch_bounds__(128) cache_append_kernel(const AppendParams p)
   }
 
   if (slot < p.n_heads) {
-    *reinterpret_cast<uint2*>(p.q_out + ((size_t)b * p.n_heads + slot) * kHead + lane * 4) =
+    *reinterpret_cast<uint2*>(p.q_out + ((size_t)row * p.n_heads + slot) * kHead + lane * 4) =
         make_uint2(F::pack(x[0], x[1]), F::pack(x[2], x[3]));
     return;
   }
@@ -1031,10 +1112,22 @@ struct b2_span_attn {
 };
 
 typedef void (*attn_kernel_t)(const AttnParams);
+typedef void (*attn_tok_kernel_t)(const AttnTokParams);
 static attn_kernel_t attn_kernel_for(const b2_span_cfg* c) {
   return with_kv_mode(c->quant_mode, [&](auto QM) {
     return with_flag(c->ft == B2_DT_F16, [&](auto H) -> attn_kernel_t { return span_attn_kernel<QM, H>; });
   });
+}
+static attn_tok_kernel_t attn_tok_kernel_for(const b2_span_cfg* c) {
+  return with_kv_mode(c->quant_mode, [&](auto QM) {
+    return with_flag(c->ft == B2_DT_F16, [&](auto H) -> attn_tok_kernel_t { return span_attn_kernel<QM, H, true>; });
+  });
+}
+
+// multi-token row blocks: whole tokens per block of 16 MMA rows
+static int tokens_per_block(const b2_span_cfg* c, int q_len) {
+  const int tpb = 16 / (c->n_heads / c->n_groups);
+  return q_len < tpb ? q_len : tpb;
 }
 
 // bytes of one token row of one kv-head in a span (KVTraits::SPAN_ROW; head 64 is bf16 only)
@@ -1064,6 +1157,7 @@ int b2_span_attn_create(b2_span_attn_t* out, const b2_span_cfg* cfg, int max_bat
   h->cfg = *cfg;
   h->max_batch = max_batch;
   attn_kernel_t kern = attn_kernel_for(cfg);
+  attn_tok_kernel_t kern_mt = attn_tok_kernel_for(cfg);
   int sb = 0;
   with_kv_mode(cfg->quant_mode, [&](auto QM) {
     sb = KVTraits<QM>::STAGE;
@@ -1074,6 +1168,7 @@ int b2_span_attn_create(b2_span_attn_t* out, const b2_span_cfg* cfg, int max_bat
   const int merge = (4 * 16 * kMergeRS + 4 * 16 * 2) * 4;
   h->smem = h->nstage * sb > merge ? h->nstage * sb : merge;
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem);
+  if (e == cudaSuccess && cfg->head_size == kHead) e = cudaFuncSetAttribute(kern_mt, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem);
   int occ = 1;
   if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, kAttnThreads, h->smem);
   if (e != cudaSuccess) {
@@ -1084,6 +1179,9 @@ int b2_span_attn_create(b2_span_attn_t* out, const b2_span_cfg* cfg, int max_bat
   if (occ < 1) occ = 1;
   const int want = env_int("B2_ATTN_CTAS_PER_SM", 0);  // ignored when <= 0
   if (want > 0 && want < occ) occ = want;
+  // the multi-token kernel launches the same grid (and so the same partial slots): its merges are done by the last CTA to
+  // arrive and never wait for another, so any grid is correct; its register count (162-168 against 160) leaves the
+  // occupancy of these 128-thread CTAs unchanged
   h->grid = occ * sm_count();
   const int max_pieces = env_int("B2_ATTN_MAX_PIECES", 0);  // ignored when <= 0
   if (max_pieces > 0) h->max_pieces = max_pieces;
@@ -1106,13 +1204,59 @@ int b2_span_attn_destroy(b2_span_attn_t h) {
   return B2_OK;
 }
 
+}  // extern "C"
+
 // split-KV partials: at most two per CTA (its first and its last piece), independent of batch and length
 static size_t partial_slots(const b2_span_attn* h) { return (size_t)2 * h->grid; }
 
+// level-0 and level-1 partials of `rows` rows per slot
+static size_t attn_workspace_bytes(const b2_span_attn* h, int rows) {
+  return 2 * partial_slots(h) * rows * (kHead + 2) * sizeof(float) + 256;
+}
+
+// q_len == 0: the single-token kernel; otherwise the multi-token one
+static int attn_launch(b2_span_attn_t h, void* out, const void* q, const void* const* k_spans, const void* const* v_spans,
+                       const int32_t* new_lens, int batch, int q_len, void* workspace, float qk_scale, void* stream_) {
+  const int hpg = h->cfg.n_heads / h->cfg.n_groups;
+  AttnTokParams p;
+  p.q_len = q_len;
+  p.tpb = q_len ? tokens_per_block(&h->cfg, q_len) : 1;
+  p.nrb = q_len ? (q_len + p.tpb - 1) / p.tpb : 1;
+  p.rstride = p.tpb * hpg;
+  const size_t rows = p.rstride;
+  p.out = (__nv_bfloat16*)out;
+  p.q = (const __nv_bfloat16*)q;
+  p.k_spans = k_spans;
+  p.v_spans = v_spans;
+  p.lens = new_lens;
+  const size_t items = partial_slots(h);
+  p.ws_o = (float*)(((uintptr_t)workspace + 127) & ~(uintptr_t)127);
+  p.ws_ml = p.ws_o + items * rows * kHead;
+  p.ws2_o = p.ws_ml + items * rows * 2;
+  p.ws2_ml = p.ws2_o + items * rows * kHead;
+  p.counters = h->counters;
+  p.counters1 = h->counters + (size_t)h->max_batch * h->cfg.n_groups;
+  p.max_pieces = h->max_pieces;
+  p.batch = batch; p.n_heads = h->cfg.n_heads; p.n_groups = h->cfg.n_groups; p.hpg = hpg;
+  p.span_len = h->cfg.span_len; p.span_shift = ilog2(h->cfg.span_len); p.max_spans = h->cfg.max_spans_per_seq;
+  p.nstage = h->nstage;
+  p.scale_log2 = qk_scale * 1.4426950408889634f;
+  const cudaError_t e = q_len ? launch(attn_tok_kernel_for(&h->cfg), dim3(h->grid), dim3(kAttnThreads), (size_t)h->smem,
+                                        (cudaStream_t)stream_, true, p)
+                             : launch(attn_kernel_for(&h->cfg), dim3(h->grid), dim3(kAttnThreads), (size_t)h->smem,
+                                      (cudaStream_t)stream_, true, static_cast<const AttnParams&>(p));
+  if (e != cudaSuccess) {
+    set_last_error("span_attn launch", e);
+    return B2_ERR_CUDA;
+  }
+  return B2_OK;
+}
+
+extern "C" {
+
 size_t b2_span_attn_workspace_bytes(b2_span_attn_t h, int batch, int max_len) {
   if (!h || batch <= 0 || max_len <= 0) return 0;
-  const int hpg = h->cfg.n_heads / h->cfg.n_groups;
-  return 2 * partial_slots(h) * hpg * (kHead + 2) * sizeof(float) + 256;  // level-0 and level-1 partials
+  return attn_workspace_bytes(h, h->cfg.n_heads / h->cfg.n_groups);
 }
 
 int b2_span_attn_run(b2_span_attn_t h, void* out, const void* q, const void* const* k_spans, const void* const* v_spans,
@@ -1123,32 +1267,23 @@ int b2_span_attn_run(b2_span_attn_t h, void* out, const void* q, const void* con
   if (max_len <= 0 || (int64_t)(max_len + h->cfg.span_len - 1) / h->cfg.span_len > h->cfg.max_spans_per_seq) return B2_ERR_LIMIT;
   if (!workspace || workspace_bytes < b2_span_attn_workspace_bytes(h, batch, max_len)) return B2_ERR_PARAM;
   if (h->cfg.head_size == 64) return span_attn64_run(&h->cfg, out, q, k_spans, v_spans, new_lens, batch, qk_scale, (cudaStream_t)stream_);
-  const int hpg = h->cfg.n_heads / h->cfg.n_groups;
-  AttnParams p;
-  p.out = (__nv_bfloat16*)out;
-  p.q = (const __nv_bfloat16*)q;
-  p.k_spans = k_spans;
-  p.v_spans = v_spans;
-  p.lens = new_lens;
-  const size_t items = partial_slots(h);
-  p.ws_o = (float*)(((uintptr_t)workspace + 127) & ~(uintptr_t)127);
-  p.ws_ml = p.ws_o + items * hpg * kHead;
-  p.ws2_o = p.ws_ml + items * hpg * 2;
-  p.ws2_ml = p.ws2_o + items * hpg * kHead;
-  p.counters = h->counters;
-  p.counters1 = h->counters + (size_t)h->max_batch * h->cfg.n_groups;
-  p.max_pieces = h->max_pieces;
-  p.batch = batch; p.n_heads = h->cfg.n_heads; p.n_groups = h->cfg.n_groups; p.hpg = hpg;
-  p.span_len = h->cfg.span_len; p.span_shift = ilog2(h->cfg.span_len); p.max_spans = h->cfg.max_spans_per_seq;
-  p.nstage = h->nstage;
-  p.scale_log2 = qk_scale * 1.4426950408889634f;
-  attn_kernel_t kern = attn_kernel_for(&h->cfg);
-  cudaError_t e = launch(kern, dim3(h->grid), dim3(kAttnThreads), (size_t)h->smem, (cudaStream_t)stream_, true, p);
-  if (e != cudaSuccess) {
-    set_last_error("span_attn launch", e);
-    return B2_ERR_CUDA;
-  }
-  return B2_OK;
+  return attn_launch(h, out, q, k_spans, v_spans, new_lens, batch, 0, workspace, qk_scale, stream_);
+}
+
+size_t b2_span_attn_tokens_workspace_bytes(b2_span_attn_t h, int batch, int q_len, int max_len) {
+  if (!h || batch <= 0 || q_len < 1 || q_len > 16 || max_len <= 0) return 0;
+  return attn_workspace_bytes(h, tokens_per_block(&h->cfg, q_len) * (h->cfg.n_heads / h->cfg.n_groups));
+}
+
+int b2_span_attn_run_tokens(b2_span_attn_t h, void* out, const void* q, const void* const* k_spans, const void* const* v_spans,
+                            const int32_t* new_lens, int batch, int q_len, int max_len, void* workspace, size_t workspace_bytes,
+                            float qk_scale, void* stream_) {
+  if (!h || !out || !q || !k_spans || !v_spans || !new_lens) return B2_ERR_PARAM;
+  if (h->cfg.head_size != kHead) return B2_ERR_UNSUPPORTED;
+  if (q_len < 1 || q_len > 16 || batch <= 0 || (int64_t)batch * q_len > h->max_batch) return B2_ERR_LIMIT;
+  if (max_len <= 0 || (int64_t)(max_len + h->cfg.span_len - 1) / h->cfg.span_len > h->cfg.max_spans_per_seq) return B2_ERR_LIMIT;
+  if (!workspace || workspace_bytes < b2_span_attn_tokens_workspace_bytes(h, batch, q_len, max_len)) return B2_ERR_PARAM;
+  return attn_launch(h, out, q, k_spans, v_spans, new_lens, batch, q_len, workspace, qk_scale, stream_);
 }
 
 int b2_span_context_copy(const b2_span_cfg* cfg, void* const* spans, const void* src, int64_t token_stride, int seq_len,
@@ -1175,11 +1310,11 @@ int b2_span_context_copy(const b2_span_cfg* cfg, void* const* spans, const void*
   return B2_OK;
 }
 
-int b2_span_cache_append(const b2_span_cfg* cfg, void* const* k_spans, void* const* v_spans, void* q_out,
-                         const void* qkv, const int32_t* old_lens, int batch, const b2_rope_cfg* rope, void* stream_) {
-  if (int st = check_cfg(cfg)) return st;
-  if (!k_spans || !v_spans || !q_out || !qkv || !old_lens || batch <= 0) return B2_ERR_PARAM;
-  if (cfg->head_size == 64) return span_append64_run(cfg, k_spans, v_spans, q_out, qkv, old_lens, batch, rope, (cudaStream_t)stream_);
+}  // extern "C"
+
+// q_len == 0: one row per sequence (cache_append_kernel<..., MT = false>); otherwise q_len rows per sequence
+static int cache_append_launch(const b2_span_cfg* cfg, void* const* k_spans, void* const* v_spans, void* q_out, const void* qkv,
+                               const int32_t* old_lens, int batch, int q_len, const b2_rope_cfg* rope, void* stream_) {
   if (rope && (rope->rotary_dim != 128 && rope->rotary_dim != 64)) return B2_ERR_UNSUPPORTED;
   AppendParams p;
   p.k_spans = k_spans; p.v_spans = v_spans;
@@ -1189,11 +1324,14 @@ int b2_span_cache_append(const b2_span_cfg* cfg, void* const* k_spans, void* con
   p.rope = rope ? 1 : 0;
   p.rotary_dim = rope ? rope->rotary_dim : 0;
   p.log2_base = rope ? log2f(rope->base) : 0.f;
-  const int warps = batch * (cfg->n_heads + 2 * cfg->n_groups);
+  p.q_len = q_len;
+  const int warps = batch * (q_len ? q_len : 1) * (cfg->n_heads + 2 * cfg->n_groups);
   const dim3 grid((warps + 3) / 4), block(128);
   const cudaError_t e = with_kv_mode(cfg->quant_mode, [&](auto QM) {
     return with_flag(cfg->ft == B2_DT_F16, [&](auto H) {
-      return launch(cache_append_kernel<QM, H>, grid, block, 0, (cudaStream_t)stream_, true, p);
+      return with_flag(q_len != 0, [&](auto MT) {
+        return launch(cache_append_kernel<QM, H, MT>, grid, block, 0, (cudaStream_t)stream_, true, p);
+      });
     });
   });
   if (e != cudaSuccess) {
@@ -1201,6 +1339,25 @@ int b2_span_cache_append(const b2_span_cfg* cfg, void* const* k_spans, void* con
     return B2_ERR_CUDA;
   }
   return B2_OK;
+}
+
+extern "C" {
+
+int b2_span_cache_append(const b2_span_cfg* cfg, void* const* k_spans, void* const* v_spans, void* q_out,
+                         const void* qkv, const int32_t* old_lens, int batch, const b2_rope_cfg* rope, void* stream_) {
+  if (int st = check_cfg(cfg)) return st;
+  if (!k_spans || !v_spans || !q_out || !qkv || !old_lens || batch <= 0) return B2_ERR_PARAM;
+  if (cfg->head_size == 64) return span_append64_run(cfg, k_spans, v_spans, q_out, qkv, old_lens, batch, rope, (cudaStream_t)stream_);
+  return cache_append_launch(cfg, k_spans, v_spans, q_out, qkv, old_lens, batch, 0, rope, stream_);
+}
+
+int b2_span_cache_append_tokens(const b2_span_cfg* cfg, void* const* k_spans, void* const* v_spans, void* q_out, const void* qkv,
+                                const int32_t* old_lens, int batch, int q_len, const b2_rope_cfg* rope, void* stream_) {
+  if (int st = check_cfg(cfg)) return st;
+  if (cfg->head_size != kHead) return B2_ERR_UNSUPPORTED;
+  if (!k_spans || !v_spans || !q_out || !qkv || !old_lens || batch <= 0) return B2_ERR_PARAM;
+  if (q_len < 1 || q_len > 16) return B2_ERR_LIMIT;
+  return cache_append_launch(cfg, k_spans, v_spans, q_out, qkv, old_lens, batch, q_len, rope, stream_);
 }
 
 }  // extern "C"

@@ -123,14 +123,21 @@ class _RefView:
 class DecodeStack:
     def __init__(self, cfg, batch, max_len, wbits=4, group=-1, kv="none", span=128, seed=1234, device="cuda",
                  keep_ref=False, layers=None, tp_rank=0, tp_size=1, tp_group=None, fuse_swiglu=True, fuse_norm=False,
-                 collective=None, comm=None, dtype=torch.bfloat16):
+                 collective=None, comm=None, dtype=torch.bfloat16, q_len=1):
         """tp_size > 1: the reference's tensor-parallel layout (QKV/gate/up column split, o/down row split + all-reduce,
         vocab-split lm_head + B-element all-gather); every rank builds the SAME full synthetic weights from `seed` and
-        keeps its shard, exactly like the reference splits an already-quantized checkpoint."""
+        keeps its shard, exactly like the reference splits an already-quantized checkpoint.
+        q_len = T > 1: multi-token verify steps (speculative decoding).  Every step runs T rows per sequence: self.tokens
+        [B, T] holds the last emitted token (column 0, written by the step itself) and T-1 drafts (filled by the caller);
+        step() returns (pred [B, T], accepted [B]) and advances the lengths by the accepted counts on the device."""
         global _DT
         assert dtype in (torch.bfloat16, torch.float16) and (dtype == torch.bfloat16 or (tp_size == 1 and cfg.head == 128)), \
             "fp16: single GPU, head size 128 (the communicator and the head-64 kernels are bf16)"
+        assert 1 <= q_len <= 16 and (q_len == 1 or (tp_size == 1 and cfg.head == 128)), \
+            "multi-token steps: q_len <= 16, single GPU, head size 128"
         self.dtype = _DT = dtype
+        self.q_len = q_len
+        rows = batch * q_len  # activation rows of a step
         self.cfg, self.B, self.max_len = cfg, batch, max_len
         self.tp_rank, self.tp, self.tp_group = tp_rank, tp_size, tp_group
         # tensor-parallel exchange: "fused" = all-reduce inside the row-parallel GEMV's epilogue (b2_gemm_wq_run_allreduce;
@@ -158,38 +165,42 @@ class DecodeStack:
         for _ in range(self.n_layers):
             L = {}
             L["g1"] = (1.0 + 0.1 * torch.randn(H, generator=gen, device=device)).to(_DT)
-            L["qkv"] = QuantLinear(H, (nH + 2 * nG) * hd, wbits, group, gen, device, batch, bias=cfg.qkv_bias, keep_ref=keep_ref,
+            L["qkv"] = QuantLinear(H, (nH + 2 * nG) * hd, wbits, group, gen, device, rows, bias=cfg.qkv_bias, keep_ref=keep_ref,
                                    shard=col_qkv)
-            L["o"] = QuantLinear(nH * hd, H, wbits, group, gen, device, batch, keep_ref=keep_ref, shard=row)
+            L["o"] = QuantLinear(nH * hd, H, wbits, group, gen, device, rows, keep_ref=keep_ref, shard=row)
             L["g2"] = (1.0 + 0.1 * torch.randn(H, generator=gen, device=device)).to(_DT)
             if fuse_swiglu:
-                L["gateup"] = SwiGLULinear(H, I, wbits, group, gen, device, batch, keep_ref=keep_ref, shard=col_i)
+                L["gateup"] = SwiGLULinear(H, I, wbits, group, gen, device, rows, keep_ref=keep_ref, shard=col_i)
                 if keep_ref:
                     L["gate"], L["up"] = _RefView(L["gateup"].ref[0]), _RefView(L["gateup"].ref[1])
             else:
-                L["gate"] = QuantLinear(H, I, wbits, group, gen, device, batch, keep_ref=keep_ref, shard=col_i)
-                L["up"] = QuantLinear(H, I, wbits, group, gen, device, batch, keep_ref=keep_ref, shard=col_i)
-            L["down"] = QuantLinear(I, H, wbits, group, gen, device, batch, keep_ref=keep_ref, shard=row)
+                L["gate"] = QuantLinear(H, I, wbits, group, gen, device, rows, keep_ref=keep_ref, shard=col_i)
+                L["up"] = QuantLinear(H, I, wbits, group, gen, device, rows, keep_ref=keep_ref, shard=col_i)
+            L["down"] = QuantLinear(I, H, wbits, group, gen, device, rows, keep_ref=keep_ref, shard=row)
             L["cache"] = ops.SpanCache(batch, max_len, nHl, nGl, span, self.kv_mode, device, head=hd, dtype=dtype)
             self.layers.append(L)
         self.gf = (1.0 + 0.1 * torch.randn(H, generator=gen, device=device)).to(_DT)
         self.vocab_l = cfg.vocab // tp
-        self.lm_head = QuantLinear(H, cfg.vocab, 16, -1, gen, device, batch, keep_ref=keep_ref,
+        self.lm_head = QuantLinear(H, cfg.vocab, 16, -1, gen, device, rows, keep_ref=keep_ref,
                                    shard=("cols", TP.col_range_even(cfg.vocab, r, tp)) if tp > 1 else None)
-        self.attn = ops.SpanAttn(self.layers[0]["cache"].cfg, batch)
+        self.attn = ops.SpanAttn(self.layers[0]["cache"].cfg, rows)
         self.ws = ops.Workspace(device)
         self.rope = (cfg.rope_base, hd)
         # device-resident step state, allocated for the construction batch; set_batch() re-views it for a smaller batch
         self.Bmax = batch
         self._lens_old = torch.zeros(batch, dtype=torch.int32, device=device)
-        self._lens_new = torch.ones(batch, dtype=torch.int32, device=device)
+        self._lens_new = torch.full((batch,), q_len, dtype=torch.int32, device=device)  # lens_old + q_len
         self._ids = torch.zeros(batch, dtype=torch.int64, device=device)
         self._next_ids = torch.zeros(batch, dtype=torch.int64, device=device)
+        if q_len > 1:
+            self._tokens = torch.zeros(batch, q_len, dtype=torch.int64, device=device)
+            self._pred = torch.zeros(batch, q_len, dtype=torch.int64, device=device)
+            self._accepted = torch.zeros(batch, dtype=torch.int32, device=device)
         bf = dict(dtype=_DT, device=device)
-        self._bufs = dict(x=torch.empty(batch, H, **bf), xn=torch.empty(batch, H, **bf),
-                          qkv=torch.empty(batch, (nHl + 2 * nGl) * hd, **bf), q=torch.empty(batch, nHl * hd, **bf),
-                          ao=torch.empty(batch, nHl * hd, **bf), gate=torch.empty(batch, self.I_l, **bf),
-                          up=torch.empty(batch, self.I_l, **bf), logits=torch.empty(batch, self.vocab_l, **bf))
+        self._bufs = dict(x=torch.empty(rows, H, **bf), xn=torch.empty(rows, H, **bf),
+                          qkv=torch.empty(rows, (nHl + 2 * nGl) * hd, **bf), q=torch.empty(rows, nHl * hd, **bf),
+                          ao=torch.empty(rows, nHl * hd, **bf), gate=torch.empty(rows, self.I_l, **bf),
+                          up=torch.empty(rows, self.I_l, **bf), logits=torch.empty(rows, self.vocab_l, **bf))
         if tp > 1:
             if self.collective != "nccl" and self.comm is None:
                 self.comm = ops.Comm(tp_rank, tp, max(batch * H * 2, 4096)).connect_group(tp_group)
@@ -204,10 +215,10 @@ class DecodeStack:
         # consumers normalise while staging activations; only layer 0's first norm stays a stand-alone kernel.
         # Off by default: it removes 2 launches/layer but lengthens every GEMV's dependent chain (statistics load + barrier
         # before staging).
-        self.fuse_norm = fuse_norm and tp == 1 and batch <= 16
+        self.fuse_norm = fuse_norm and tp == 1 and rows <= 16
         if self.fuse_norm:
-            self.ssq_o = torch.zeros(self.layers[0]["o"].op.sumsq_parts(), batch, dtype=torch.float32, device=device)
-            self.ssq_d = torch.zeros(self.layers[0]["down"].op.sumsq_parts(), batch, dtype=torch.float32, device=device)
+            self.ssq_o = torch.zeros(self.layers[0]["o"].op.sumsq_parts(), rows, dtype=torch.float32, device=device)
+            self.ssq_d = torch.zeros(self.layers[0]["down"].op.sumsq_parts(), rows, dtype=torch.float32, device=device)
         # Self-contained RMSNorm fusion (any TP): the column-parallel GEMVs (qkv, gate/up) stage bf16(x * gamma), collect
         # sum x^2 in the same pass and scale their reduced tile by 1/rms — two launches per layer disappear.  Every CTA
         # repeats the normalisation of its k-slice of every live row, so the saving shrinks with the batch.  Default: batches <= 2.
@@ -219,9 +230,9 @@ class DecodeStack:
         # 1/rms.  Only layer 0's first norm stays a stand-alone kernel (2 launches per layer fewer).
         self.norm_handoff = (os.environ.get("B2_NORM_HANDOFF", "1") != "0" and tp == 1 and not self.fuse_norm
                              and (group == -1 or wbits == 4))
-        if self.norm_handoff and batch >= 17:
-            self._ssq_o = torch.zeros(self.layers[0]["o"].op.sumsq_parts() * batch, dtype=torch.float32, device=device)
-            self._ssq_d = torch.zeros(self.layers[0]["down"].op.sumsq_parts() * batch, dtype=torch.float32, device=device)
+        if self.norm_handoff and rows >= 17:
+            self._ssq_o = torch.zeros(self.layers[0]["o"].op.sumsq_parts() * rows, dtype=torch.float32, device=device)
+            self._ssq_d = torch.zeros(self.layers[0]["down"].op.sumsq_parts() * rows, dtype=torch.float32, device=device)
         self.launches_per_step = 0
 
     def set_batch(self, b):
@@ -231,9 +242,11 @@ class DecodeStack:
         assert 1 <= b <= self.Bmax
         self.B = b
         for k, v in self._bufs.items():
-            setattr(self, k, v[:b])
+            setattr(self, k, v[:b * self.q_len])
         self.lens_old, self.lens_new = self._lens_old[:b], self._lens_new[:b]
         self.ids, self.next_ids = self._ids[:b], self._next_ids[:b]
+        if self.q_len > 1:
+            self.tokens, self.pred, self.accepted = self._tokens[:b], self._pred[:b], self._accepted[:b]
         self.graph = None
         assert not getattr(self, "fuse_norm", False) or b == self.Bmax, "the fused-norm statistics are laid out for one batch"
 
@@ -259,7 +272,7 @@ class DecodeStack:
                 ops.context_copy(L["cache"], "k", b, rows[:, :kw])
                 ops.context_copy(L["cache"], "v", b, rows[:, kw:])
         self._lens_old.fill_(ctx)
-        self._lens_new.fill_(ctx + 1)
+        self._lens_new.fill_(ctx + self.q_len)
         torch.cuda.synchronize()
 
     # ------------------------------------------------------------------ one decode step (eager or captured)
@@ -301,13 +314,15 @@ class DecodeStack:
         cfg, ws = self.cfg, self.ws
         H = cfg.hidden
         fn = self.fuse_norm
-        ns = self.norm_self and self.B <= min(16, self.norm_self_max_b)
-        nh = self.norm_handoff and self.B >= 17
+        T = self.q_len
+        R = self.B * T  # activation rows: the fusion thresholds follow them
+        ns = self.norm_self and R <= min(16, self.norm_self_max_b)
+        nh = self.norm_handoff and R >= 17
         if nh:
-            ssq_o = self._ssq_o[:self._ssq_o.numel() // self.Bmax * self.B].view(-1, self.B)
-            ssq_d = self._ssq_d[:self._ssq_d.numel() // self.Bmax * self.B].view(-1, self.B)
+            ssq_o = self._ssq_o[:self._ssq_o.numel() // self.Bmax * self.B].view(-1, R)
+            ssq_d = self._ssq_d[:self._ssq_d.numel() // self.Bmax * self.B].view(-1, R)
         n = 0
-        ops.embedding(self.embed, self.ids, out=self.x); n += 1
+        ops.embedding(self.embed, self.ids if T == 1 else self.tokens.view(-1), out=self.x); n += 1
         for li, L in enumerate(self.layers):
             if fn and li > 0:  # x and its row statistics come from the previous layer's down_proj
                 L["qkv"](self.x, ws, out=self.qkv, norm_in=(self.ssq_d, L["g1"], H, cfg.eps)); n += 1
@@ -318,8 +333,12 @@ class DecodeStack:
             else:
                 ops.rmsnorm(self.x, L["g1"], cfg.eps, out=self.xn); n += 1
                 L["qkv"](self.xn, ws, out=self.qkv); n += 1
-            ops.cache_append(L["cache"], self.qkv, self.lens_old, q_out=self.q, rope=self.rope); n += 1
-            self.attn(self.q, L["cache"], self.lens_new, self.max_len, ws, out=self.ao); n += 1
+            if T == 1:
+                ops.cache_append(L["cache"], self.qkv, self.lens_old, q_out=self.q, rope=self.rope); n += 1
+                self.attn(self.q, L["cache"], self.lens_new, self.max_len, ws, out=self.ao); n += 1
+            else:
+                ops.cache_append_tokens(L["cache"], self.qkv, self.lens_old, T, q_out=self.q, rope=self.rope); n += 1
+                self.attn.run_tokens(self.q, L["cache"], self.lens_new, T, self.max_len, ws, out=self.ao); n += 1
             if fn:
                 L["o"](self.ao, ws, out=self.x, residual=self.x, sumsq_out=self.ssq_o); n += 1
                 mlp_in, nin = self.x, (self.ssq_o, L["g2"], H, cfg.eps)
@@ -353,7 +372,9 @@ class DecodeStack:
         else:
             ops.rmsnorm(self.x, self.gf, cfg.eps, out=self.xn); n += 1
             self.lm_head(self.xn, ws, out=self.logits); n += 1
-        if self.tp == 1:
+        if T > 1:
+            ops.argmax(self.logits, out=self.pred.view(-1)); n += 1
+        elif self.tp == 1:
             ops.argmax(self.logits, out=self.next_ids); n += 1
         else:  # vocab-split lm_head: local (max, argmax) + B-element all-gather instead of all-reducing 152064 logits
             ops.argmax_shard(self.logits, self.tp_rank * self.vocab_l, self.loc_ids, self.loc_val); n += 1
@@ -365,32 +386,42 @@ class DecodeStack:
                 self.comm.allgather(self.loc_val, self.all_val); n += 1
                 self.comm.allgather(self.loc_ids, self.all_ids); n += 1
             ops.argmax_merge(self.all_val, self.all_ids, out=self.next_ids); n += 1  # lowest rank on ties == lowest vocab id
-        ops.lens_add(self.lens_old, 1); n += 1
-        ops.lens_add(self.lens_new, 1); n += 1
-        # rows per launch above batch 16: 64 on the wgmma path (per-channel int4/int8, bf16 lm_head), 16 for sub-channel
-        # weights (mma.sync path); below, one launch takes the whole batch
-        hchunks = (self.B + 63) // 64 if self.B > 16 else 1
-        qchunks = ((self.B + 15) // 16 if (self.group_size != -1 and self.wbits != 4) else hchunks) if self.B > 16 else 1
+        if T > 1:  # greedy verification: accepted counts, next token and lengths stay on the device
+            ops.spec_accept(self.accepted, self.next_ids, self.lens_old, self.lens_new, self.tokens, self.pred); n += 1
+        else:
+            ops.lens_add(self.lens_old, 1); n += 1
+            ops.lens_add(self.lens_new, 1); n += 1
+        # rows per launch above 16 rows: 64 on the wgmma path (per-channel int4/int8, bf16 lm_head), 16 for sub-channel
+        # weights (mma.sync path); below, one launch takes all rows
+        hchunks = (R + 63) // 64 if R > 16 else 1
+        qchunks = ((R + 15) // 16 if (self.group_size != -1 and self.wbits != 4) else hchunks) if R > 16 else 1
         n += (qchunks - 1) * (4 if self.fuse_swiglu else 5) * len(self.layers) + (hchunks - 1)
         self.launches_per_step = n
 
     def step(self):
+        """q_len 1: returns next_ids [B].  q_len > 1: one verify step, returns (pred [B, T], accepted [B]); the step's
+        emitted tokens are pred[b, :accepted[b]]."""
         if self.graph is not None:
             self.graph.replay()
         else:
             self._step_ops()
-        return self.next_ids
+        return self.next_ids if self.q_len == 1 else (self.pred, self.accepted)
 
     def capture(self):
         """Warm up once eagerly (plans, workspace growth), rewind the lengths, then capture one step."""
         lo, ln = self.lens_old.clone(), self.lens_new.clone()
+        tk = self.tokens.clone() if self.q_len > 1 else None  # the accept kernel rewrites column 0
         self._step_ops()
         torch.cuda.synchronize()
         self.lens_old.copy_(lo); self.lens_new.copy_(ln)
+        if tk is not None:
+            self.tokens.copy_(tk)
         g = torch.cuda.CUDAGraph()
         with torch.cuda.graph(g):
             self._step_ops()
         self.lens_old.copy_(lo); self.lens_new.copy_(ln)
+        if tk is not None:
+            self.tokens.copy_(tk)
         torch.cuda.synchronize()
         self.graph = g
         return g

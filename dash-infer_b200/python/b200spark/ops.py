@@ -248,6 +248,30 @@ def cache_append(cache, qkv, old_lens, q_out=None, rope=None):
     return q_out
 
 
+def cache_append_tokens(cache, qkv, old_lens, q_len, q_out=None, rope=None):
+    """Multi-token append: row b*q_len + t of qkv is token t of sequence b, written at position old_lens[b] + t."""
+    cfg = cache.cfg
+    rows = qkv.shape[0]
+    assert rows % q_len == 0
+    if q_out is None:
+        q_out = torch.empty(rows, cfg.n_heads * cfg.head_size, dtype=qkv.dtype, device=qkv.device)
+    r = RopeCfg(float(rope[0]), int(rope[1]), 0) if rope is not None else None
+    check(lib.b2_span_cache_append_tokens(C.byref(cfg), _ptr(cache.k_tab), _ptr(cache.v_tab), _ptr(q_out), _ptr(qkv),
+                                          _ptr(old_lens), rows // q_len, int(q_len), C.byref(r) if r is not None else None,
+                                          _stream()), "b2_span_cache_append_tokens")
+    return q_out
+
+
+def spec_accept(accepted, next_ids, old_lens, new_lens, tokens, pred):
+    """Greedy verification of a multi-token step (b2_spec_accept): tokens / pred int64 [B, T]; writes accepted (int32 [B]),
+    next_ids (int64 [B] or None) and tokens[:, 0], advances old_lens by the accepted counts and sets new_lens = old_lens + T."""
+    B, T = tokens.shape
+    assert tokens.is_contiguous() and pred.is_contiguous() and pred.shape == tokens.shape
+    check(lib.b2_spec_accept(_ptr(accepted), _ptr(next_ids), _ptr(old_lens), _ptr(new_lens), _ptr(tokens), _ptr(pred), B, T,
+                             _stream()), "b2_spec_accept")
+    return accepted
+
+
 def context_copy(cache, which, b, src, seq_len=None):
     """Prefill: write sequence b's K (which='k') or V ('v') rows src [seq, ..., n_groups*128 leading values per token] into its
     spans (b2_span_context_copy).  src may be a strided view (e.g. the K part of a fused qkv tensor)."""
@@ -276,6 +300,22 @@ class SpanAttn:
         wsb = ws.reserve(self.workspace_bytes(B, max_len))
         check(lib.b2_span_attn_run(self.h, _ptr(out), _ptr(q), _ptr(cache.k_tab), _ptr(cache.v_tab), _ptr(new_lens), B,
                                    int(max_len), _ptr(wsb), wsb.numel(), float(scale), _stream()), "b2_span_attn_run")
+        return out
+
+    def tokens_workspace_bytes(self, batch, q_len, max_len):
+        return lib.b2_span_attn_tokens_workspace_bytes(self.h, batch, q_len, max_len)
+
+    def run_tokens(self, q, cache, new_lens, q_len, max_len, ws, out=None, scale=None):
+        """Multi-token attention: q [batch*q_len, nH*128]; row b*q_len + t attends to tokens 0 .. new_lens[b] - q_len + t."""
+        B = q.shape[0] // q_len
+        if out is None:
+            out = torch.empty_like(q)
+        if scale is None:
+            scale = 1.0 / (self.cfg.head_size ** 0.5)
+        wsb = ws.reserve(self.tokens_workspace_bytes(B, q_len, max_len))
+        check(lib.b2_span_attn_run_tokens(self.h, _ptr(out), _ptr(q), _ptr(cache.k_tab), _ptr(cache.v_tab), _ptr(new_lens), B,
+                                          int(q_len), int(max_len), _ptr(wsb), wsb.numel(), float(scale), _stream()),
+              "b2_span_attn_run_tokens")
         return out
 
     def algo_bytes(self, total_tokens):

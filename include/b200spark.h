@@ -232,6 +232,25 @@ int b2_span_attn_run(b2_span_attn_t handle, void* out, const void* q, const void
 /* Algorithmic KV bytes for a given total token count (sum of lens): 2 * n_groups * (row + param). */
 size_t b2_span_attn_algo_bytes(const b2_span_cfg* cfg, int64_t total_tokens);
 
+/* ---- Multi-token decode steps (speculative decoding: verify up to 16 drafted tokens per sequence in one step).
+ * Layout: with q_len = T, row b*T + t of every activation (qkv, q, out) holds token t of sequence b.  Head 128 only
+ * (B2_ERR_UNSUPPORTED otherwise); 1 <= q_len <= 16 (B2_ERR_LIMIT otherwise).
+ *
+ * Append: row (b, t) of qkv [batch*q_len, (n_heads + 2*n_groups) * 128] is written at position old_lens[b] + t (fused rotary
+ * at that position) and its q heads go to q_out [batch*q_len, n_heads * 128].  The span bytes and {zero, scale} equal those
+ * of q_len successive b2_span_cache_append calls. */
+int b2_span_cache_append_tokens(const b2_span_cfg* cfg, void* const* k_spans, void* const* v_spans, void* q_out,
+                                const void* qkv, const int32_t* old_lens, int batch, int q_len, const b2_rope_cfg* rope,
+                                void* stream);
+/* Attention: q, out [batch*q_len, n_heads*128]; row (b, t) attends to tokens 0 .. new_lens[b] - q_len + t (itself and the
+ * tokens before it).  Precondition new_lens[b] >= q_len.  batch * q_len <= the handle's max_batch (B2_ERR_LIMIT).  The
+ * q-heads of whole tokens share the 16 rows of one MMA tile (floor(16 / (n_heads/n_groups)) tokens per row block), so K and
+ * V are read once per row block. */
+size_t b2_span_attn_tokens_workspace_bytes(b2_span_attn_t handle, int batch, int q_len, int max_len);
+int b2_span_attn_run_tokens(b2_span_attn_t handle, void* out, const void* q, const void* const* k_spans,
+                            const void* const* v_spans, const int32_t* new_lens, int batch, int q_len, int max_len,
+                            void* workspace, size_t workspace_bytes, float qk_scale, void* stream);
+
 /* =====================================================================================
  * Glue ops of the decode graph ("next" rows): element-wise / norm / lookup, FT = bf16.
  * ===================================================================================== */
@@ -260,6 +279,14 @@ int b2_argmax_shard(int64_t* ids_out, float* vals_out, const void* logits, int b
 int b2_argmax_merge(int64_t* ids_out, const float* all_vals, const int64_t* all_ids, int nranks, int batch, void* stream);
 /* lens[b] += delta for b < batch (keeps sequence lengths device-resident under CUDA graphs) */
 int b2_lens_add(int32_t* lens, int batch, int delta, void* stream);
+/* Greedy verification of a multi-token step, on the device (CUDA-graph replayable).  tokens [batch][q_len] int64: column 0
+ * is the last emitted token, columns 1.. the draft; pred [batch][q_len] = argmax of the step's rows.
+ *   n_b = 1 + the number of leading i >= 1 with tokens[b][i] == pred[b][i-1]
+ * writes accepted[b] = n_b (int32), next_ids[b] = pred[b][n_b-1] (may be NULL) and tokens[b][0] = pred[b][n_b-1] (the last
+ * emitted token of the next step); old_lens[b] += n_b, new_lens[b] = old_lens[b] + q_len.  The emitted tokens of the step are
+ * pred[b][0 .. n_b-1].  Rows of rejected drafts stay in the cache; the next step overwrites them. */
+int b2_spec_accept(int32_t* accepted, int64_t* next_ids, int32_t* old_lens, int32_t* new_lens, int64_t* tokens,
+                   const int64_t* pred, int batch, int q_len, void* stream);
 
 /* =====================================================================================
  * Tensor-parallel exchange over NVLink peer memory (replaces AllReduceOp / ncclAllReduce for the decode step's
