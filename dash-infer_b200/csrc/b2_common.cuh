@@ -126,6 +126,25 @@ __device__ __forceinline__ float ld_dsmem_f(uint32_t addr) {
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
+// ---- draft trees of speculative verification (tree format: include/b200spark.h, "Tree-structured verification").
+// par = parents[b][0 .. q_len-1]: node t >= 1 hangs below par[t] in [0, t); par[0] is ignored.  A parent outside [0, t) is
+// a caller error; it is read as the root, so every walk stays inside the row and ends within t steps.
+__device__ __forceinline__ int tree_parent(const int32_t* par, int t) {
+  const int p = par[t];
+  return (unsigned)p < (unsigned)t ? p : 0;
+}
+// anc(t): bit j set for t and each of its ancestors j; depth: the parent steps from t to node 0 (the root).  A chain
+// (par[t] = t - 1) gives bits 0..t and depth t.
+__device__ __forceinline__ unsigned tree_walk(const int32_t* par, int t, int& depth) {
+  unsigned anc = 1u << t;
+  depth = 0;
+  for (int u = t; u > 0; ++depth) {
+    u = tree_parent(par, u);
+    anc |= 1u << u;
+  }
+  return anc;
+}
+
 // ---- mbarrier
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");

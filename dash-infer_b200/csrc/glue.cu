@@ -285,6 +285,36 @@ __global__ void spec_accept_kernel(int32_t* accepted, int64_t* next_ids, int32_t
   new_lens[b] = ol + q_len;
 }
 
+// greedy verification of a draft tree: from the root u = 0, step to the lowest-index child c of u (tree_parent(c) == u) with
+// tokens[b][c] == pred[b][u] while there is one.  Children have larger indices than their parent, so one pass over c finds
+// the path; a chain gives spec_accept_kernel's result.
+__global__ void spec_accept_tree_kernel(int32_t* accepted, int32_t* path, int64_t* next_ids, int32_t* old_lens, int32_t* new_lens,
+                                        int64_t* tokens, const int64_t* pred, const int32_t* parents, int batch, int q_len) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= batch) return;
+  const int64_t* tk = tokens + (size_t)b * q_len;
+  const int64_t* pr = pred + (size_t)b * q_len;
+  const int32_t* par = parents + (size_t)b * q_len;
+  int32_t* pa = path + (size_t)b * q_len;
+  int n = 1, u = 0;
+  pa[0] = 0;
+  for (int c = 1; c < q_len; ++c) {
+    if (tree_parent(par, c) == u && tk[c] == pr[u]) {
+      pa[n++] = c;
+      u = c;
+    }
+  }
+  const int64_t next = pr[u];
+  accepted[b] = n;
+  if (next_ids) next_ids[b] = next;
+  tokens[(size_t)b * q_len] = next;
+  const int ol = old_lens[b] + n;
+  old_lens[b] = ol;
+  new_lens[b] = ol + q_len;
+}
+
 // vocab-split lm_head: pick the global winner among the ranks' (max, argmax) pairs; ties -> lowest rank == lowest vocab id
 __global__ void argmax_merge_kernel(int64_t* ids_out, const float* vals, const int64_t* ids, int nranks, int batch) {
   pdl_wait();
@@ -416,6 +446,15 @@ int b2_spec_accept(int32_t* accepted, int64_t* next_ids, int32_t* old_lens, int3
   if (q_len < 1 || q_len > 16) return B2_ERR_LIMIT;
   B2_LAUNCH_CHECK("spec_accept", launch(spec_accept_kernel, dim3((batch + 127) / 128), dim3(128), 0, (cudaStream_t)stream, true,
                                         accepted, next_ids, old_lens, new_lens, tokens, pred, batch, q_len));
+  return B2_OK;
+}
+
+int b2_spec_accept_tree(int32_t* accepted, int32_t* path, int64_t* next_ids, int32_t* old_lens, int32_t* new_lens, int64_t* tokens,
+                        const int64_t* pred, const int32_t* parents, int batch, int q_len, void* stream) {
+  if (!accepted || !path || !old_lens || !new_lens || !tokens || !pred || !parents || batch <= 0) return B2_ERR_PARAM;
+  if (q_len < 1 || q_len > 16) return B2_ERR_LIMIT;
+  B2_LAUNCH_CHECK("spec_accept_tree", launch(spec_accept_tree_kernel, dim3((batch + 127) / 128), dim3(128), 0, (cudaStream_t)stream,
+                                             true, accepted, path, next_ids, old_lens, new_lens, tokens, pred, parents, batch, q_len));
   return B2_OK;
 }
 

@@ -25,6 +25,7 @@ constexpr int kAttnThreads = 128;  // 4 warps, 16 tokens of each 64-token tile p
 constexpr int kTile = 64;
 constexpr int kHead = 128;
 constexpr int kMaxBatch = 1024;
+constexpr int kMaxQLen = 16;  // tokens per sequence of a multi-token step (draft-tree nodes: a 16-bit ancestor mask)
 constexpr int kMergeRS = 136;  // padded fp32 row stride of the merge buffer (conflict-free float2 stores)
 constexpr int kMergeDirect = 16;  // up to this many pieces per (sequence, kv-head): the last CTA merges them all
 constexpr int kMergeFan = 8;      // above: groups of 8 pieces are merged by their last CTA, the last group merges the groups
@@ -53,8 +54,19 @@ struct AttnParams {
 struct AttnTokParams : AttnParams {
   int q_len, tpb, nrb, rstride;
 };
-template <bool MT>
-using AttnArgs = std::conditional_t<MT, AttnTokParams, AttnParams>;
+// Tree form (span_attn_kernel<..., MT = true, TREE = true>): the q_len rows of a sequence are the nodes of a draft tree.
+//   parents [batch][q_len] int32: node t >= 1 hangs below parents[b][t] in [0, t) (topological order); node 0 is the
+//   root (the last emitted token) and parents[b][0] is ignored.  depth(t) = parent steps from t to 0; anc(t) = the 16-bit
+//   mask of t and its ancestors (tree_walk in b2_common.cuh, shared with the append and the accept kernels).
+//   Node t sits in slot lens[b] - q_len + t and carries rotary position lens[b] - q_len + depth(t); row t attends to the
+//   prefix (tokens < lens[b] - q_len) and to the slots lens[b] - q_len + j, j in anc(t).  A chain (parents[t] = t - 1) is
+//   the plain multi-token step.  Malformed parents read as the root (tree_parent): results unspecified, accesses in bounds.
+// A node's ancestors have smaller indices, so a row block streams the same tiles as in the chain form.
+struct AttnTreeParams : AttnTokParams {
+  const int32_t* parents;
+};
+template <bool MT, bool TREE = false>
+using AttnArgs = std::conditional_t<TREE, AttnTreeParams, std::conditional_t<MT, AttnTokParams, AttnParams>>;
 
 // ---- span format (one description for the writers, the tile loader, the tile math and the host sizes) ----
 // A span holds span_len tokens of one sequence for all n_groups kv-heads (the wire format of decoder_cache_append.cuh:33-92):
@@ -192,12 +204,19 @@ __device__ __forceinline__ void softmax_sum(float (&psum)[2], float (&lrow)[2], 
   }
 }
 
+// Tree form: is token tok visible to the thread's row rr (0: gq, 1: gq+8)?  lim[rr] is the prefix end; past it, the token's
+// draft slot tok - lim[rr] must be in the row's ancestor mask am[rr] (tok < tok1 <= the block's length keeps it below 16).
+__device__ __forceinline__ bool tree_visible(int tok, int tok1, const int (&lim)[2], const unsigned (&am)[2], int rr) {
+  return tok < lim[rr] || (tok < tok1 && ((am[rr] >> (tok - lim[rr])) & 1u));
+}
+
 // One 64-token tile of attention math for this warp's 16-token slice (cache in the 16-bit type FT: bf16, or fp16 when H).
-// Tokens >= tok1 are masked; multi-token (MT): rows gq and gq+8 are masked at their own limits lim[0] and lim[1] (<= tok1).
-template <bool H, bool MT>
+// Tokens >= tok1 are masked; multi-token (MT): rows gq and gq+8 are masked at their own limits lim[0] and lim[1] (<= tok1);
+// tree (TREE): at their prefix ends lim[] and ancestor masks am[] (tree_visible above).
+template <bool H, bool MT, bool TREE = false>
 __device__ __forceinline__ void tile_compute_bf16(const uint8_t* st, int warp, int lane, int wtok, int tok1, const int (&lim)[2],
-                                                  float scale_log2, const uint32_t (&qa)[8][4], float (&o)[16][4],
-                                                  float (&mrow)[2], float (&lrow)[2]) {
+                                                  const unsigned (&am)[2], float scale_log2, const uint32_t (&qa)[8][4],
+                                                  float (&o)[16][4], float (&mrow)[2], float (&lrow)[2]) {
   using T = KVTraits<B2_KV_NONE>;
   const int t = lane & 3;
   const uint32_t kb = smem_u32(st), vb = kb + T::TILE;
@@ -224,7 +243,9 @@ __device__ __forceinline__ void tile_compute_bf16(const uint8_t* st, int warp, i
 #pragma unroll
     for (int cc = 0; cc < 4; ++cc) {
       const int tok = wtok + nt * 8 + 2 * t + (cc & 1);
-      const float v = tok < (MT ? lim[cc >> 1] : tok1) ? sc[nt][cc] * scale_log2 : -INFINITY;
+      float v;
+      if constexpr (TREE) v = tree_visible(tok, tok1, lim, am, cc >> 1) ? sc[nt][cc] * scale_log2 : -INFINITY;
+      else v = tok < (MT ? lim[cc >> 1] : tok1) ? sc[nt][cc] * scale_log2 : -INFINITY;
       sc[nt][cc] = v;
       mx[cc >> 1] = fmaxf(mx[cc >> 1], v);
     }
@@ -281,9 +302,9 @@ __device__ __forceinline__ uint32_t e4m3x2_to_f16x2(uint32_t w) {
   return d;
 }
 
-template <int QM, bool MT>
+template <int QM, bool MT, bool TREE = false>
 __device__ __forceinline__ void tile_compute_q(const uint8_t* st, int warp, int lane, int wtok, int tok1, const int (&lim)[2],
-                                               float scale_log2, const uint32_t (&qa)[8][4], const float (&sq)[2],
+                                               const unsigned (&am)[2], float scale_log2, const uint32_t (&qa)[8][4], const float (&sq)[2],
                                                float (&o)[16][4], float (&mrow)[2], float (&lrow)[2], float (&cacc)[2]) {
   using T = KVTraits<QM>;
   constexpr float BIAS = QM == B2_KV_I8 ? 1152.f : 1024.f;
@@ -346,7 +367,9 @@ __device__ __forceinline__ void tile_compute_q(const uint8_t* st, int warp, int 
       const int tok = wtok + nt * 8 + 2 * t + (cc & 1);
       const float kz = (cc & 1) ? kp.z : kp.x, ksc = (cc & 1) ? kp.w : kp.y;
       const float raw = T::kZeroPoint ? ksc * (sc[nt][cc] - (BIAS + kz) * sq[cc >> 1]) : ksc * sc[nt][cc];
-      const float v = tok < (MT ? lim[cc >> 1] : tok1) ? raw * scale_log2 : -INFINITY;
+      float v;
+      if constexpr (TREE) v = tree_visible(tok, tok1, lim, am, cc >> 1) ? raw * scale_log2 : -INFINITY;
+      else v = tok < (MT ? lim[cc >> 1] : tok1) ? raw * scale_log2 : -INFINITY;
       sc[nt][cc] = v;
       mx[cc >> 1] = fmaxf(mx[cc >> 1], v);
     }
@@ -551,8 +574,8 @@ __device__ __forceinline__ size_t tok_row(const AttnTokParams& p, int b, int qt0
   return ((size_t)b * p.q_len + qt0 + r / p.hpg) * p.n_heads * kHead + ((size_t)g * p.hpg + r % p.hpg) * kHead;
 }
 
-template <int QM, bool H, bool MT = false>
-__global__ void __launch_bounds__(kAttnThreads) span_attn_kernel(const AttnArgs<MT> p) {
+template <int QM, bool H, bool MT = false, bool TREE = false>
+__global__ void __launch_bounds__(kAttnThreads) span_attn_kernel(const AttnArgs<MT, TREE> p) {
   using F = Ft<H>;  // the 16-bit type of Q, the output and an unquantized cache
   using T = KVTraits<QM>;
   extern __shared__ __align__(128) uint8_t smem[];
@@ -645,8 +668,10 @@ __global__ void __launch_bounds__(kAttnThreads) span_attn_kernel(const AttnArgs<
     const void* const* vtab = p.v_spans + (size_t)b * p.max_spans;
     // multi-token: this row block's tokens qt0 .. qt0+ntok-1 sit in MMA rows 0 .. nrows-1 (row r: token qt0 + r / hpg,
     // head r % hpg).  Row r sees the tokens before len - ntok + 1 + r / hpg (lim[] for the thread's rows gq and gq+8).
+    // Tree: lim[] is the prefix end len - ntok - qt0 and am[] the row's ancestor mask (a dead row: lim = len, am = 0).
     int nrows, rstride, qt0;  // live rows, rows of a partial slot (set below, next to the single-token kernel's first use of hpg)
     int lim[2];
+    unsigned am[2];
 
     // ---- start streaming: the piece's first nstage-1 tiles are requested NOW (span-table lookups + cp.async), so their
     //      HBM latency overlaps the load of the query rows below
@@ -674,7 +699,13 @@ __global__ void __launch_bounds__(kAttnThreads) span_attn_kernel(const AttnArgs<
 #pragma unroll
         for (int rr = 0; rr < 2; ++rr) {
           const int r = gq + 8 * rr;
-          lim[rr] = r < nrows ? len - ntok + 1 + r / p.hpg : len;
+          if constexpr (TREE) {
+            int depth;
+            am[rr] = r < nrows ? tree_walk(p.parents + (size_t)b * p.q_len, qt0 + r / p.hpg, depth) : 0u;
+            lim[rr] = r < nrows ? len - ntok - qt0 : len;
+          } else {
+            lim[rr] = r < nrows ? len - ntok + 1 + r / p.hpg : len;
+          }
         }
       } else {
         nrows = rstride = p.hpg;
@@ -753,8 +784,9 @@ __global__ void __launch_bounds__(kAttnThreads) span_attn_kernel(const AttnArgs<
       if (tr0 && i == 0) B2_TR(g_attn_tr, 4);
       const int wtok = tok0 + i * kTile + warp * 16;  // first token of this warp's slice
       if (wtok < tok1) {
-        if constexpr (!T::kCodesF16) tile_compute_bf16<H, MT>(smem + slot * T::STAGE, warp, lane, wtok, tok1, lim, p.scale_log2, qa, o, mrow, lrow);
-        else tile_compute_q<QM, MT>(smem + slot * T::STAGE, warp, lane, wtok, tok1, lim, p.scale_log2, qa, sq, o, mrow, lrow, cacc);
+        if constexpr (!T::kCodesF16)
+          tile_compute_bf16<H, MT, TREE>(smem + slot * T::STAGE, warp, lane, wtok, tok1, lim, am, p.scale_log2, qa, o, mrow, lrow);
+        else tile_compute_q<QM, MT, TREE>(smem + slot * T::STAGE, warp, lane, wtok, tok1, lim, am, p.scale_log2, qa, sq, o, mrow, lrow, cacc);
       }
       __syncthreads();  // this stage may be refilled by the next iteration's prefetch
       slot = slot + 1 == p.nstage ? 0 : slot + 1;
@@ -1026,10 +1058,16 @@ struct AppendParams {
   int q_len;       // multi-token form: rows per sequence
 };
 
+// tree form: the draft tree of each sequence (format: AttnTreeParams)
+struct AppendTreeParams : AppendParams {
+  const int32_t* parents;
+};
+
 // MT = false: row b of qkv / q_out is sequence b, written at position old_lens[b].  MT = true: row b*q_len + t is token t of
-// sequence b, written at position old_lens[b] + t.
-template <int QM, bool H, bool MT = false>
-__global__ void __launch_bounds__(128) cache_append_kernel(const AppendParams p) {
+// sequence b, written at position old_lens[b] + t.  TREE (with MT): written at slot old_lens[b] + t, rotary position
+// old_lens[b] + depth(t).
+template <int QM, bool H, bool MT = false, bool TREE = false>
+__global__ void __launch_bounds__(128) cache_append_kernel(const std::conditional_t<TREE, AppendTreeParams, AppendParams> p) {
   using F = Ft<H>;
   pdl_wait();
   pdl_launch_dependents();
@@ -1042,7 +1080,13 @@ __global__ void __launch_bounds__(128) cache_append_kernel(const AppendParams p)
   const __nv_bfloat16* src = p.qkv + ((size_t)row * slots + slot) * kHead + lane * 4;
   const uint2 raw = *reinterpret_cast<const uint2*>(src);
   float x[4] = {F::lo(raw.x), F::hi(raw.x), F::lo(raw.y), F::hi(raw.y)};
-  const int pos = MT ? p.old_lens[b] + (row - b * p.q_len) : p.old_lens[b];
+  int pos = MT ? p.old_lens[b] + (row - b * p.q_len) : p.old_lens[b];  // the rotary position, and the slot unless TREE
+  const int wpos = pos;
+  if constexpr (TREE) {
+    int depth;
+    tree_walk(p.parents + (size_t)b * p.q_len, row - b * p.q_len, depth);
+    pos = p.old_lens[b] + depth;
+  }
   const bool is_v = slot >= p.n_heads + p.n_groups;
 
   if (p.rope && !is_v) {
@@ -1074,10 +1118,72 @@ __global__ void __launch_bounds__(128) cache_append_kernel(const AppendParams p)
   }
   const int g = is_v ? slot - p.n_heads - p.n_groups : slot - p.n_heads;
   void* const* tab = (is_v ? p.v_spans : p.k_spans) + (size_t)b * p.max_spans;
-  const int si = pos >> p.span_shift, ps = pos & (p.span_len - 1);
+  const int si = wpos >> p.span_shift, ps = wpos & (p.span_len - 1);
   uint8_t* span = reinterpret_cast<uint8_t*>(tab[si]);
   const size_t rowi = (size_t)g * p.span_len + ps;
   store_row<QM, H>(span, rowi, p.n_groups * p.span_len, lane, x);
+}
+
+// ------------------------------------------------------------------------------------------------
+// compaction after tree acceptance: the accepted path's rows (slots base + path[i]) move to slots base + i, for every layer.
+// One warp per (layer, sequence, K or V, kv-head) reads all of its source rows (and their {zero, scale}) before it writes
+// any: path[j] == i for j < i is possible (path [0, 2, 3] reads slot 2 while slot 2 is being written).  A row carries RoPE at
+// base + depth = base + i already, so the copy is exact bytes.
+// ------------------------------------------------------------------------------------------------
+struct CompactParams {
+  void* const* const* k_tables;  // [n_layers] -> span table [batch][max_spans]
+  void* const* const* v_tables;
+  const int32_t* old_lens;       // as b2_spec_accept_tree left them: base = old_lens[b] - accepted[b]
+  const int32_t* accepted;
+  const int32_t* path;           // [batch][q_len]
+  int n_layers, batch, q_len, n_groups, span_len, span_shift, max_spans;
+};
+
+template <int QM>
+__global__ void __launch_bounds__(128) cache_compact_kernel(const CompactParams p) {
+  using T = KVTraits<QM>;
+  constexpr int BPL = T::ROW / 32;  // row bytes per lane: 8 / 4 / 2
+  using Chunk = std::conditional_t<BPL == 8, uint2, std::conditional_t<BPL == 4, uint32_t, uint16_t>>;
+  pdl_wait();
+  pdl_launch_dependents();
+  const int lane = threadIdx.x & 31;
+  const int wid = blockIdx.x * 4 + (threadIdx.x >> 5);
+  if (wid >= p.n_layers * p.batch * 2 * p.n_groups) return;
+  const int g = wid % p.n_groups, which = (wid / p.n_groups) & 1;
+  const int b = (wid / (2 * p.n_groups)) % p.batch, layer = wid / (2 * p.n_groups * p.batch);
+  const int n = min(max(p.accepted[b], 1), p.q_len);
+  const int base = p.old_lens[b] - n;
+  const int32_t* path = p.path + (size_t)b * p.q_len;
+  void* const* tab = (which ? p.v_tables : p.k_tables)[layer] + (size_t)b * p.max_spans;
+  const size_t n_rows = (size_t)p.n_groups * p.span_len;
+  auto row_of = [&](int s, uint8_t*& span) {  // span and row index of slot s
+    span = reinterpret_cast<uint8_t*>(tab[s >> p.span_shift]);
+    return (size_t)g * p.span_len + (s & (p.span_len - 1));
+  };
+  Chunk buf[kMaxQLen];
+  float2 prm = make_float2(0.f, 0.f);
+  int src[kMaxQLen];
+#pragma unroll
+  for (int i = 1; i < kMaxQLen; ++i) {
+    const int j = i < n ? path[i] : i;
+    src[i] = (unsigned)j < (unsigned)p.q_len ? j : i;  // a malformed path entry: no move
+    if (src[i] != i) {
+      uint8_t* span;
+      const size_t r = row_of(base + src[i], span);
+      buf[i] = *reinterpret_cast<const Chunk*>(span + r * T::ROW + lane * BPL);
+      if (T::kCodesF16 && lane == i) prm = *reinterpret_cast<const float2*>(span + T::param_offset(n_rows, r));
+    }
+  }
+  __syncwarp();
+#pragma unroll
+  for (int i = 1; i < kMaxQLen; ++i) {
+    if (src[i] != i) {
+      uint8_t* span;
+      const size_t r = row_of(base + i, span);
+      *reinterpret_cast<Chunk*>(span + r * T::ROW + lane * BPL) = buf[i];
+      if (T::kCodesF16 && lane == i) *reinterpret_cast<float2*>(span + T::param_offset(n_rows, r)) = prm;
+    }
+  }
 }
 
 int span_attn64_run(const b2_span_cfg* c, void* out, const void* q, const void* const* k_spans, const void* const* v_spans,
@@ -1123,6 +1229,12 @@ static attn_tok_kernel_t attn_tok_kernel_for(const b2_span_cfg* c) {
     return with_flag(c->ft == B2_DT_F16, [&](auto H) -> attn_tok_kernel_t { return span_attn_kernel<QM, H, true>; });
   });
 }
+typedef void (*attn_tree_kernel_t)(const AttnTreeParams);
+static attn_tree_kernel_t attn_tree_kernel_for(const b2_span_cfg* c) {
+  return with_kv_mode(c->quant_mode, [&](auto QM) {
+    return with_flag(c->ft == B2_DT_F16, [&](auto H) -> attn_tree_kernel_t { return span_attn_kernel<QM, H, true, true>; });
+  });
+}
 
 // multi-token row blocks: whole tokens per block of 16 MMA rows
 static int tokens_per_block(const b2_span_cfg* c, int q_len) {
@@ -1158,6 +1270,7 @@ int b2_span_attn_create(b2_span_attn_t* out, const b2_span_cfg* cfg, int max_bat
   h->max_batch = max_batch;
   attn_kernel_t kern = attn_kernel_for(cfg);
   attn_tok_kernel_t kern_mt = attn_tok_kernel_for(cfg);
+  attn_tree_kernel_t kern_tree = attn_tree_kernel_for(cfg);
   int sb = 0;
   with_kv_mode(cfg->quant_mode, [&](auto QM) {
     sb = KVTraits<QM>::STAGE;
@@ -1169,6 +1282,7 @@ int b2_span_attn_create(b2_span_attn_t* out, const b2_span_cfg* cfg, int max_bat
   h->smem = h->nstage * sb > merge ? h->nstage * sb : merge;
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem);
   if (e == cudaSuccess && cfg->head_size == kHead) e = cudaFuncSetAttribute(kern_mt, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem);
+  if (e == cudaSuccess && cfg->head_size == kHead) e = cudaFuncSetAttribute(kern_tree, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem);
   int occ = 1;
   if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, kAttnThreads, h->smem);
   if (e != cudaSuccess) {
@@ -1214,11 +1328,13 @@ static size_t attn_workspace_bytes(const b2_span_attn* h, int rows) {
   return 2 * partial_slots(h) * rows * (kHead + 2) * sizeof(float) + 256;
 }
 
-// q_len == 0: the single-token kernel; otherwise the multi-token one
+// q_len == 0: the single-token kernel; otherwise the multi-token one, in its tree form when parents != NULL
 static int attn_launch(b2_span_attn_t h, void* out, const void* q, const void* const* k_spans, const void* const* v_spans,
-                       const int32_t* new_lens, int batch, int q_len, void* workspace, float qk_scale, void* stream_) {
+                       const int32_t* new_lens, int batch, int q_len, void* workspace, float qk_scale, void* stream_,
+                       const int32_t* parents = nullptr) {
   const int hpg = h->cfg.n_heads / h->cfg.n_groups;
-  AttnTokParams p;
+  AttnTreeParams p;
+  p.parents = parents;
   p.q_len = q_len;
   p.tpb = q_len ? tokens_per_block(&h->cfg, q_len) : 1;
   p.nrb = q_len ? (q_len + p.tpb - 1) / p.tpb : 1;
@@ -1241,10 +1357,12 @@ static int attn_launch(b2_span_attn_t h, void* out, const void* q, const void* c
   p.span_len = h->cfg.span_len; p.span_shift = ilog2(h->cfg.span_len); p.max_spans = h->cfg.max_spans_per_seq;
   p.nstage = h->nstage;
   p.scale_log2 = qk_scale * 1.4426950408889634f;
-  const cudaError_t e = q_len ? launch(attn_tok_kernel_for(&h->cfg), dim3(h->grid), dim3(kAttnThreads), (size_t)h->smem,
-                                        (cudaStream_t)stream_, true, p)
-                             : launch(attn_kernel_for(&h->cfg), dim3(h->grid), dim3(kAttnThreads), (size_t)h->smem,
-                                      (cudaStream_t)stream_, true, static_cast<const AttnParams&>(p));
+  const cudaError_t e =
+      parents ? launch(attn_tree_kernel_for(&h->cfg), dim3(h->grid), dim3(kAttnThreads), (size_t)h->smem, (cudaStream_t)stream_, true, p)
+      : q_len ? launch(attn_tok_kernel_for(&h->cfg), dim3(h->grid), dim3(kAttnThreads), (size_t)h->smem, (cudaStream_t)stream_, true,
+                       static_cast<const AttnTokParams&>(p))
+              : launch(attn_kernel_for(&h->cfg), dim3(h->grid), dim3(kAttnThreads), (size_t)h->smem,
+                       (cudaStream_t)stream_, true, static_cast<const AttnParams&>(p));
   if (e != cudaSuccess) {
     set_last_error("span_attn launch", e);
     return B2_ERR_CUDA;
@@ -1286,6 +1404,17 @@ int b2_span_attn_run_tokens(b2_span_attn_t h, void* out, const void* q, const vo
   return attn_launch(h, out, q, k_spans, v_spans, new_lens, batch, q_len, workspace, qk_scale, stream_);
 }
 
+int b2_span_attn_run_tree(b2_span_attn_t h, void* out, const void* q, const void* const* k_spans, const void* const* v_spans,
+                          const int32_t* new_lens, const int32_t* parents, int batch, int q_len, int max_len, void* workspace,
+                          size_t workspace_bytes, float qk_scale, void* stream_) {
+  if (!h || !out || !q || !k_spans || !v_spans || !new_lens || !parents) return B2_ERR_PARAM;
+  if (h->cfg.head_size != kHead) return B2_ERR_UNSUPPORTED;
+  if (q_len < 1 || q_len > kMaxQLen || batch <= 0 || (int64_t)batch * q_len > h->max_batch) return B2_ERR_LIMIT;
+  if (max_len <= 0 || (int64_t)(max_len + h->cfg.span_len - 1) / h->cfg.span_len > h->cfg.max_spans_per_seq) return B2_ERR_LIMIT;
+  if (!workspace || workspace_bytes < b2_span_attn_tokens_workspace_bytes(h, batch, q_len, max_len)) return B2_ERR_PARAM;
+  return attn_launch(h, out, q, k_spans, v_spans, new_lens, batch, q_len, workspace, qk_scale, stream_, parents);
+}
+
 int b2_span_context_copy(const b2_span_cfg* cfg, void* const* spans, const void* src, int64_t token_stride, int seq_len,
                          void* stream_) {
   if (int st = check_cfg(cfg)) return st;
@@ -1312,11 +1441,14 @@ int b2_span_context_copy(const b2_span_cfg* cfg, void* const* spans, const void*
 
 }  // extern "C"
 
-// q_len == 0: one row per sequence (cache_append_kernel<..., MT = false>); otherwise q_len rows per sequence
+// q_len == 0: one row per sequence (cache_append_kernel<..., MT = false>); otherwise q_len rows per sequence, the nodes of a
+// draft tree when parents != NULL
 static int cache_append_launch(const b2_span_cfg* cfg, void* const* k_spans, void* const* v_spans, void* q_out, const void* qkv,
-                               const int32_t* old_lens, int batch, int q_len, const b2_rope_cfg* rope, void* stream_) {
+                               const int32_t* old_lens, int batch, int q_len, const b2_rope_cfg* rope, void* stream_,
+                               const int32_t* parents = nullptr) {
   if (rope && (rope->rotary_dim != 128 && rope->rotary_dim != 64)) return B2_ERR_UNSUPPORTED;
-  AppendParams p;
+  AppendTreeParams p;
+  p.parents = parents;
   p.k_spans = k_spans; p.v_spans = v_spans;
   p.q_out = (__nv_bfloat16*)q_out; p.qkv = (const __nv_bfloat16*)qkv; p.old_lens = old_lens;
   p.batch = batch; p.n_heads = cfg->n_heads; p.n_groups = cfg->n_groups;
@@ -1329,8 +1461,10 @@ static int cache_append_launch(const b2_span_cfg* cfg, void* const* k_spans, voi
   const dim3 grid((warps + 3) / 4), block(128);
   const cudaError_t e = with_kv_mode(cfg->quant_mode, [&](auto QM) {
     return with_flag(cfg->ft == B2_DT_F16, [&](auto H) {
+      if (parents) return launch(cache_append_kernel<QM, H, true, true>, grid, block, 0, (cudaStream_t)stream_, true, p);
       return with_flag(q_len != 0, [&](auto MT) {
-        return launch(cache_append_kernel<QM, H, MT>, grid, block, 0, (cudaStream_t)stream_, true, p);
+        return launch(cache_append_kernel<QM, H, MT>, grid, block, 0, (cudaStream_t)stream_, true,
+                      static_cast<const AppendParams&>(p));
       });
     });
   });
@@ -1358,6 +1492,41 @@ int b2_span_cache_append_tokens(const b2_span_cfg* cfg, void* const* k_spans, vo
   if (!k_spans || !v_spans || !q_out || !qkv || !old_lens || batch <= 0) return B2_ERR_PARAM;
   if (q_len < 1 || q_len > 16) return B2_ERR_LIMIT;
   return cache_append_launch(cfg, k_spans, v_spans, q_out, qkv, old_lens, batch, q_len, rope, stream_);
+}
+
+int b2_span_cache_append_tree(const b2_span_cfg* cfg, void* const* k_spans, void* const* v_spans, void* q_out, const void* qkv,
+                              const int32_t* old_lens, const int32_t* parents, int batch, int q_len, const b2_rope_cfg* rope,
+                              void* stream_) {
+  if (int st = check_cfg(cfg)) return st;
+  if (cfg->head_size != kHead) return B2_ERR_UNSUPPORTED;
+  if (!k_spans || !v_spans || !q_out || !qkv || !old_lens || !parents || batch <= 0) return B2_ERR_PARAM;
+  if (q_len < 1 || q_len > kMaxQLen) return B2_ERR_LIMIT;
+  return cache_append_launch(cfg, k_spans, v_spans, q_out, qkv, old_lens, batch, q_len, rope, stream_, parents);
+}
+
+int b2_span_cache_compact(const b2_span_cfg* cfg, void* const* const* k_tables, void* const* const* v_tables, int n_layers,
+                          const int32_t* old_lens, const int32_t* accepted, const int32_t* path, int batch, int q_len,
+                          void* stream_) {
+  if (int st = check_cfg(cfg)) return st;
+  if (cfg->head_size != kHead) return B2_ERR_UNSUPPORTED;
+  if (!k_tables || !v_tables || !old_lens || !accepted || !path || n_layers <= 0 || batch <= 0) return B2_ERR_PARAM;
+  if (q_len < 1 || q_len > kMaxQLen) return B2_ERR_LIMIT;
+  CompactParams p;
+  p.k_tables = k_tables; p.v_tables = v_tables;
+  p.old_lens = old_lens; p.accepted = accepted; p.path = path;
+  p.n_layers = n_layers; p.batch = batch; p.q_len = q_len; p.n_groups = cfg->n_groups;
+  p.span_len = cfg->span_len; p.span_shift = ilog2(cfg->span_len); p.max_spans = cfg->max_spans_per_seq;
+  const int64_t warps = (int64_t)n_layers * batch * 2 * cfg->n_groups;
+  if (warps > (int64_t)1 << 30) return B2_ERR_LIMIT;
+  const dim3 grid((unsigned)((warps + 3) / 4)), block(128);
+  const cudaError_t e = with_kv_mode(cfg->quant_mode, [&](auto QM) {
+    return launch(cache_compact_kernel<QM>, grid, block, 0, (cudaStream_t)stream_, true, p);
+  });
+  if (e != cudaSuccess) {
+    set_last_error("cache_compact launch", e);
+    return B2_ERR_CUDA;
+  }
+  return B2_OK;
 }
 
 }  // extern "C"

@@ -16,6 +16,7 @@ SYMBOLS = [
     "b2_span_bytes", "b2_span_cache_append", "b2_span_context_copy", "b2_span_attn_create", "b2_span_attn_destroy",
     "b2_span_attn_workspace_bytes", "b2_span_attn_run", "b2_span_attn_algo_bytes",
     "b2_span_cache_append_tokens", "b2_span_attn_tokens_workspace_bytes", "b2_span_attn_run_tokens", "b2_spec_accept",
+    "b2_span_cache_append_tree", "b2_span_attn_run_tree", "b2_spec_accept_tree", "b2_span_cache_compact",
     "b2_rmsnorm", "b2_rotary", "b2_binary", "b2_embedding", "b2_argmax", "b2_argmax_shard", "b2_argmax_merge", "b2_lens_add",
     "b2_rmsnorm_ft", "b2_binary_ft", "b2_argmax_ft",
     "b2_comm_create", "b2_comm_destroy", "b2_comm_buffer_bytes", "b2_comm_export", "b2_comm_connect", "b2_comm_connect_pointers",
@@ -94,6 +95,10 @@ def _load():
         "b2_span_attn_tokens_workspace_bytes": (sz, [vp, i32, i32, i32]),
         "b2_span_attn_run_tokens": (i32, [vp, vp, vp, vp, vp, vp, i32, i32, i32, vp, sz, f32, vp]),
         "b2_spec_accept": (i32, [vp, vp, vp, vp, vp, vp, i32, i32, vp]),
+        "b2_span_cache_append_tree": (i32, [C.POINTER(SpanCfg), vp, vp, vp, vp, vp, vp, i32, i32, C.POINTER(RopeCfg), vp]),
+        "b2_span_attn_run_tree": (i32, [vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, vp, sz, f32, vp]),
+        "b2_spec_accept_tree": (i32, [vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, vp]),
+        "b2_span_cache_compact": (i32, [C.POINTER(SpanCfg), vp, vp, i32, vp, vp, vp, i32, i32, vp]),
         "b2_rmsnorm": (i32, [vp, vp, vp, i32, i32, f32, vp]),
         "b2_rmsnorm_ft": (i32, [vp, vp, vp, i32, i32, f32, i32, vp]),
         "b2_binary_ft": (i32, [vp, vp, vp, i64, i32, i32, vp]),

@@ -123,20 +123,25 @@ class _RefView:
 class DecodeStack:
     def __init__(self, cfg, batch, max_len, wbits=4, group=-1, kv="none", span=128, seed=1234, device="cuda",
                  keep_ref=False, layers=None, tp_rank=0, tp_size=1, tp_group=None, fuse_swiglu=True, fuse_norm=False,
-                 collective=None, comm=None, dtype=torch.bfloat16, q_len=1):
+                 collective=None, comm=None, dtype=torch.bfloat16, q_len=1, tree=False):
         """tp_size > 1: the reference's tensor-parallel layout (QKV/gate/up column split, o/down row split + all-reduce,
         vocab-split lm_head + B-element all-gather); every rank builds the SAME full synthetic weights from `seed` and
         keeps its shard, exactly like the reference splits an already-quantized checkpoint.
         q_len = T > 1: multi-token verify steps (speculative decoding).  Every step runs T rows per sequence: self.tokens
         [B, T] holds the last emitted token (column 0, written by the step itself) and T-1 drafts (filled by the caller);
-        step() returns (pred [B, T], accepted [B]) and advances the lengths by the accepted counts on the device."""
+        step() returns (pred [B, T], accepted [B]) and advances the lengths by the accepted counts on the device.
+        tree=True (with q_len = T > 1): the T rows of a sequence are the nodes of a draft tree.  self.parents [B, T] int32
+        (tree format: include/b200spark.h) is filled by the caller next to self.tokens before each step; the step appends
+        and attends in tree form, accepts the longest greedy path and compacts the path's cache rows in every layer.
+        step() returns (pred [B, T], accepted [B], path [B, T]); the emitted tokens are pred[b, path[b, :accepted[b]]]."""
         global _DT
         assert dtype in (torch.bfloat16, torch.float16) and (dtype == torch.bfloat16 or (tp_size == 1 and cfg.head == 128)), \
             "fp16: single GPU, head size 128 (the communicator and the head-64 kernels are bf16)"
         assert 1 <= q_len <= 16 and (q_len == 1 or (tp_size == 1 and cfg.head == 128)), \
             "multi-token steps: q_len <= 16, single GPU, head size 128"
+        assert not tree or (q_len > 1 and tp_size == 1 and cfg.head == 128), "draft trees: q_len > 1, single GPU, head size 128"
         self.dtype = _DT = dtype
-        self.q_len = q_len
+        self.q_len, self.tree = q_len, tree
         rows = batch * q_len  # activation rows of a step
         self.cfg, self.B, self.max_len = cfg, batch, max_len
         self.tp_rank, self.tp, self.tp_group = tp_rank, tp_size, tp_group
@@ -196,6 +201,9 @@ class DecodeStack:
             self._tokens = torch.zeros(batch, q_len, dtype=torch.int64, device=device)
             self._pred = torch.zeros(batch, q_len, dtype=torch.int64, device=device)
             self._accepted = torch.zeros(batch, dtype=torch.int32, device=device)
+        if tree:  # a chain until the caller writes its trees
+            self._parents = (torch.arange(q_len, dtype=torch.int32, device=device) - 1).clamp_(min=0).repeat(batch, 1)
+            self._path = torch.zeros(batch, q_len, dtype=torch.int32, device=device)
         bf = dict(dtype=_DT, device=device)
         self._bufs = dict(x=torch.empty(rows, H, **bf), xn=torch.empty(rows, H, **bf),
                           qkv=torch.empty(rows, (nHl + 2 * nGl) * hd, **bf), q=torch.empty(rows, nHl * hd, **bf),
@@ -247,6 +255,8 @@ class DecodeStack:
         self.ids, self.next_ids = self._ids[:b], self._next_ids[:b]
         if self.q_len > 1:
             self.tokens, self.pred, self.accepted = self._tokens[:b], self._pred[:b], self._accepted[:b]
+        if self.tree:
+            self.parents, self.path = self._parents[:b], self._path[:b]
         self.graph = None
         assert not getattr(self, "fuse_norm", False) or b == self.Bmax, "the fused-norm statistics are laid out for one batch"
 
@@ -336,6 +346,9 @@ class DecodeStack:
             if T == 1:
                 ops.cache_append(L["cache"], self.qkv, self.lens_old, q_out=self.q, rope=self.rope); n += 1
                 self.attn(self.q, L["cache"], self.lens_new, self.max_len, ws, out=self.ao); n += 1
+            elif self.tree:
+                ops.cache_append_tree(L["cache"], self.qkv, self.lens_old, self.parents, T, q_out=self.q, rope=self.rope); n += 1
+                self.attn.run_tree(self.q, L["cache"], self.lens_new, self.parents, T, self.max_len, ws, out=self.ao); n += 1
             else:
                 ops.cache_append_tokens(L["cache"], self.qkv, self.lens_old, T, q_out=self.q, rope=self.rope); n += 1
                 self.attn.run_tokens(self.q, L["cache"], self.lens_new, T, self.max_len, ws, out=self.ao); n += 1
@@ -386,7 +399,11 @@ class DecodeStack:
                 self.comm.allgather(self.loc_val, self.all_val); n += 1
                 self.comm.allgather(self.loc_ids, self.all_ids); n += 1
             ops.argmax_merge(self.all_val, self.all_ids, out=self.next_ids); n += 1  # lowest rank on ties == lowest vocab id
-        if T > 1:  # greedy verification: accepted counts, next token and lengths stay on the device
+        if self.tree:  # greedy tree verification, then the accepted path's rows move to consecutive slots in every layer
+            ops.spec_accept_tree(self.accepted, self.path, self.next_ids, self.lens_old, self.lens_new, self.tokens, self.pred,
+                                 self.parents); n += 1
+            ops.cache_compact([L["cache"] for L in self.layers], self.lens_old, self.accepted, self.path, T); n += 1
+        elif T > 1:  # greedy verification: accepted counts, next token and lengths stay on the device
             ops.spec_accept(self.accepted, self.next_ids, self.lens_old, self.lens_new, self.tokens, self.pred); n += 1
         else:
             ops.lens_add(self.lens_old, 1); n += 1
@@ -400,11 +417,13 @@ class DecodeStack:
 
     def step(self):
         """q_len 1: returns next_ids [B].  q_len > 1: one verify step, returns (pred [B, T], accepted [B]); the step's
-        emitted tokens are pred[b, :accepted[b]]."""
+        emitted tokens are pred[b, :accepted[b]].  Tree: (pred, accepted, path [B, T]), emitted pred[b, path[b, :accepted[b]]]."""
         if self.graph is not None:
             self.graph.replay()
         else:
             self._step_ops()
+        if self.tree:
+            return self.pred, self.accepted, self.path
         return self.next_ids if self.q_len == 1 else (self.pred, self.accepted)
 
     def capture(self):

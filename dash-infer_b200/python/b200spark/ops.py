@@ -272,6 +272,57 @@ def spec_accept(accepted, next_ids, old_lens, new_lens, tokens, pred):
     return accepted
 
 
+def cache_append_tree(cache, qkv, old_lens, parents, q_len, q_out=None, rope=None):
+    """Draft-tree append (b2_span_cache_append_tree): row b*q_len + t of qkv is node t of sequence b's tree (parents int32
+    [B, q_len]), written at slot old_lens[b] + t with rotary position old_lens[b] + depth(t)."""
+    cfg = cache.cfg
+    rows = qkv.shape[0]
+    assert rows % q_len == 0 and parents.dtype == torch.int32 and parents.is_contiguous()
+    if q_out is None:
+        q_out = torch.empty(rows, cfg.n_heads * cfg.head_size, dtype=qkv.dtype, device=qkv.device)
+    r = RopeCfg(float(rope[0]), int(rope[1]), 0) if rope is not None else None
+    check(lib.b2_span_cache_append_tree(C.byref(cfg), _ptr(cache.k_tab), _ptr(cache.v_tab), _ptr(q_out), _ptr(qkv),
+                                        _ptr(old_lens), _ptr(parents), rows // q_len, int(q_len),
+                                        C.byref(r) if r is not None else None, _stream()), "b2_span_cache_append_tree")
+    return q_out
+
+
+def spec_accept_tree(accepted, path, next_ids, old_lens, new_lens, tokens, pred, parents):
+    """Greedy verification of a draft tree (b2_spec_accept_tree): tokens / pred int64 [B, T], parents int32 [B, T]; writes
+    accepted (int32 [B]), path (int32 [B, T], the first accepted[b] entries), next_ids (int64 [B] or None) and tokens[:, 0],
+    advances old_lens by the accepted counts and sets new_lens = old_lens + T."""
+    B, T = tokens.shape
+    assert tokens.is_contiguous() and pred.is_contiguous() and pred.shape == tokens.shape
+    assert parents.dtype == torch.int32 and parents.is_contiguous() and parents.shape == tokens.shape
+    assert path.dtype == torch.int32 and path.is_contiguous() and path.shape == tokens.shape
+    check(lib.b2_spec_accept_tree(_ptr(accepted), _ptr(path), _ptr(next_ids), _ptr(old_lens), _ptr(new_lens), _ptr(tokens),
+                                  _ptr(pred), _ptr(parents), B, T, _stream()), "b2_spec_accept_tree")
+    return accepted, path
+
+
+_COMPACT_TABLES = {}
+
+
+def compact_tables(caches):
+    """Device arrays of the caches' K and V span-table pointers (one per layer), built once per set of tables.  The key is
+    the tables' addresses, which are exactly what the arrays hold, so a cached entry is right for any caches at them."""
+    key = tuple((c.k_tab.data_ptr(), c.v_tab.data_ptr()) for c in caches)
+    if key not in _COMPACT_TABLES:
+        dev = caches[0].k_tab.device
+        _COMPACT_TABLES[key] = (torch.tensor([k for k, _ in key], dtype=torch.int64, device=dev),
+                                torch.tensor([v for _, v in key], dtype=torch.int64, device=dev))
+    return _COMPACT_TABLES[key]
+
+
+def cache_compact(caches, old_lens, accepted, path, q_len):
+    """After spec_accept_tree: move the accepted path's rows to consecutive slots in every cache (one per layer, all of one
+    config) with one launch (b2_span_cache_compact).  Call compact_tables(caches) once before capturing a CUDA graph."""
+    kt, vt = compact_tables(caches)
+    B = accepted.shape[0]
+    check(lib.b2_span_cache_compact(C.byref(caches[0].cfg), _ptr(kt), _ptr(vt), len(caches), _ptr(old_lens), _ptr(accepted),
+                                    _ptr(path), B, int(q_len), _stream()), "b2_span_cache_compact")
+
+
 def context_copy(cache, which, b, src, seq_len=None):
     """Prefill: write sequence b's K (which='k') or V ('v') rows src [seq, ..., n_groups*128 leading values per token] into its
     spans (b2_span_context_copy).  src may be a strided view (e.g. the K part of a fused qkv tensor)."""
@@ -316,6 +367,21 @@ class SpanAttn:
         check(lib.b2_span_attn_run_tokens(self.h, _ptr(out), _ptr(q), _ptr(cache.k_tab), _ptr(cache.v_tab), _ptr(new_lens), B,
                                           int(q_len), int(max_len), _ptr(wsb), wsb.numel(), float(scale), _stream()),
               "b2_span_attn_run_tokens")
+        return out
+
+    def run_tree(self, q, cache, new_lens, parents, q_len, max_len, ws, out=None, scale=None):
+        """Draft-tree attention: q [batch*q_len, nH*128]; row b*q_len + t attends to the prefix (tokens < new_lens[b] - q_len)
+        and to the slots new_lens[b] - q_len + j of t and its ancestors in parents (int32 [batch, q_len])."""
+        B = q.shape[0] // q_len
+        assert parents.dtype == torch.int32 and parents.is_contiguous()
+        if out is None:
+            out = torch.empty_like(q)
+        if scale is None:
+            scale = 1.0 / (self.cfg.head_size ** 0.5)
+        wsb = ws.reserve(self.tokens_workspace_bytes(B, q_len, max_len))
+        check(lib.b2_span_attn_run_tree(self.h, _ptr(out), _ptr(q), _ptr(cache.k_tab), _ptr(cache.v_tab), _ptr(new_lens),
+                                        _ptr(parents), B, int(q_len), int(max_len), _ptr(wsb), wsb.numel(), float(scale),
+                                        _stream()), "b2_span_attn_run_tree")
         return out
 
     def algo_bytes(self, total_tokens):

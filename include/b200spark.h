@@ -251,6 +251,27 @@ int b2_span_attn_run_tokens(b2_span_attn_t handle, void* out, const void* q, con
                             const void* const* v_spans, const int32_t* new_lens, int batch, int q_len, int max_len,
                             void* workspace, size_t workspace_bytes, float qk_scale, void* stream);
 
+/* ---- Tree-structured verification (Medusa / EAGLE-style draft trees).  The q_len rows of a sequence are the nodes of a
+ * draft tree; the layout, limits and handle rules of the multi-token entry points above apply.
+ * Tree format: parents [batch][q_len] int32, device-resident, filled by the caller before each step like the tokens.
+ *   Node 0 is the root (the last emitted token); parents[b][0] is ignored.  For t >= 1, parents[b][t] lies in [0, t): nodes
+ *   are in topological order.  Trees may differ per sequence.
+ *   depth(t) = the parent steps from t to node 0; anc(t) = the 16-bit mask of t and its ancestors.  Both are derived on the
+ *   device (a walk of at most q_len - 1 steps).
+ *   A chain (parents[b][t] = t - 1: depth t, anc bits 0..t) reproduces the multi-token entry points bit for bit.
+ *   Malformed parents are a caller error: results are unspecified, but no kernel reads or writes out of bounds or loops
+ *   without bound, for any int32 input.
+ *
+ * Append: row (b, t) is written at slot old_lens[b] + t, with fused rotary at position old_lens[b] + depth(t). */
+int b2_span_cache_append_tree(const b2_span_cfg* cfg, void* const* k_spans, void* const* v_spans, void* q_out, const void* qkv,
+                              const int32_t* old_lens, const int32_t* parents, int batch, int q_len, const b2_rope_cfg* rope,
+                              void* stream);
+/* Attention: row (b, t) attends to the prefix (tokens < new_lens[b] - q_len) and to the slots new_lens[b] - q_len + j for
+ * every j in anc(t).  Workspace: b2_span_attn_tokens_workspace_bytes. */
+int b2_span_attn_run_tree(b2_span_attn_t handle, void* out, const void* q, const void* const* k_spans,
+                          const void* const* v_spans, const int32_t* new_lens, const int32_t* parents, int batch, int q_len,
+                          int max_len, void* workspace, size_t workspace_bytes, float qk_scale, void* stream);
+
 /* =====================================================================================
  * Glue ops of the decode graph ("next" rows): element-wise / norm / lookup, FT = bf16.
  * ===================================================================================== */
@@ -287,6 +308,23 @@ int b2_lens_add(int32_t* lens, int batch, int delta, void* stream);
  * pred[b][0 .. n_b-1].  Rows of rejected drafts stay in the cache; the next step overwrites them. */
 int b2_spec_accept(int32_t* accepted, int64_t* next_ids, int32_t* old_lens, int32_t* new_lens, int64_t* tokens,
                    const int64_t* pred, int batch, int q_len, void* stream);
+/* Greedy verification of a draft tree (tree format: b2_span_cache_append_tree).  From u = 0: while some child c of u has
+ * tokens[b][c] == pred[b][u], take the lowest-index such c, append it to the path and set u = c.  Writes accepted[b] = n (the
+ * path length, >= 1), path[b][0 .. n-1] (int32 [batch][q_len], path[b][0] = 0; later entries untouched), next_ids[b] (may be
+ * NULL) = tokens[b][0] = pred[b][u]; old_lens[b] += n, new_lens[b] = old_lens[b] + q_len.  The emitted tokens of the step
+ * are pred[b][path[b][i]], i < n.  A chain gives b2_spec_accept's results. */
+int b2_spec_accept_tree(int32_t* accepted, int32_t* path, int64_t* next_ids, int32_t* old_lens, int32_t* new_lens,
+                        int64_t* tokens, const int64_t* pred, const int32_t* parents, int batch, int q_len, void* stream);
+/* Move the accepted path's K/V rows to consecutive slots, in every layer with one launch.  k_tables / v_tables: device
+ * arrays of n_layers span-table pointers (each table [batch][max_spans_per_seq], as for the other span entry points).  With
+ * base = old_lens[b] - accepted[b] (the lengths as b2_spec_accept_tree left them), slot base + path[b][i] is copied to slot
+ * base + i for 1 <= i < accepted[b] where path[b][i] != i: the row bytes of every kv-head of K and V, and their {zero,
+ * scale} in the quantized modes.  A node at depth i carries rotary position base + i already, so the copy is exact.  All
+ * source rows of a (sequence, layer, kv-head) are read before any is written (path [0, 2, 3] reads slot 2 while slot 2 is
+ * written).  Rows of rejected nodes stay; the next step overwrites them.  Head 128 only. */
+int b2_span_cache_compact(const b2_span_cfg* cfg, void* const* const* k_tables, void* const* const* v_tables, int n_layers,
+                          const int32_t* old_lens, const int32_t* accepted, const int32_t* path, int batch, int q_len,
+                          void* stream);
 
 /* =====================================================================================
  * Tensor-parallel exchange over NVLink peer memory (replaces AllReduceOp / ncclAllReduce for the decode step's
