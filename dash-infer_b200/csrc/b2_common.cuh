@@ -129,6 +129,7 @@ __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepc
 // ---- draft trees of speculative verification (tree format: include/b200spark.h, "Tree-structured verification").
 // par = parents[b][0 .. q_len-1]: node t >= 1 hangs below par[t] in [0, t); par[0] is ignored.  A parent outside [0, t) is
 // a caller error; it is read as the root, so every walk stays inside the row and ends within t steps.
+constexpr int kMaxQLen = 16;  // tokens per sequence of a multi-token step (draft-tree nodes: tree_walk's 16-bit ancestor mask)
 __device__ __forceinline__ int tree_parent(const int32_t* par, int t) {
   const int p = par[t];
   return (unsigned)p < (unsigned)t ? p : 0;

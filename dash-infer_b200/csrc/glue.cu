@@ -264,52 +264,34 @@ __global__ void lens_add_kernel(int32_t* lens, int batch, int delta) {
   if (i < batch) lens[i] += delta;
 }
 
-// greedy verification of a multi-token step: row t of sequence b predicted pred[b][t] after tokens[b][0..t]; the drafts
-// tokens[b][1..] are accepted while each equals the prediction before it
-__global__ void spec_accept_kernel(int32_t* accepted, int64_t* next_ids, int32_t* old_lens, int32_t* new_lens, int64_t* tokens,
-                                   const int64_t* pred, int batch, int q_len) {
+// greedy verification of a multi-token step: row t of sequence b predicted pred[b][t] after tokens[b][0..t] (a draft tree:
+// after t's path from the root).  From the root u = 0, step to the lowest-index child c of u with tokens[b][c] == pred[b][u]
+// while there is one.  Children have larger indices than their parent, so one pass over c finds the path.  A chain
+// (TREE = false) has the parent of c at c - 1, so its drafts tokens[b][1..] are accepted while each equals the prediction
+// before it, and it records no path.
+template <bool TREE>
+__global__ void spec_accept_kernel(int32_t* accepted, int32_t* path, int64_t* next_ids, int32_t* old_lens, int32_t* new_lens,
+                                   int64_t* tokens, const int64_t* pred, const int32_t* parents, int batch, int q_len) {
   pdl_wait();
   pdl_launch_dependents();
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= batch) return;
   const int64_t* tk = tokens + (size_t)b * q_len;
   const int64_t* pr = pred + (size_t)b * q_len;
-  int n = 1;
-  while (n < q_len && tk[n] == pr[n - 1]) ++n;
-  const int64_t next = pr[n - 1];
-  accepted[b] = n;
-  if (next_ids) next_ids[b] = next;
-  tokens[(size_t)b * q_len] = next;  // the last emitted token of the next step
-  const int ol = old_lens[b] + n;
-  old_lens[b] = ol;
-  new_lens[b] = ol + q_len;
-}
-
-// greedy verification of a draft tree: from the root u = 0, step to the lowest-index child c of u (tree_parent(c) == u) with
-// tokens[b][c] == pred[b][u] while there is one.  Children have larger indices than their parent, so one pass over c finds
-// the path; a chain gives spec_accept_kernel's result.
-__global__ void spec_accept_tree_kernel(int32_t* accepted, int32_t* path, int64_t* next_ids, int32_t* old_lens, int32_t* new_lens,
-                                        int64_t* tokens, const int64_t* pred, const int32_t* parents, int batch, int q_len) {
-  pdl_wait();
-  pdl_launch_dependents();
-  const int b = blockIdx.x * blockDim.x + threadIdx.x;
-  if (b >= batch) return;
-  const int64_t* tk = tokens + (size_t)b * q_len;
-  const int64_t* pr = pred + (size_t)b * q_len;
-  const int32_t* par = parents + (size_t)b * q_len;
-  int32_t* pa = path + (size_t)b * q_len;
   int n = 1, u = 0;
-  pa[0] = 0;
+  if (TREE) path[(size_t)b * q_len] = 0;
   for (int c = 1; c < q_len; ++c) {
-    if (tree_parent(par, c) == u && tk[c] == pr[u]) {
-      pa[n++] = c;
+    const int parent = TREE ? tree_parent(parents + (size_t)b * q_len, c) : c - 1;
+    if (parent == u && tk[c] == pr[u]) {
+      if (TREE) path[(size_t)b * q_len + n] = c;
+      ++n;
       u = c;
     }
   }
   const int64_t next = pr[u];
   accepted[b] = n;
   if (next_ids) next_ids[b] = next;
-  tokens[(size_t)b * q_len] = next;
+  tokens[(size_t)b * q_len] = next;  // the last emitted token of the next step
   const int ol = old_lens[b] + n;
   old_lens[b] = ol;
   new_lens[b] = ol + q_len;
@@ -342,6 +324,17 @@ using namespace b2;
       return B2_ERR_CUDA;                      \
     }                                          \
   } while (0)
+
+// path and parents: the tree form's
+static int spec_accept(int32_t* accepted, int32_t* path, int64_t* next_ids, int32_t* old_lens, int32_t* new_lens, int64_t* tokens,
+                       const int64_t* pred, const int32_t* parents, bool tree, int batch, int q_len, void* stream) {
+  if (!accepted || !old_lens || !new_lens || !tokens || !pred || (tree && (!path || !parents)) || batch <= 0) return B2_ERR_PARAM;
+  if (q_len < 1 || q_len > kMaxQLen) return B2_ERR_LIMIT;
+  B2_LAUNCH_CHECK(tree ? "spec_accept_tree" : "spec_accept",
+                  launch(tree ? spec_accept_kernel<true> : spec_accept_kernel<false>, dim3((batch + 127) / 128), dim3(128), 0,
+                         (cudaStream_t)stream, true, accepted, path, next_ids, old_lens, new_lens, tokens, pred, parents, batch, q_len));
+  return B2_OK;
+}
 
 extern "C" {
 
@@ -442,20 +435,12 @@ int b2_lens_add(int32_t* lens, int batch, int delta, void* stream) {
 
 int b2_spec_accept(int32_t* accepted, int64_t* next_ids, int32_t* old_lens, int32_t* new_lens, int64_t* tokens, const int64_t* pred,
                    int batch, int q_len, void* stream) {
-  if (!accepted || !old_lens || !new_lens || !tokens || !pred || batch <= 0) return B2_ERR_PARAM;
-  if (q_len < 1 || q_len > 16) return B2_ERR_LIMIT;
-  B2_LAUNCH_CHECK("spec_accept", launch(spec_accept_kernel, dim3((batch + 127) / 128), dim3(128), 0, (cudaStream_t)stream, true,
-                                        accepted, next_ids, old_lens, new_lens, tokens, pred, batch, q_len));
-  return B2_OK;
+  return spec_accept(accepted, nullptr, next_ids, old_lens, new_lens, tokens, pred, nullptr, false, batch, q_len, stream);
 }
 
 int b2_spec_accept_tree(int32_t* accepted, int32_t* path, int64_t* next_ids, int32_t* old_lens, int32_t* new_lens, int64_t* tokens,
                         const int64_t* pred, const int32_t* parents, int batch, int q_len, void* stream) {
-  if (!accepted || !path || !old_lens || !new_lens || !tokens || !pred || !parents || batch <= 0) return B2_ERR_PARAM;
-  if (q_len < 1 || q_len > 16) return B2_ERR_LIMIT;
-  B2_LAUNCH_CHECK("spec_accept_tree", launch(spec_accept_tree_kernel, dim3((batch + 127) / 128), dim3(128), 0, (cudaStream_t)stream,
-                                             true, accepted, path, next_ids, old_lens, new_lens, tokens, pred, parents, batch, q_len));
-  return B2_OK;
+  return spec_accept(accepted, path, next_ids, old_lens, new_lens, tokens, pred, parents, true, batch, q_len, stream);
 }
 
 }  // extern "C"

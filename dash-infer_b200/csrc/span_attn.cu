@@ -13,7 +13,8 @@
 //   * split-KV partials (fp32, unnormalised) go to the caller's workspace; the last CTA of a
 //     (sequence, kv-head) — device counter, self-resetting — merges them in fixed order.
 //
-// The span format and its shared-memory tile are described once, by KVTraits below.
+// The span format and its shared-memory tile are described once, by KVTraits below; how the 16 MMA rows of a piece map to
+// sequences, tokens, heads and visible tokens (single-token, chain and tree steps) once, by QueryRows.
 // Roofline: HBM-bound; algorithmic bytes = sum_b len_b * 2 * n_groups * KVTraits<QM>::SPAN_ROW.
 #include <new>
 
@@ -25,7 +26,6 @@ constexpr int kAttnThreads = 128;  // 4 warps, 16 tokens of each 64-token tile p
 constexpr int kTile = 64;
 constexpr int kHead = 128;
 constexpr int kMaxBatch = 1024;
-constexpr int kMaxQLen = 16;  // tokens per sequence of a multi-token step (draft-tree nodes: a 16-bit ancestor mask)
 constexpr int kMergeRS = 136;  // padded fp32 row stride of the merge buffer (conflict-free float2 stores)
 constexpr int kMergeDirect = 16;  // up to this many pieces per (sequence, kv-head): the last CTA merges them all
 constexpr int kMergeFan = 8;      // above: groups of 8 pieces are merged by their last CTA, the last group merges the groups
@@ -204,18 +204,101 @@ __device__ __forceinline__ void softmax_sum(float (&psum)[2], float (&lrow)[2], 
   }
 }
 
-// Tree form: is token tok visible to the thread's row rr (0: gq, 1: gq+8)?  lim[rr] is the prefix end; past it, the token's
-// draft slot tok - lim[rr] must be in the row's ancestor mask am[rr] (tok < tok1 <= the block's length keeps it below 16).
-__device__ __forceinline__ bool tree_visible(int tok, int tok1, const int (&lim)[2], const unsigned (&am)[2], int rr) {
-  return tok < lim[rr] || (tok < tok1 && ((am[rr] >> (tok - lim[rr])) & 1u));
-}
+// ---- the query rows of a piece: the one place that knows how the 16 MMA rows of a work item map to sequences, tokens and
+// heads, and which cached tokens each row may see.  Three step forms (span_attn_kernel<QM, H, MT, TREE>):
+//   single token   item = sequence b; row r = head r of kv-group g; every row sees the item's len = lens[b] tokens.
+//   chain (MT)     item = (sequence b, row block rb): tokens qt0 = rb*tpb .. qt0+ntok-1 of the step's q_len, row r = token
+//                  qt0 + r / hpg, head r % hpg.  Token t sees the first lens[b] - q_len + t + 1 tokens, so the item streams the
+//                  len tiles its last token sees and each row is masked at its own limit.
+//   tree (TREE)    the chain's rows; row r sees the prefix (tokens < lens[b] - q_len) and the draft slots of node qt0 + r / hpg
+//                  and its ancestors (AttnTreeParams).  Ancestors have smaller indices: the same tiles as the chain.
+// The scheduler treats every item alike: counters and partials are per (item, kv-head), a partial slot holds rstride rows.
+
+// What the calling thread's rows gq (rr = 0) and gq + 8 (rr = 1) may see.  tok1, the end of the piece, bounds every row.
+template <bool MT, bool TREE>
+struct RowMask {
+  int tok1;
+  int lim[2] = {0, 0};        // chain: the row's own end (<= tok1).  Tree: the prefix end.  A dead row: the item's len
+  unsigned am[2] = {0u, 0u};  // tree: tree_walk's ancestor mask of the row's node (a dead row: 0)
+  __device__ __forceinline__ bool visible(int tok, int rr) const {
+    // tree: past the prefix, the token's draft slot tok - lim must be an ancestor's (tok < tok1 keeps the shift below 16)
+    if constexpr (TREE) return tok < lim[rr] || (tok < tok1 && ((am[rr] >> (tok - lim[rr])) & 1u));
+    else if constexpr (MT) return tok < lim[rr];
+    else return tok < tok1;
+  }
+};
+
+template <bool MT, bool TREE>
+struct QueryRows;
+
+// Single token.  (A specialisation of its own, not `MT ? :` expressions: these kernels are the decode hot path and must see
+// no multi-token arithmetic.)
+template <>
+struct QueryRows<false, false> {
+  __device__ __forceinline__ static int n_items(const AttnParams& p) { return p.batch; }
+  __device__ __forceinline__ static int seq(const AttnParams&, int item) { return item; }
+  __device__ __forceinline__ static int item_len(const AttnParams& p, int item) { return p.lens[item]; }  // tokens attended to
+
+  int nrows, rstride;  // live MMA rows; rows of a partial slot
+  size_t row0;
+  RowMask<false, false> mask;
+
+  // the piece of `item` (sequence b, len tokens) for kv-head g that ends at token tok1; gq = lane / 4
+  __device__ __forceinline__ QueryRows(const AttnParams& p, int item, int b, int g, int len, int tok1, int gq) {
+    row0 = ((size_t)b * p.n_heads + (size_t)g * p.hpg) * kHead;
+    nrows = rstride = p.hpg;
+    mask.tok1 = tok1;
+  }
+  // MMA row r in q or in out (same layout)
+  template <class E>
+  __device__ __forceinline__ E* at(E* base, int r) const { return base + row0 + r * kHead; }
+};
+
+// Chain and tree: the same members for a row block.
+template <bool TREE>
+struct QueryRows<true, TREE> {
+  using Params = AttnArgs<true, TREE>;
+  __device__ __forceinline__ static int n_items(const Params& p) { return p.batch * p.nrb; }
+  __device__ __forceinline__ static int seq(const Params& p, int item) { return item / p.nrb; }
+  __device__ __forceinline__ static int item_len(const Params& p, int item) {
+    const int b = item / p.nrb, rb = item - b * p.nrb;
+    return p.lens[b] - p.q_len + min(p.q_len, (rb + 1) * p.tpb);
+  }
+
+  const Params& p;
+  int b, g, qt0;
+  int nrows, rstride;
+  RowMask<true, TREE> mask;
+
+  __device__ __forceinline__ QueryRows(const Params& p_, int item, int b_, int g_, int len, int tok1, int gq) : p(p_), b(b_), g(g_) {
+    qt0 = (item - b * p.nrb) * p.tpb;
+    const int ntok = min(p.tpb, p.q_len - qt0);
+    nrows = ntok * p.hpg;
+    rstride = p.rstride;
+    mask.tok1 = tok1;
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr) {
+      const int r = gq + 8 * rr;
+      if constexpr (TREE) {
+        int depth;
+        mask.am[rr] = r < nrows ? tree_walk(p.parents + (size_t)b * p.q_len, qt0 + r / p.hpg, depth) : 0u;
+        mask.lim[rr] = r < nrows ? len - ntok - qt0 : len;
+      } else {
+        mask.lim[rr] = r < nrows ? len - ntok + 1 + r / p.hpg : len;
+      }
+    }
+  }
+  template <class E>
+  __device__ __forceinline__ E* at(E* base, int r) const {
+    return base + ((size_t)b * p.q_len + qt0 + r / p.hpg) * p.n_heads * kHead + ((size_t)g * p.hpg + r % p.hpg) * kHead;
+  }
+};
 
 // One 64-token tile of attention math for this warp's 16-token slice (cache in the 16-bit type FT: bf16, or fp16 when H).
-// Tokens >= tok1 are masked; multi-token (MT): rows gq and gq+8 are masked at their own limits lim[0] and lim[1] (<= tok1);
-// tree (TREE): at their prefix ends lim[] and ancestor masks am[] (tree_visible above).
-template <bool H, bool MT, bool TREE = false>
-__device__ __forceinline__ void tile_compute_bf16(const uint8_t* st, int warp, int lane, int wtok, int tok1, const int (&lim)[2],
-                                                  const unsigned (&am)[2], float scale_log2, const uint32_t (&qa)[8][4],
+// mask says which tokens the thread's rows gq and gq+8 see.
+template <bool H, bool MT, bool TREE>
+__device__ __forceinline__ void tile_compute_bf16(const uint8_t* st, int warp, int lane, int wtok, const RowMask<MT, TREE>& mask,
+                                                  float scale_log2, const uint32_t (&qa)[8][4],
                                                   float (&o)[16][4], float (&mrow)[2], float (&lrow)[2]) {
   using T = KVTraits<B2_KV_NONE>;
   const int t = lane & 3;
@@ -243,9 +326,7 @@ __device__ __forceinline__ void tile_compute_bf16(const uint8_t* st, int warp, i
 #pragma unroll
     for (int cc = 0; cc < 4; ++cc) {
       const int tok = wtok + nt * 8 + 2 * t + (cc & 1);
-      float v;
-      if constexpr (TREE) v = tree_visible(tok, tok1, lim, am, cc >> 1) ? sc[nt][cc] * scale_log2 : -INFINITY;
-      else v = tok < (MT ? lim[cc >> 1] : tok1) ? sc[nt][cc] * scale_log2 : -INFINITY;
+      const float v = mask.visible(tok, cc >> 1) ? sc[nt][cc] * scale_log2 : -INFINITY;
       sc[nt][cc] = v;
       mx[cc >> 1] = fmaxf(mx[cc >> 1], v);
     }
@@ -302,9 +383,9 @@ __device__ __forceinline__ uint32_t e4m3x2_to_f16x2(uint32_t w) {
   return d;
 }
 
-template <int QM, bool MT, bool TREE = false>
-__device__ __forceinline__ void tile_compute_q(const uint8_t* st, int warp, int lane, int wtok, int tok1, const int (&lim)[2],
-                                               const unsigned (&am)[2], float scale_log2, const uint32_t (&qa)[8][4], const float (&sq)[2],
+template <int QM, bool MT, bool TREE>
+__device__ __forceinline__ void tile_compute_q(const uint8_t* st, int warp, int lane, int wtok, const RowMask<MT, TREE>& mask,
+                                               float scale_log2, const uint32_t (&qa)[8][4], const float (&sq)[2],
                                                float (&o)[16][4], float (&mrow)[2], float (&lrow)[2], float (&cacc)[2]) {
   using T = KVTraits<QM>;
   constexpr float BIAS = QM == B2_KV_I8 ? 1152.f : 1024.f;
@@ -359,7 +440,7 @@ __device__ __forceinline__ void tile_compute_q(const uint8_t* st, int warp, int 
     // tokens at or beyond tok1 carry whatever the span memory held (the reference's span manager never zeroes frames,
     // and the 16-byte param chunk of an odd-length tail covers one unwritten token): their V params must not reach
     // the arithmetic (0 * NaN), so they are forced to zero exactly like the scores are forced to -inf
-    const bool live0 = wtok + nt * 8 + 2 * t < tok1, live1 = wtok + nt * 8 + 2 * t + 1 < tok1;
+    const bool live0 = wtok + nt * 8 + 2 * t < mask.tok1, live1 = wtok + nt * 8 + 2 * t + 1 < mask.tok1;
     vz[nt][0] = live0 ? vp.x : 0.f; vs[nt][0] = live0 ? vp.y : 0.f;
     vz[nt][1] = live1 ? vp.z : 0.f; vs[nt][1] = live1 ? vp.w : 0.f;
 #pragma unroll
@@ -367,9 +448,7 @@ __device__ __forceinline__ void tile_compute_q(const uint8_t* st, int warp, int 
       const int tok = wtok + nt * 8 + 2 * t + (cc & 1);
       const float kz = (cc & 1) ? kp.z : kp.x, ksc = (cc & 1) ? kp.w : kp.y;
       const float raw = T::kZeroPoint ? ksc * (sc[nt][cc] - (BIAS + kz) * sq[cc >> 1]) : ksc * sc[nt][cc];
-      float v;
-      if constexpr (TREE) v = tree_visible(tok, tok1, lim, am, cc >> 1) ? raw * scale_log2 : -INFINITY;
-      else v = tok < (MT ? lim[cc >> 1] : tok1) ? raw * scale_log2 : -INFINITY;
+      const float v = mask.visible(tok, cc >> 1) ? raw * scale_log2 : -INFINITY;
       sc[nt][cc] = v;
       mx[cc >> 1] = fmaxf(mx[cc >> 1], v);
     }
@@ -436,17 +515,15 @@ __device__ __forceinline__ void tile_compute_q(const uint8_t* st, int warp, int 
 // merge of up to 8 sources (every level-1 group, most final merges) is ONE round trip; longer lists take one more per 8.
 // FINAL writes softmax-normalised bf16 rows of `out`; otherwise the merged, still unnormalised partial goes to slot
 // `dst_slot` of (dst_o, dst_ml).  s_w: shared scratch [kMergeMaxSrc][16] floats (weights), s_ML: [16][2].
-// A slot holds `hpg` rows.  Multi-token (MT): a slot holds `hpg` = rstride rows of which the first `rows` are live, and
-// row r of the output is head r % qh of token r / qh, tokens tok_stride elements apart.
+// A slot holds rows.rstride rows of which the first rows.nrows are live; FINAL puts row r at out + rows.row(r).
 constexpr int kMergeMaxSrc = 96;  // sources of one merge call (final level: ceil(pieces / kMergeFan)); more -> looped M pass
-template <bool FINAL, bool H, bool MT = false>
+template <bool FINAL, bool H, class Rows>
 __device__ __forceinline__ void merge_partials(const float* src_o, const float* src_ml, int slot0, int stride2, int par0, int n,
-                                               int hpg, __nv_bfloat16* out_rows, float* dst_o, float* dst_ml, int dst_slot,
-                                               float* s_w, float* s_ML, int rows = 0, int qh = 0, int tok_stride = 0) {
+                                               const Rows& rows, __nv_bfloat16* out, float* dst_o, float* dst_ml, int dst_slot,
+                                               float* s_w, float* s_ML) {
   const int tid = threadIdx.x;
   auto slot_of = [&](int i) { return slot0 + i * stride2 + (i == 0 ? par0 : 0); };
-  int R = hpg;  // rows merged
-  if constexpr (MT) R = rows;
+  const int R = rows.nrows, hpg = rows.rstride;  // rows merged, rows of a slot
   const int nunits = R * 32;  // (row, float4) units
   // ---- request the first batch of rows and every (m, l) pair before waiting for anything
   float4 v[2][8];
@@ -533,12 +610,8 @@ __device__ __forceinline__ void merge_partials(const float* src_o, const float* 
       const int r = u >> 5, c4 = u & 31;
       if (FINAL) {
         const float inv = 1.f / s_ML[r * 2 + 1];
-        if constexpr (MT)
-          *reinterpret_cast<uint2*>(out_rows + (size_t)(r / qh) * tok_stride + (size_t)(r % qh) * kHead + c4 * 4) =
-              make_uint2(Ft<H>::pack(acc[uu].x * inv, acc[uu].y * inv), Ft<H>::pack(acc[uu].z * inv, acc[uu].w * inv));
-        else
-          *reinterpret_cast<uint2*>(out_rows + (size_t)r * kHead + c4 * 4) =
-              make_uint2(Ft<H>::pack(acc[uu].x * inv, acc[uu].y * inv), Ft<H>::pack(acc[uu].z * inv, acc[uu].w * inv));
+        *reinterpret_cast<uint2*>(rows.at(out, r) + c4 * 4) =
+            make_uint2(Ft<H>::pack(acc[uu].x * inv, acc[uu].y * inv), Ft<H>::pack(acc[uu].z * inv, acc[uu].w * inv));
       } else {
         const size_t row = (size_t)dst_slot * hpg + r;
         *(reinterpret_cast<float4*>(dst_o + row * kHead) + c4) = acc[uu];
@@ -557,27 +630,11 @@ B2_TRACE_DECL(g_attn_tr)
 extern "C" int b2_debug_trace_attn(unsigned long long* host_out) { return (int)cudaMemcpyFromSymbol(host_out, g_attn_tr, sizeof(g_attn_tr)); }
 #endif
 
-// Multi-token form (MT): the work items are (sequence, row block, kv-head, tile).  Row block rb of sequence b holds
-// tokens rb*tpb .. min(q_len, (rb+1)*tpb) - 1; token t attends to the first lens[b] - q_len + t + 1 tokens, so the block
-// streams the tiles its last token sees and masks each row at its own limit.  The scheduler below treats each
-// (sequence, row block) as one item of length block_len: counters and partials are per (item, kv-head).
-// (Overloads rather than `MT ? :` expressions: the single-token kernels then compile to the code they had before.)
-__device__ __forceinline__ int n_items(const AttnParams& p) { return p.batch; }
-__device__ __forceinline__ int n_items(const AttnTokParams& p) { return p.batch * p.nrb; }
-__device__ __forceinline__ int item_len(const AttnParams& p, int b) { return p.lens[b]; }
-__device__ __forceinline__ int item_len(const AttnTokParams& p, int v) {
-  const int b = v / p.nrb, rb = v - b * p.nrb;
-  return p.lens[b] - p.q_len + min(p.q_len, (rb + 1) * p.tpb);
-}
-// offset of MMA row r of the row block starting at token qt0 of sequence b, kv-head g, in q and out
-__device__ __forceinline__ size_t tok_row(const AttnTokParams& p, int b, int qt0, int g, int r) {
-  return ((size_t)b * p.q_len + qt0 + r / p.hpg) * p.n_heads * kHead + ((size_t)g * p.hpg + r % p.hpg) * kHead;
-}
-
 template <int QM, bool H, bool MT = false, bool TREE = false>
 __global__ void __launch_bounds__(kAttnThreads) span_attn_kernel(const AttnArgs<MT, TREE> p) {
   using F = Ft<H>;  // the 16-bit type of Q, the output and an unquantized cache
   using T = KVTraits<QM>;
+  using Rows = QueryRows<MT, TREE>;
   extern __shared__ __align__(128) uint8_t smem[];
   __shared__ int s_prefix[kMaxBatch + 1];  // flat tile index of each sequence's first tile (x n_groups)
   __shared__ int s_red[8];
@@ -593,11 +650,11 @@ __global__ void __launch_bounds__(kAttnThreads) span_attn_kernel(const AttnArgs<
   if (tr0) B2_TR(g_attn_tr, 1);
 
   // ---------------- device-side work decomposition (ONE global round trip: the lengths) ----------------
-  // items: sequences, or (sequence, row block)s
+  // items: sequences, or (sequence, row block)s (QueryRows)
   {
     int my_tiles = 0, my_max = 0;
-    for (int b = tid; b < n_items(p); b += kAttnThreads) {
-      const int tl = (item_len(p, b) + kTile - 1) / kTile;
+    for (int b = tid; b < Rows::n_items(p); b += kAttnThreads) {
+      const int tl = (Rows::item_len(p, b) + kTile - 1) / kTile;
       s_prefix[b] = tl;  // tile count for now; warp 0 turns it into the exclusive scan below
       my_tiles += tl;
       my_max = max(my_max, tl);
@@ -619,18 +676,18 @@ __global__ void __launch_bounds__(kAttnThreads) span_attn_kernel(const AttnArgs<
   if (lo >= hi) return;
   if (warp == 0) {  // exclusive scan of tiles*n_groups per sequence
     int carry = 0;
-    for (int b0 = 0; b0 < n_items(p); b0 += 32) {
+    for (int b0 = 0; b0 < Rows::n_items(p); b0 += 32) {
       const int b = b0 + lane;
-      int v = b < n_items(p) ? s_prefix[b] * p.n_groups : 0, x = v;
+      int v = b < Rows::n_items(p) ? s_prefix[b] * p.n_groups : 0, x = v;
 #pragma unroll
       for (int o = 1; o < 32; o <<= 1) {
         const int y = __shfl_up_sync(0xffffffffu, x, o);
         if (lane >= o) x += y;
       }
-      if (b < n_items(p)) s_prefix[b] = carry + x - v;
+      if (b < Rows::n_items(p)) s_prefix[b] = carry + x - v;
       carry += __shfl_sync(0xffffffffu, x, 31);
     }
-    if (lane == 0) s_prefix[n_items(p)] = carry;
+    if (lane == 0) s_prefix[Rows::n_items(p)] = carry;
   }
   __syncthreads();
 
@@ -645,15 +702,13 @@ __global__ void __launch_bounds__(kAttnThreads) span_attn_kernel(const AttnArgs<
   int pos = lo;
   while (pos < hi) {
     // ---- locate (b, g, first tile) of the piece starting at flat index pos
-    int blo = 0, bhi = n_items(p) - 1;
+    int blo = 0, bhi = Rows::n_items(p) - 1;
     while (blo < bhi) {
       const int mid = (blo + bhi + 1) >> 1;
       if (s_prefix[mid] <= pos) blo = mid; else bhi = mid - 1;
     }
     const int item = blo;
-    int b, len;  // the sequence, the tokens the item attends to
-    if constexpr (MT) { b = item / p.nrb; len = item_len(p, item); }
-    else { b = blo; len = p.lens[b]; }
+    const int b = Rows::seq(p, item), len = Rows::item_len(p, item);  // the sequence, the tokens the item attends to
     const int tiles_b = (len + kTile - 1) / kTile;
     const int within = pos - s_prefix[item];
     const int g = within / tiles_b, t0 = within - g * tiles_b;
@@ -666,12 +721,6 @@ __global__ void __launch_bounds__(kAttnThreads) span_attn_kernel(const AttnArgs<
     const int npieces = (bg_end - 1) / Tc - k0 + 1;
     const void* const* ktab = p.k_spans + (size_t)b * p.max_spans;
     const void* const* vtab = p.v_spans + (size_t)b * p.max_spans;
-    // multi-token: this row block's tokens qt0 .. qt0+ntok-1 sit in MMA rows 0 .. nrows-1 (row r: token qt0 + r / hpg,
-    // head r % hpg).  Row r sees the tokens before len - ntok + 1 + r / hpg (lim[] for the thread's rows gq and gq+8).
-    // Tree: lim[] is the prefix end len - ntok - qt0 and am[] the row's ancestor mask (a dead row: lim = len, am = 0).
-    int nrows, rstride, qt0;  // live rows, rows of a partial slot (set below, next to the single-token kernel's first use of hpg)
-    int lim[2];
-    unsigned am[2];
 
     // ---- start streaming: the piece's first nstage-1 tiles are requested NOW (span-table lookups + cp.async), so their
     //      HBM latency overlaps the load of the query rows below
@@ -683,6 +732,7 @@ __global__ void __launch_bounds__(kAttnThreads) span_attn_kernel(const AttnArgs<
     // ---- Q fragments (A operand, rows = q-heads of this kv-group).  The head-dim order each thread uses is free as
     //      long as Q and K agree, so it follows how that thread reads K: natural for bf16 (ldmatrix), per-thread
     //      contiguous 32-d slices for the quantized modes.  Quantized modes run the MMAs in fp16.
+    const Rows rows(p, item, b, g, len, tok1, gq);  // after the prefetch: a tree's ancestor walk reads global memory
     uint32_t qa[8][4];
     float sq[2] = {0.f, 0.f};  // sum_d Q[row][d] over this thread's d-slice, then over the quad (quantized modes)
     {
@@ -690,55 +740,24 @@ __global__ void __launch_bounds__(kAttnThreads) span_attn_kernel(const AttnArgs<
       // trip; their fragment orders would otherwise need 64 scalar loads per thread: 3.3 us measured at ctx 32768)
       // [16][128] in the LAST ring stage: the only one the prefetch above does not write (it is first filled at iteration 0)
       __nv_bfloat16* qs = reinterpret_cast<__nv_bfloat16*>(smem + (p.nstage - 1) * T::STAGE);
-      const __nv_bfloat16* qb = p.q + ((size_t)b * p.n_heads + (size_t)g * p.hpg) * kHead;
-      if constexpr (MT) {
-        qt0 = (item - b * p.nrb) * p.tpb;
-        const int ntok = min(p.tpb, p.q_len - qt0);
-        nrows = ntok * p.hpg;
-        rstride = p.rstride;
-#pragma unroll
-        for (int rr = 0; rr < 2; ++rr) {
-          const int r = gq + 8 * rr;
-          if constexpr (TREE) {
-            int depth;
-            am[rr] = r < nrows ? tree_walk(p.parents + (size_t)b * p.q_len, qt0 + r / p.hpg, depth) : 0u;
-            lim[rr] = r < nrows ? len - ntok - qt0 : len;
-          } else {
-            lim[rr] = r < nrows ? len - ntok + 1 + r / p.hpg : len;
-          }
-        }
-      } else {
-        nrows = rstride = p.hpg;
-      }
       if (QM != B2_KV_NONE) {
         for (int i = tid; i < 16 * (kHead / 8); i += kAttnThreads) {
           const int row = i >> 4;
-          if constexpr (MT)
-            *reinterpret_cast<uint4*>(qs + row * kHead + (i & 15) * 8) =
-                row < nrows ? *reinterpret_cast<const uint4*>(p.q + tok_row(p, b, qt0, g, row) + (i & 15) * 8) : make_uint4(0, 0, 0, 0);
-          else
-            *reinterpret_cast<uint4*>(qs + row * kHead + (i & 15) * 8) =
-                row < p.hpg ? *reinterpret_cast<const uint4*>(qb + row * kHead + (i & 15) * 8) : make_uint4(0, 0, 0, 0);
+          *reinterpret_cast<uint4*>(qs + row * kHead + (i & 15) * 8) =
+              row < rows.nrows ? *reinterpret_cast<const uint4*>(rows.at(p.q, row) + (i & 15) * 8) : make_uint4(0, 0, 0, 0);
         }
         __syncthreads();
       }
-      const bool r0 = gq < nrows, r1 = (gq + 8) < nrows;
+      const bool r0 = gq < rows.nrows, r1 = (gq + 8) < rows.nrows;
 #pragma unroll
       for (int ks = 0; ks < 8; ++ks) {
         if (QM == B2_KV_NONE) {  // natural d order: 32 independent 4-byte loads per thread straight from global memory
           const int d0 = 16 * ks + 2 * t;
-          if constexpr (MT) {
-            const __nv_bfloat16 *q0 = p.q + tok_row(p, b, qt0, g, gq), *q1 = p.q + tok_row(p, b, qt0, g, gq + 8);
-            qa[ks][0] = r0 ? *reinterpret_cast<const uint32_t*>(q0 + d0) : 0u;
-            qa[ks][1] = r1 ? *reinterpret_cast<const uint32_t*>(q1 + d0) : 0u;
-            qa[ks][2] = r0 ? *reinterpret_cast<const uint32_t*>(q0 + d0 + 8) : 0u;
-            qa[ks][3] = r1 ? *reinterpret_cast<const uint32_t*>(q1 + d0 + 8) : 0u;
-          } else {
-            qa[ks][0] = r0 ? *reinterpret_cast<const uint32_t*>(qb + gq * kHead + d0) : 0u;
-            qa[ks][1] = r1 ? *reinterpret_cast<const uint32_t*>(qb + (gq + 8) * kHead + d0) : 0u;
-            qa[ks][2] = r0 ? *reinterpret_cast<const uint32_t*>(qb + gq * kHead + d0 + 8) : 0u;
-            qa[ks][3] = r1 ? *reinterpret_cast<const uint32_t*>(qb + (gq + 8) * kHead + d0 + 8) : 0u;
-          }
+          const __nv_bfloat16 *q0 = rows.at(p.q, gq), *q1 = rows.at(p.q, gq + 8);
+          qa[ks][0] = r0 ? *reinterpret_cast<const uint32_t*>(q0 + d0) : 0u;
+          qa[ks][1] = r1 ? *reinterpret_cast<const uint32_t*>(q1 + d0) : 0u;
+          qa[ks][2] = r0 ? *reinterpret_cast<const uint32_t*>(q0 + d0 + 8) : 0u;
+          qa[ks][3] = r1 ? *reinterpret_cast<const uint32_t*>(q1 + d0 + 8) : 0u;
         } else {
           float f[2][4];
 #pragma unroll
@@ -785,8 +804,8 @@ __global__ void __launch_bounds__(kAttnThreads) span_attn_kernel(const AttnArgs<
       const int wtok = tok0 + i * kTile + warp * 16;  // first token of this warp's slice
       if (wtok < tok1) {
         if constexpr (!T::kCodesF16)
-          tile_compute_bf16<H, MT, TREE>(smem + slot * T::STAGE, warp, lane, wtok, tok1, lim, am, p.scale_log2, qa, o, mrow, lrow);
-        else tile_compute_q<QM, MT, TREE>(smem + slot * T::STAGE, warp, lane, wtok, tok1, lim, am, p.scale_log2, qa, sq, o, mrow, lrow, cacc);
+          tile_compute_bf16<H>(smem + slot * T::STAGE, warp, lane, wtok, rows.mask, p.scale_log2, qa, o, mrow, lrow);
+        else tile_compute_q<QM>(smem + slot * T::STAGE, warp, lane, wtok, rows.mask, p.scale_log2, qa, sq, o, mrow, lrow, cacc);
       }
       __syncthreads();  // this stage may be refilled by the next iteration's prefetch
       slot = slot + 1 == p.nstage ? 0 : slot + 1;
@@ -846,7 +865,7 @@ __global__ void __launch_bounds__(kAttnThreads) span_attn_kernel(const AttnArgs<
     // thread d = tid handles column d of every head row
     const int cnt_idx = item * p.n_groups + g;
     const int my_slot = 2 * blockIdx.x + (pos != lo ? 1 : 0);
-    for (int r = 0; r < nrows; ++r) {
+    for (int r = 0; r < rows.nrows; ++r) {
       float M = -INFINITY;
 #pragma unroll
       for (int w = 0; w < 4; ++w) M = fmaxf(M, mrg_ml[(w * 16 + r) * 2]);
@@ -859,13 +878,12 @@ __global__ void __launch_bounds__(kAttnThreads) span_attn_kernel(const AttnArgs<
         acc += f * mrg[(w * 16 + r) * kMergeRS + tid];
       }
       if (npieces == 1) {
-        if constexpr (MT) p.out[tok_row(p, b, qt0, g, r) + tid] = F::from_f(acc / L);
-        else p.out[((size_t)b * p.n_heads + (size_t)g * p.hpg + r) * kHead + tid] = F::from_f(acc / L);
+        rows.at(p.out, r)[tid] = F::from_f(acc / L);
       } else {
-        p.ws_o[((size_t)my_slot * rstride + r) * kHead + tid] = acc;
+        p.ws_o[((size_t)my_slot * rows.rstride + r) * kHead + tid] = acc;
         if (tid == 0) {
-          p.ws_ml[((size_t)my_slot * rstride + r) * 2] = M;
-          p.ws_ml[((size_t)my_slot * rstride + r) * 2 + 1] = L;
+          p.ws_ml[((size_t)my_slot * rows.rstride + r) * 2] = M;
+          p.ws_ml[((size_t)my_slot * rows.rstride + r) * 2 + 1] = L;
         }
       }
     }
@@ -877,17 +895,13 @@ __global__ void __launch_bounds__(kAttnThreads) span_attn_kernel(const AttnArgs<
       // pieces of this (sequence, kv-head) come from CTAs k0 .. k0+npieces-1 (one each); only CTA k0's piece can start
       // inside its range (slot parity 1)
       const int first_par = bg_start > k0 * Tc ? 1 : 0;
-      __nv_bfloat16* out_rows;
-      if constexpr (MT) out_rows = p.out + tok_row(p, b, qt0, g, 0);
-      else out_rows = p.out + ((size_t)b * p.n_heads + (size_t)g * p.hpg) * kHead;
       if (npieces <= kMergeDirect) {
         if (tid == 0) s_is_last = atomicAdd(&p.counters[cnt_idx], 1u) == (unsigned)(npieces - 1);
         __syncthreads();
         if (s_is_last) {
           __threadfence();
           if (tid == 0 && cnt_idx == 0) B2_TR(g_attn_tr, 10);
-          merge_partials<true, H, MT>(p.ws_o, p.ws_ml, 2 * k0, 2, first_par, npieces, rstride, out_rows, nullptr, nullptr, 0, s_w, s_ML,
-                                      nrows, p.hpg, p.n_heads * kHead);
+          merge_partials<true, H>(p.ws_o, p.ws_ml, 2 * k0, 2, first_par, npieces, rows, p.out, nullptr, nullptr, 0, s_w, s_ML);
           if (tid == 0) p.counters[cnt_idx] = 0;  // re-arm
           if (tid == 0 && cnt_idx == 0) B2_TR(g_attn_tr, 11);
         }
@@ -905,8 +919,8 @@ __global__ void __launch_bounds__(kAttnThreads) span_attn_kernel(const AttnArgs<
         if (s_is_last) {
           __threadfence();
           if (tid == 0 && cnt_idx == 0 && q == 0) B2_TR(g_attn_tr, 8);
-          merge_partials<false, H, MT>(p.ws_o, p.ws_ml, 2 * (k0 + q * kMergeFan), 2, q == 0 ? first_par : 0, gsize, rstride, nullptr,
-                                       p.ws2_o, p.ws2_ml, lead, s_w, s_ML, nrows, p.hpg, p.n_heads * kHead);
+          merge_partials<false, H>(p.ws_o, p.ws_ml, 2 * (k0 + q * kMergeFan), 2, q == 0 ? first_par : 0, gsize, rows, nullptr,
+                                   p.ws2_o, p.ws2_ml, lead, s_w, s_ML);
           if (tid == 0 && cnt_idx == 0 && q == 0) B2_TR(g_attn_tr, 9);
           if (tid == 0) p.counters1[lead] = 0;
           __threadfence();
@@ -916,8 +930,8 @@ __global__ void __launch_bounds__(kAttnThreads) span_attn_kernel(const AttnArgs<
           if (s_is_last) {
             __threadfence();
             if (tid == 0 && cnt_idx == 0) B2_TR(g_attn_tr, 10);
-            merge_partials<true, H, MT>(p.ws2_o, p.ws2_ml, 2 * k0, 2 * kMergeFan, first_par, ngroups, rstride, out_rows, nullptr, nullptr, 0,
-                                        s_w, s_ML, nrows, p.hpg, p.n_heads * kHead);
+            merge_partials<true, H>(p.ws2_o, p.ws2_ml, 2 * k0, 2 * kMergeFan, first_par, ngroups, rows, p.out, nullptr, nullptr, 0,
+                                    s_w, s_ML);
             if (tid == 0) p.counters[cnt_idx] = 0;
             if (tid == 0 && cnt_idx == 0) B2_TR(g_attn_tr, 11);
           }
@@ -1055,19 +1069,26 @@ struct AppendParams {
   int rope;        // 0/1
   int rotary_dim;
   float log2_base;
-  int q_len;       // multi-token form: rows per sequence
+  int q_len;       // multi-token forms: rows per sequence
+  const int32_t* parents;  // tree form: the draft tree of each sequence (format: AttnTreeParams)
 };
 
-// tree form: the draft tree of each sequence (format: AttnTreeParams)
-struct AppendTreeParams : AppendParams {
-  const int32_t* parents;
-};
+// Where row `row` of qkv / q_out goes: its sequence b, the slot it is written to and its rotary position.
+// MT = false: row b is sequence b, at position old_lens[b].  MT = true: row b*q_len + t is token t of sequence b, at position
+// old_lens[b] + t.  TREE (with MT): at slot old_lens[b] + t, rotary position old_lens[b] + depth(t).
+template <bool MT, bool TREE>
+__device__ __forceinline__ void append_row(const AppendParams& p, int row, int& b, int& slot, int& pos) {
+  b = MT ? row / p.q_len : row;
+  slot = pos = MT ? p.old_lens[b] + (row - b * p.q_len) : p.old_lens[b];
+  if constexpr (TREE) {
+    int depth;
+    tree_walk(p.parents + (size_t)b * p.q_len, row - b * p.q_len, depth);
+    pos = p.old_lens[b] + depth;
+  }
+}
 
-// MT = false: row b of qkv / q_out is sequence b, written at position old_lens[b].  MT = true: row b*q_len + t is token t of
-// sequence b, written at position old_lens[b] + t.  TREE (with MT): written at slot old_lens[b] + t, rotary position
-// old_lens[b] + depth(t).
 template <int QM, bool H, bool MT = false, bool TREE = false>
-__global__ void __launch_bounds__(128) cache_append_kernel(const std::conditional_t<TREE, AppendTreeParams, AppendParams> p) {
+__global__ void __launch_bounds__(128) cache_append_kernel(const AppendParams p) {
   using F = Ft<H>;
   pdl_wait();
   pdl_launch_dependents();
@@ -1076,17 +1097,11 @@ __global__ void __launch_bounds__(128) cache_append_kernel(const std::conditiona
   const int wid = blockIdx.x * 4 + (threadIdx.x >> 5);
   if (wid >= (MT ? p.batch * p.q_len : p.batch) * slots) return;
   const int row = wid / slots, slot = wid - row * slots;
-  const int b = MT ? row / p.q_len : row;
   const __nv_bfloat16* src = p.qkv + ((size_t)row * slots + slot) * kHead + lane * 4;
   const uint2 raw = *reinterpret_cast<const uint2*>(src);
   float x[4] = {F::lo(raw.x), F::hi(raw.x), F::lo(raw.y), F::hi(raw.y)};
-  int pos = MT ? p.old_lens[b] + (row - b * p.q_len) : p.old_lens[b];  // the rotary position, and the slot unless TREE
-  const int wpos = pos;
-  if constexpr (TREE) {
-    int depth;
-    tree_walk(p.parents + (size_t)b * p.q_len, row - b * p.q_len, depth);
-    pos = p.old_lens[b] + depth;
-  }
+  int b, wpos, pos;
+  append_row<MT, TREE>(p, row, b, wpos, pos);
   const bool is_v = slot >= p.n_heads + p.n_groups;
 
   if (p.rope && !is_v) {
@@ -1217,22 +1232,20 @@ struct b2_span_attn {
   int grid = 0, nstage = 2, smem = 0, max_pieces = 1 << 20;
 };
 
-typedef void (*attn_kernel_t)(const AttnParams);
-typedef void (*attn_tok_kernel_t)(const AttnTokParams);
-static attn_kernel_t attn_kernel_for(const b2_span_cfg* c) {
-  return with_kv_mode(c->quant_mode, [&](auto QM) {
-    return with_flag(c->ft == B2_DT_F16, [&](auto H) -> attn_kernel_t { return span_attn_kernel<QM, H>; });
-  });
+// The step forms of the attention and append kernels: 0 single token, 1 chain (MT), 2 tree (MT, TREE).
+// form -> template arguments: f(std::bool_constant<MT>, std::bool_constant<TREE>)
+template <typename F>
+static auto with_step_form(int form, F&& f) {
+  if (form == 2) return f(std::true_type{}, std::true_type{});
+  if (form == 1) return f(std::true_type{}, std::false_type{});
+  return f(std::false_type{}, std::false_type{});
 }
-static attn_tok_kernel_t attn_tok_kernel_for(const b2_span_cfg* c) {
+
+template <bool MT, bool TREE>
+static auto attn_kernel_for(const b2_span_cfg* c) {
+  using kernel_t = void (*)(const AttnArgs<MT, TREE>);
   return with_kv_mode(c->quant_mode, [&](auto QM) {
-    return with_flag(c->ft == B2_DT_F16, [&](auto H) -> attn_tok_kernel_t { return span_attn_kernel<QM, H, true>; });
-  });
-}
-typedef void (*attn_tree_kernel_t)(const AttnTreeParams);
-static attn_tree_kernel_t attn_tree_kernel_for(const b2_span_cfg* c) {
-  return with_kv_mode(c->quant_mode, [&](auto QM) {
-    return with_flag(c->ft == B2_DT_F16, [&](auto H) -> attn_tree_kernel_t { return span_attn_kernel<QM, H, true, true>; });
+    return with_flag(c->ft == B2_DT_F16, [&](auto H) -> kernel_t { return span_attn_kernel<QM, H, MT, TREE>; });
   });
 }
 
@@ -1268,9 +1281,7 @@ int b2_span_attn_create(b2_span_attn_t* out, const b2_span_cfg* cfg, int max_bat
   if (!h) return B2_ERR_RUNTIME;
   h->cfg = *cfg;
   h->max_batch = max_batch;
-  attn_kernel_t kern = attn_kernel_for(cfg);
-  attn_tok_kernel_t kern_mt = attn_tok_kernel_for(cfg);
-  attn_tree_kernel_t kern_tree = attn_tree_kernel_for(cfg);
+  const auto kern = attn_kernel_for<false, false>(cfg);
   int sb = 0;
   with_kv_mode(cfg->quant_mode, [&](auto QM) {
     sb = KVTraits<QM>::STAGE;
@@ -1280,9 +1291,11 @@ int b2_span_attn_create(b2_span_attn_t* out, const b2_span_cfg* cfg, int max_bat
   if (h->nstage > 4) h->nstage = 4;
   const int merge = (4 * 16 * kMergeRS + 4 * 16 * 2) * 4;
   h->smem = h->nstage * sb > merge ? h->nstage * sb : merge;
-  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem);
-  if (e == cudaSuccess && cfg->head_size == kHead) e = cudaFuncSetAttribute(kern_mt, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem);
-  if (e == cudaSuccess && cfg->head_size == kHead) e = cudaFuncSetAttribute(kern_tree, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem);
+  cudaError_t e = cudaSuccess;
+  for (int form = 0; form < (cfg->head_size == kHead ? 3 : 1) && e == cudaSuccess; ++form)  // head 64 has the single-token form only
+    e = with_step_form(form, [&](auto MT, auto TREE) {
+      return cudaFuncSetAttribute(attn_kernel_for<MT, TREE>(cfg), cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem);
+    });
   int occ = 1;
   if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, kAttnThreads, h->smem);
   if (e != cudaSuccess) {
@@ -1328,16 +1341,32 @@ static size_t attn_workspace_bytes(const b2_span_attn* h, int rows) {
   return 2 * partial_slots(h) * rows * (kHead + 2) * sizeof(float) + 256;
 }
 
-// q_len == 0: the single-token kernel; otherwise the multi-token one, in its tree form when parents != NULL
+// the workspace of a step of q_len tokens per sequence (1: the single-token form)
+static size_t attn_step_workspace_bytes(const b2_span_attn* h, int q_len) {
+  return attn_workspace_bytes(h, tokens_per_block(&h->cfg, q_len) * (h->cfg.n_heads / h->cfg.n_groups));
+}
+
+// The checks of the attention entry points, in the order their callers observe.  ptrs_ok: no required pointer is NULL.
+static int attn_check(b2_span_attn_t h, bool ptrs_ok, int form, int batch, int q_len, int max_len, const void* workspace,
+                      size_t workspace_bytes) {
+  if (!h || !ptrs_ok) return B2_ERR_PARAM;
+  if (form != 0 && h->cfg.head_size != kHead) return B2_ERR_UNSUPPORTED;
+  if (q_len < 1 || q_len > kMaxQLen || batch <= 0 || (int64_t)batch * q_len > h->max_batch) return B2_ERR_LIMIT;
+  if (max_len <= 0 || (int64_t)(max_len + h->cfg.span_len - 1) / h->cfg.span_len > h->cfg.max_spans_per_seq) return B2_ERR_LIMIT;
+  if (!workspace || workspace_bytes < attn_step_workspace_bytes(h, q_len)) return B2_ERR_PARAM;
+  return B2_OK;
+}
+
+// q_len tokens per sequence (1 in the single-token form); parents: the tree form's
 static int attn_launch(b2_span_attn_t h, void* out, const void* q, const void* const* k_spans, const void* const* v_spans,
-                       const int32_t* new_lens, int batch, int q_len, void* workspace, float qk_scale, void* stream_,
-                       const int32_t* parents = nullptr) {
+                       const int32_t* new_lens, const int32_t* parents, int form, int batch, int q_len, void* workspace,
+                       float qk_scale, void* stream_) {
   const int hpg = h->cfg.n_heads / h->cfg.n_groups;
-  AttnTreeParams p;
+  AttnTreeParams p;  // each form's kernel takes the base it needs (AttnArgs)
   p.parents = parents;
   p.q_len = q_len;
-  p.tpb = q_len ? tokens_per_block(&h->cfg, q_len) : 1;
-  p.nrb = q_len ? (q_len + p.tpb - 1) / p.tpb : 1;
+  p.tpb = tokens_per_block(&h->cfg, q_len);
+  p.nrb = (q_len + p.tpb - 1) / p.tpb;
   p.rstride = p.tpb * hpg;
   const size_t rows = p.rstride;
   p.out = (__nv_bfloat16*)out;
@@ -1357,12 +1386,9 @@ static int attn_launch(b2_span_attn_t h, void* out, const void* q, const void* c
   p.span_len = h->cfg.span_len; p.span_shift = ilog2(h->cfg.span_len); p.max_spans = h->cfg.max_spans_per_seq;
   p.nstage = h->nstage;
   p.scale_log2 = qk_scale * 1.4426950408889634f;
-  const cudaError_t e =
-      parents ? launch(attn_tree_kernel_for(&h->cfg), dim3(h->grid), dim3(kAttnThreads), (size_t)h->smem, (cudaStream_t)stream_, true, p)
-      : q_len ? launch(attn_tok_kernel_for(&h->cfg), dim3(h->grid), dim3(kAttnThreads), (size_t)h->smem, (cudaStream_t)stream_, true,
-                       static_cast<const AttnTokParams&>(p))
-              : launch(attn_kernel_for(&h->cfg), dim3(h->grid), dim3(kAttnThreads), (size_t)h->smem,
-                       (cudaStream_t)stream_, true, static_cast<const AttnParams&>(p));
+  const cudaError_t e = with_step_form(form, [&](auto MT, auto TREE) {
+    return launch(attn_kernel_for<MT, TREE>(&h->cfg), dim3(h->grid), dim3(kAttnThreads), (size_t)h->smem, (cudaStream_t)stream_, true, p);
+  });
   if (e != cudaSuccess) {
     set_last_error("span_attn launch", e);
     return B2_ERR_CUDA;
@@ -1374,45 +1400,35 @@ extern "C" {
 
 size_t b2_span_attn_workspace_bytes(b2_span_attn_t h, int batch, int max_len) {
   if (!h || batch <= 0 || max_len <= 0) return 0;
-  return attn_workspace_bytes(h, h->cfg.n_heads / h->cfg.n_groups);
+  return attn_step_workspace_bytes(h, 1);
 }
 
 int b2_span_attn_run(b2_span_attn_t h, void* out, const void* q, const void* const* k_spans, const void* const* v_spans,
                      const int32_t* new_lens, int batch, int max_len, void* workspace, size_t workspace_bytes,
                      float qk_scale, void* stream_) {
-  if (!h || !out || !q || !k_spans || !v_spans || !new_lens) return B2_ERR_PARAM;
-  if (batch <= 0 || batch > h->max_batch) return B2_ERR_LIMIT;
-  if (max_len <= 0 || (int64_t)(max_len + h->cfg.span_len - 1) / h->cfg.span_len > h->cfg.max_spans_per_seq) return B2_ERR_LIMIT;
-  if (!workspace || workspace_bytes < b2_span_attn_workspace_bytes(h, batch, max_len)) return B2_ERR_PARAM;
+  if (int st = attn_check(h, out && q && k_spans && v_spans && new_lens, 0, batch, 1, max_len, workspace, workspace_bytes)) return st;
   if (h->cfg.head_size == 64) return span_attn64_run(&h->cfg, out, q, k_spans, v_spans, new_lens, batch, qk_scale, (cudaStream_t)stream_);
-  return attn_launch(h, out, q, k_spans, v_spans, new_lens, batch, 0, workspace, qk_scale, stream_);
+  return attn_launch(h, out, q, k_spans, v_spans, new_lens, nullptr, 0, batch, 1, workspace, qk_scale, stream_);
 }
 
 size_t b2_span_attn_tokens_workspace_bytes(b2_span_attn_t h, int batch, int q_len, int max_len) {
-  if (!h || batch <= 0 || q_len < 1 || q_len > 16 || max_len <= 0) return 0;
-  return attn_workspace_bytes(h, tokens_per_block(&h->cfg, q_len) * (h->cfg.n_heads / h->cfg.n_groups));
+  if (!h || batch <= 0 || q_len < 1 || q_len > kMaxQLen || max_len <= 0) return 0;
+  return attn_step_workspace_bytes(h, q_len);
 }
 
 int b2_span_attn_run_tokens(b2_span_attn_t h, void* out, const void* q, const void* const* k_spans, const void* const* v_spans,
                             const int32_t* new_lens, int batch, int q_len, int max_len, void* workspace, size_t workspace_bytes,
                             float qk_scale, void* stream_) {
-  if (!h || !out || !q || !k_spans || !v_spans || !new_lens) return B2_ERR_PARAM;
-  if (h->cfg.head_size != kHead) return B2_ERR_UNSUPPORTED;
-  if (q_len < 1 || q_len > 16 || batch <= 0 || (int64_t)batch * q_len > h->max_batch) return B2_ERR_LIMIT;
-  if (max_len <= 0 || (int64_t)(max_len + h->cfg.span_len - 1) / h->cfg.span_len > h->cfg.max_spans_per_seq) return B2_ERR_LIMIT;
-  if (!workspace || workspace_bytes < b2_span_attn_tokens_workspace_bytes(h, batch, q_len, max_len)) return B2_ERR_PARAM;
-  return attn_launch(h, out, q, k_spans, v_spans, new_lens, batch, q_len, workspace, qk_scale, stream_);
+  if (int st = attn_check(h, out && q && k_spans && v_spans && new_lens, 1, batch, q_len, max_len, workspace, workspace_bytes)) return st;
+  return attn_launch(h, out, q, k_spans, v_spans, new_lens, nullptr, 1, batch, q_len, workspace, qk_scale, stream_);
 }
 
 int b2_span_attn_run_tree(b2_span_attn_t h, void* out, const void* q, const void* const* k_spans, const void* const* v_spans,
                           const int32_t* new_lens, const int32_t* parents, int batch, int q_len, int max_len, void* workspace,
                           size_t workspace_bytes, float qk_scale, void* stream_) {
-  if (!h || !out || !q || !k_spans || !v_spans || !new_lens || !parents) return B2_ERR_PARAM;
-  if (h->cfg.head_size != kHead) return B2_ERR_UNSUPPORTED;
-  if (q_len < 1 || q_len > kMaxQLen || batch <= 0 || (int64_t)batch * q_len > h->max_batch) return B2_ERR_LIMIT;
-  if (max_len <= 0 || (int64_t)(max_len + h->cfg.span_len - 1) / h->cfg.span_len > h->cfg.max_spans_per_seq) return B2_ERR_LIMIT;
-  if (!workspace || workspace_bytes < b2_span_attn_tokens_workspace_bytes(h, batch, q_len, max_len)) return B2_ERR_PARAM;
-  return attn_launch(h, out, q, k_spans, v_spans, new_lens, batch, q_len, workspace, qk_scale, stream_, parents);
+  if (int st = attn_check(h, out && q && k_spans && v_spans && new_lens && parents, 2, batch, q_len, max_len, workspace, workspace_bytes))
+    return st;
+  return attn_launch(h, out, q, k_spans, v_spans, new_lens, parents, 2, batch, q_len, workspace, qk_scale, stream_);
 }
 
 int b2_span_context_copy(const b2_span_cfg* cfg, void* const* spans, const void* src, int64_t token_stride, int seq_len,
@@ -1441,13 +1457,22 @@ int b2_span_context_copy(const b2_span_cfg* cfg, void* const* spans, const void*
 
 }  // extern "C"
 
-// q_len == 0: one row per sequence (cache_append_kernel<..., MT = false>); otherwise q_len rows per sequence, the nodes of a
-// draft tree when parents != NULL
+// The checks of the append and compaction entry points, in the order their callers observe.  args_ok: no required pointer
+// is NULL and every count is positive.
+static int append_check(const b2_span_cfg* cfg, bool args_ok, int form, int q_len) {
+  if (int st = check_cfg(cfg)) return st;
+  if (form != 0 && cfg->head_size != kHead) return B2_ERR_UNSUPPORTED;
+  if (!args_ok) return B2_ERR_PARAM;
+  if (q_len < 1 || q_len > kMaxQLen) return B2_ERR_LIMIT;
+  return B2_OK;
+}
+
+// q_len rows per sequence (1 in the single-token form), the nodes of the draft tree `parents` in the tree form
 static int cache_append_launch(const b2_span_cfg* cfg, void* const* k_spans, void* const* v_spans, void* q_out, const void* qkv,
-                               const int32_t* old_lens, int batch, int q_len, const b2_rope_cfg* rope, void* stream_,
-                               const int32_t* parents = nullptr) {
+                               const int32_t* old_lens, const int32_t* parents, int form, int batch, int q_len,
+                               const b2_rope_cfg* rope, void* stream_) {
   if (rope && (rope->rotary_dim != 128 && rope->rotary_dim != 64)) return B2_ERR_UNSUPPORTED;
-  AppendTreeParams p;
+  AppendParams p;
   p.parents = parents;
   p.k_spans = k_spans; p.v_spans = v_spans;
   p.q_out = (__nv_bfloat16*)q_out; p.qkv = (const __nv_bfloat16*)qkv; p.old_lens = old_lens;
@@ -1457,14 +1482,12 @@ static int cache_append_launch(const b2_span_cfg* cfg, void* const* k_spans, voi
   p.rotary_dim = rope ? rope->rotary_dim : 0;
   p.log2_base = rope ? log2f(rope->base) : 0.f;
   p.q_len = q_len;
-  const int warps = batch * (q_len ? q_len : 1) * (cfg->n_heads + 2 * cfg->n_groups);
+  const int warps = batch * q_len * (cfg->n_heads + 2 * cfg->n_groups);
   const dim3 grid((warps + 3) / 4), block(128);
   const cudaError_t e = with_kv_mode(cfg->quant_mode, [&](auto QM) {
     return with_flag(cfg->ft == B2_DT_F16, [&](auto H) {
-      if (parents) return launch(cache_append_kernel<QM, H, true, true>, grid, block, 0, (cudaStream_t)stream_, true, p);
-      return with_flag(q_len != 0, [&](auto MT) {
-        return launch(cache_append_kernel<QM, H, MT>, grid, block, 0, (cudaStream_t)stream_, true,
-                      static_cast<const AppendParams&>(p));
+      return with_step_form(form, [&](auto MT, auto TREE) {
+        return launch(cache_append_kernel<QM, H, MT, TREE>, grid, block, 0, (cudaStream_t)stream_, true, p);
       });
     });
   });
@@ -1479,38 +1502,28 @@ extern "C" {
 
 int b2_span_cache_append(const b2_span_cfg* cfg, void* const* k_spans, void* const* v_spans, void* q_out,
                          const void* qkv, const int32_t* old_lens, int batch, const b2_rope_cfg* rope, void* stream_) {
-  if (int st = check_cfg(cfg)) return st;
-  if (!k_spans || !v_spans || !q_out || !qkv || !old_lens || batch <= 0) return B2_ERR_PARAM;
+  if (int st = append_check(cfg, k_spans && v_spans && q_out && qkv && old_lens && batch > 0, 0, 1)) return st;
   if (cfg->head_size == 64) return span_append64_run(cfg, k_spans, v_spans, q_out, qkv, old_lens, batch, rope, (cudaStream_t)stream_);
-  return cache_append_launch(cfg, k_spans, v_spans, q_out, qkv, old_lens, batch, 0, rope, stream_);
+  return cache_append_launch(cfg, k_spans, v_spans, q_out, qkv, old_lens, nullptr, 0, batch, 1, rope, stream_);
 }
 
 int b2_span_cache_append_tokens(const b2_span_cfg* cfg, void* const* k_spans, void* const* v_spans, void* q_out, const void* qkv,
                                 const int32_t* old_lens, int batch, int q_len, const b2_rope_cfg* rope, void* stream_) {
-  if (int st = check_cfg(cfg)) return st;
-  if (cfg->head_size != kHead) return B2_ERR_UNSUPPORTED;
-  if (!k_spans || !v_spans || !q_out || !qkv || !old_lens || batch <= 0) return B2_ERR_PARAM;
-  if (q_len < 1 || q_len > 16) return B2_ERR_LIMIT;
-  return cache_append_launch(cfg, k_spans, v_spans, q_out, qkv, old_lens, batch, q_len, rope, stream_);
+  if (int st = append_check(cfg, k_spans && v_spans && q_out && qkv && old_lens && batch > 0, 1, q_len)) return st;
+  return cache_append_launch(cfg, k_spans, v_spans, q_out, qkv, old_lens, nullptr, 1, batch, q_len, rope, stream_);
 }
 
 int b2_span_cache_append_tree(const b2_span_cfg* cfg, void* const* k_spans, void* const* v_spans, void* q_out, const void* qkv,
                               const int32_t* old_lens, const int32_t* parents, int batch, int q_len, const b2_rope_cfg* rope,
                               void* stream_) {
-  if (int st = check_cfg(cfg)) return st;
-  if (cfg->head_size != kHead) return B2_ERR_UNSUPPORTED;
-  if (!k_spans || !v_spans || !q_out || !qkv || !old_lens || !parents || batch <= 0) return B2_ERR_PARAM;
-  if (q_len < 1 || q_len > kMaxQLen) return B2_ERR_LIMIT;
-  return cache_append_launch(cfg, k_spans, v_spans, q_out, qkv, old_lens, batch, q_len, rope, stream_, parents);
+  if (int st = append_check(cfg, k_spans && v_spans && q_out && qkv && old_lens && parents && batch > 0, 2, q_len)) return st;
+  return cache_append_launch(cfg, k_spans, v_spans, q_out, qkv, old_lens, parents, 2, batch, q_len, rope, stream_);
 }
 
 int b2_span_cache_compact(const b2_span_cfg* cfg, void* const* const* k_tables, void* const* const* v_tables, int n_layers,
                           const int32_t* old_lens, const int32_t* accepted, const int32_t* path, int batch, int q_len,
                           void* stream_) {
-  if (int st = check_cfg(cfg)) return st;
-  if (cfg->head_size != kHead) return B2_ERR_UNSUPPORTED;
-  if (!k_tables || !v_tables || !old_lens || !accepted || !path || n_layers <= 0 || batch <= 0) return B2_ERR_PARAM;
-  if (q_len < 1 || q_len > kMaxQLen) return B2_ERR_LIMIT;
+  if (int st = append_check(cfg, k_tables && v_tables && old_lens && accepted && path && n_layers > 0 && batch > 0, 2, q_len)) return st;
   CompactParams p;
   p.k_tables = k_tables; p.v_tables = v_tables;
   p.old_lens = old_lens; p.accepted = accepted; p.path = path;

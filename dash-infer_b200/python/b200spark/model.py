@@ -331,6 +331,8 @@ class DecodeStack:
         if nh:
             ssq_o = self._ssq_o[:self._ssq_o.numel() // self.Bmax * self.B].view(-1, R)
             ssq_d = self._ssq_d[:self._ssq_d.numel() // self.Bmax * self.B].view(-1, R)
+        # the step form of append + attention: single token, chain of T tokens, or draft tree
+        form = {} if T == 1 else {"q_len": T, "parents": self.parents if self.tree else None}
         n = 0
         ops.embedding(self.embed, self.ids if T == 1 else self.tokens.view(-1), out=self.x); n += 1
         for li, L in enumerate(self.layers):
@@ -343,15 +345,8 @@ class DecodeStack:
             else:
                 ops.rmsnorm(self.x, L["g1"], cfg.eps, out=self.xn); n += 1
                 L["qkv"](self.xn, ws, out=self.qkv); n += 1
-            if T == 1:
-                ops.cache_append(L["cache"], self.qkv, self.lens_old, q_out=self.q, rope=self.rope); n += 1
-                self.attn(self.q, L["cache"], self.lens_new, self.max_len, ws, out=self.ao); n += 1
-            elif self.tree:
-                ops.cache_append_tree(L["cache"], self.qkv, self.lens_old, self.parents, T, q_out=self.q, rope=self.rope); n += 1
-                self.attn.run_tree(self.q, L["cache"], self.lens_new, self.parents, T, self.max_len, ws, out=self.ao); n += 1
-            else:
-                ops.cache_append_tokens(L["cache"], self.qkv, self.lens_old, T, q_out=self.q, rope=self.rope); n += 1
-                self.attn.run_tokens(self.q, L["cache"], self.lens_new, T, self.max_len, ws, out=self.ao); n += 1
+            ops._cache_append(L["cache"], self.qkv, self.lens_old, q_out=self.q, rope=self.rope, **form); n += 1
+            self.attn._run(self.q, L["cache"], self.lens_new, self.max_len, ws, out=self.ao, **form); n += 1
             if fn:
                 L["o"](self.ao, ws, out=self.x, residual=self.x, sumsq_out=self.ssq_o); n += 1
                 mlp_in, nin = self.x, (self.ssq_o, L["g2"], H, cfg.eps)
@@ -399,12 +394,11 @@ class DecodeStack:
                 self.comm.allgather(self.loc_val, self.all_val); n += 1
                 self.comm.allgather(self.loc_ids, self.all_ids); n += 1
             ops.argmax_merge(self.all_val, self.all_ids, out=self.next_ids); n += 1  # lowest rank on ties == lowest vocab id
-        if self.tree:  # greedy tree verification, then the accepted path's rows move to consecutive slots in every layer
-            ops.spec_accept_tree(self.accepted, self.path, self.next_ids, self.lens_old, self.lens_new, self.tokens, self.pred,
-                                 self.parents); n += 1
-            ops.cache_compact([L["cache"] for L in self.layers], self.lens_old, self.accepted, self.path, T); n += 1
-        elif T > 1:  # greedy verification: accepted counts, next token and lengths stay on the device
-            ops.spec_accept(self.accepted, self.next_ids, self.lens_old, self.lens_new, self.tokens, self.pred); n += 1
+        if T > 1:  # greedy verification: accepted counts, next token and lengths stay on the device
+            ops._spec_accept(self.accepted, self.next_ids, self.lens_old, self.lens_new, self.tokens, self.pred,
+                             self.path if self.tree else None, self.parents if self.tree else None); n += 1
+            if self.tree:  # the accepted path's rows move to consecutive slots in every layer
+                ops.cache_compact([L["cache"] for L in self.layers], self.lens_old, self.accepted, self.path, T); n += 1
         else:
             ops.lens_add(self.lens_old, 1); n += 1
             ops.lens_add(self.lens_new, 1); n += 1

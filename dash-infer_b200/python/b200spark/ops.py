@@ -236,68 +236,64 @@ class SpanCache:
         return pool[off: off + self.span_bytes]
 
 
-def cache_append(cache, qkv, old_lens, q_out=None, rope=None):
+def _cache_append(cache, qkv, old_lens, q_out=None, rope=None, q_len=None, parents=None):
+    """Append one step's rows to the span cache (+ optional fused rotary).  q_len None: row b of qkv is sequence b, written at
+    position old_lens[b].  q_len: row b*q_len + t is token t of sequence b, written at position old_lens[b] + t; with parents
+    (int32 [B, q_len]) it is node t of sequence b's draft tree, written at slot old_lens[b] + t with rotary position
+    old_lens[b] + depth(t)."""
     cfg = cache.cfg
-    B = qkv.shape[0]
+    rows = qkv.shape[0]
+    assert rows % (q_len or 1) == 0 and (parents is None or (q_len and parents.dtype == torch.int32 and parents.is_contiguous()))
     if q_out is None:
-        q_out = torch.empty(B, cfg.n_heads * cfg.head_size, dtype=qkv.dtype, device=qkv.device)
+        q_out = torch.empty(rows, cfg.n_heads * cfg.head_size, dtype=qkv.dtype, device=qkv.device)
     r = RopeCfg(float(rope[0]), int(rope[1]), 0) if rope is not None else None
-    check(lib.b2_span_cache_append(C.byref(cfg), _ptr(cache.k_tab), _ptr(cache.v_tab), _ptr(q_out), _ptr(qkv),
-                                   _ptr(old_lens), B, C.byref(r) if r is not None else None, _stream()),
-          "b2_span_cache_append")
+    head = (C.byref(cfg), _ptr(cache.k_tab), _ptr(cache.v_tab), _ptr(q_out), _ptr(qkv), _ptr(old_lens))
+    tail = (C.byref(r) if r is not None else None, _stream())
+    if q_len is None:
+        check(lib.b2_span_cache_append(*head, rows, *tail), "b2_span_cache_append")
+    elif parents is None:
+        check(lib.b2_span_cache_append_tokens(*head, rows // q_len, int(q_len), *tail), "b2_span_cache_append_tokens")
+    else:
+        check(lib.b2_span_cache_append_tree(*head, _ptr(parents), rows // q_len, int(q_len), *tail), "b2_span_cache_append_tree")
     return q_out
+
+
+def cache_append(cache, qkv, old_lens, q_out=None, rope=None):
+    return _cache_append(cache, qkv, old_lens, q_out, rope)
 
 
 def cache_append_tokens(cache, qkv, old_lens, q_len, q_out=None, rope=None):
-    """Multi-token append: row b*q_len + t of qkv is token t of sequence b, written at position old_lens[b] + t."""
-    cfg = cache.cfg
-    rows = qkv.shape[0]
-    assert rows % q_len == 0
-    if q_out is None:
-        q_out = torch.empty(rows, cfg.n_heads * cfg.head_size, dtype=qkv.dtype, device=qkv.device)
-    r = RopeCfg(float(rope[0]), int(rope[1]), 0) if rope is not None else None
-    check(lib.b2_span_cache_append_tokens(C.byref(cfg), _ptr(cache.k_tab), _ptr(cache.v_tab), _ptr(q_out), _ptr(qkv),
-                                          _ptr(old_lens), rows // q_len, int(q_len), C.byref(r) if r is not None else None,
-                                          _stream()), "b2_span_cache_append_tokens")
-    return q_out
-
-
-def spec_accept(accepted, next_ids, old_lens, new_lens, tokens, pred):
-    """Greedy verification of a multi-token step (b2_spec_accept): tokens / pred int64 [B, T]; writes accepted (int32 [B]),
-    next_ids (int64 [B] or None) and tokens[:, 0], advances old_lens by the accepted counts and sets new_lens = old_lens + T."""
-    B, T = tokens.shape
-    assert tokens.is_contiguous() and pred.is_contiguous() and pred.shape == tokens.shape
-    check(lib.b2_spec_accept(_ptr(accepted), _ptr(next_ids), _ptr(old_lens), _ptr(new_lens), _ptr(tokens), _ptr(pred), B, T,
-                             _stream()), "b2_spec_accept")
-    return accepted
+    return _cache_append(cache, qkv, old_lens, q_out, rope, q_len)
 
 
 def cache_append_tree(cache, qkv, old_lens, parents, q_len, q_out=None, rope=None):
-    """Draft-tree append (b2_span_cache_append_tree): row b*q_len + t of qkv is node t of sequence b's tree (parents int32
-    [B, q_len]), written at slot old_lens[b] + t with rotary position old_lens[b] + depth(t)."""
-    cfg = cache.cfg
-    rows = qkv.shape[0]
-    assert rows % q_len == 0 and parents.dtype == torch.int32 and parents.is_contiguous()
-    if q_out is None:
-        q_out = torch.empty(rows, cfg.n_heads * cfg.head_size, dtype=qkv.dtype, device=qkv.device)
-    r = RopeCfg(float(rope[0]), int(rope[1]), 0) if rope is not None else None
-    check(lib.b2_span_cache_append_tree(C.byref(cfg), _ptr(cache.k_tab), _ptr(cache.v_tab), _ptr(q_out), _ptr(qkv),
-                                        _ptr(old_lens), _ptr(parents), rows // q_len, int(q_len),
-                                        C.byref(r) if r is not None else None, _stream()), "b2_span_cache_append_tree")
-    return q_out
+    return _cache_append(cache, qkv, old_lens, q_out, rope, q_len, parents)
 
 
-def spec_accept_tree(accepted, path, next_ids, old_lens, new_lens, tokens, pred, parents):
-    """Greedy verification of a draft tree (b2_spec_accept_tree): tokens / pred int64 [B, T], parents int32 [B, T]; writes
-    accepted (int32 [B]), path (int32 [B, T], the first accepted[b] entries), next_ids (int64 [B] or None) and tokens[:, 0],
-    advances old_lens by the accepted counts and sets new_lens = old_lens + T."""
+def _spec_accept(accepted, next_ids, old_lens, new_lens, tokens, pred, path=None, parents=None):
+    """Greedy verification of a multi-token step (b2_spec_accept): tokens / pred int64 [B, T]; writes accepted (int32 [B]),
+    next_ids (int64 [B] or None) and tokens[:, 0], advances old_lens by the accepted counts and sets new_lens = old_lens + T.
+    With parents (int32 [B, T]) the step is a draft tree (b2_spec_accept_tree), which also writes path (int32 [B, T], the first
+    accepted[b] entries)."""
     B, T = tokens.shape
     assert tokens.is_contiguous() and pred.is_contiguous() and pred.shape == tokens.shape
+    if parents is None:
+        check(lib.b2_spec_accept(_ptr(accepted), _ptr(next_ids), _ptr(old_lens), _ptr(new_lens), _ptr(tokens), _ptr(pred), B, T,
+                                 _stream()), "b2_spec_accept")
+        return accepted
     assert parents.dtype == torch.int32 and parents.is_contiguous() and parents.shape == tokens.shape
     assert path.dtype == torch.int32 and path.is_contiguous() and path.shape == tokens.shape
     check(lib.b2_spec_accept_tree(_ptr(accepted), _ptr(path), _ptr(next_ids), _ptr(old_lens), _ptr(new_lens), _ptr(tokens),
                                   _ptr(pred), _ptr(parents), B, T, _stream()), "b2_spec_accept_tree")
     return accepted, path
+
+
+def spec_accept(accepted, next_ids, old_lens, new_lens, tokens, pred):
+    return _spec_accept(accepted, next_ids, old_lens, new_lens, tokens, pred)
+
+
+def spec_accept_tree(accepted, path, next_ids, old_lens, new_lens, tokens, pred, parents):
+    return _spec_accept(accepted, next_ids, old_lens, new_lens, tokens, pred, path, parents)
 
 
 _COMPACT_TABLES = {}
@@ -342,47 +338,38 @@ class SpanAttn:
     def workspace_bytes(self, batch, max_len):
         return lib.b2_span_attn_workspace_bytes(self.h, batch, max_len)
 
-    def __call__(self, q, cache, new_lens, max_len, ws, out=None, scale=None):
-        B = q.shape[0]
-        if out is None:
-            out = torch.empty_like(q)
-        if scale is None:
-            scale = 1.0 / (self.cfg.head_size ** 0.5)
-        wsb = ws.reserve(self.workspace_bytes(B, max_len))
-        check(lib.b2_span_attn_run(self.h, _ptr(out), _ptr(q), _ptr(cache.k_tab), _ptr(cache.v_tab), _ptr(new_lens), B,
-                                   int(max_len), _ptr(wsb), wsb.numel(), float(scale), _stream()), "b2_span_attn_run")
-        return out
-
     def tokens_workspace_bytes(self, batch, q_len, max_len):
         return lib.b2_span_attn_tokens_workspace_bytes(self.h, batch, q_len, max_len)
 
-    def run_tokens(self, q, cache, new_lens, q_len, max_len, ws, out=None, scale=None):
-        """Multi-token attention: q [batch*q_len, nH*128]; row b*q_len + t attends to tokens 0 .. new_lens[b] - q_len + t."""
-        B = q.shape[0] // q_len
+    def _run(self, q, cache, new_lens, max_len, ws, out=None, scale=None, q_len=None, parents=None):
+        """q_len None: q [batch, nH*128], row b attends to tokens 0 .. new_lens[b] - 1.  q_len: q [batch*q_len, nH*128], row
+        b*q_len + t attends to tokens 0 .. new_lens[b] - q_len + t; with parents (int32 [batch, q_len], a draft tree) to the
+        prefix (tokens < new_lens[b] - q_len) and to the slots new_lens[b] - q_len + j of t and its ancestors."""
+        B = q.shape[0] // (q_len or 1)
+        assert parents is None or (q_len and parents.dtype == torch.int32 and parents.is_contiguous())
         if out is None:
             out = torch.empty_like(q)
         if scale is None:
             scale = 1.0 / (self.cfg.head_size ** 0.5)
-        wsb = ws.reserve(self.tokens_workspace_bytes(B, q_len, max_len))
-        check(lib.b2_span_attn_run_tokens(self.h, _ptr(out), _ptr(q), _ptr(cache.k_tab), _ptr(cache.v_tab), _ptr(new_lens), B,
-                                          int(q_len), int(max_len), _ptr(wsb), wsb.numel(), float(scale), _stream()),
-              "b2_span_attn_run_tokens")
+        wsb = ws.reserve(self.workspace_bytes(B, max_len) if q_len is None else self.tokens_workspace_bytes(B, q_len, max_len))
+        head = (self.h, _ptr(out), _ptr(q), _ptr(cache.k_tab), _ptr(cache.v_tab), _ptr(new_lens))
+        tail = (int(max_len), _ptr(wsb), wsb.numel(), float(scale), _stream())
+        if q_len is None:
+            check(lib.b2_span_attn_run(*head, B, *tail), "b2_span_attn_run")
+        elif parents is None:
+            check(lib.b2_span_attn_run_tokens(*head, B, int(q_len), *tail), "b2_span_attn_run_tokens")
+        else:
+            check(lib.b2_span_attn_run_tree(*head, _ptr(parents), B, int(q_len), *tail), "b2_span_attn_run_tree")
         return out
 
+    def __call__(self, q, cache, new_lens, max_len, ws, out=None, scale=None):
+        return self._run(q, cache, new_lens, max_len, ws, out, scale)
+
+    def run_tokens(self, q, cache, new_lens, q_len, max_len, ws, out=None, scale=None):
+        return self._run(q, cache, new_lens, max_len, ws, out, scale, q_len)
+
     def run_tree(self, q, cache, new_lens, parents, q_len, max_len, ws, out=None, scale=None):
-        """Draft-tree attention: q [batch*q_len, nH*128]; row b*q_len + t attends to the prefix (tokens < new_lens[b] - q_len)
-        and to the slots new_lens[b] - q_len + j of t and its ancestors in parents (int32 [batch, q_len])."""
-        B = q.shape[0] // q_len
-        assert parents.dtype == torch.int32 and parents.is_contiguous()
-        if out is None:
-            out = torch.empty_like(q)
-        if scale is None:
-            scale = 1.0 / (self.cfg.head_size ** 0.5)
-        wsb = ws.reserve(self.tokens_workspace_bytes(B, q_len, max_len))
-        check(lib.b2_span_attn_run_tree(self.h, _ptr(out), _ptr(q), _ptr(cache.k_tab), _ptr(cache.v_tab), _ptr(new_lens),
-                                        _ptr(parents), B, int(q_len), int(max_len), _ptr(wsb), wsb.numel(), float(scale),
-                                        _stream()), "b2_span_attn_run_tree")
-        return out
+        return self._run(q, cache, new_lens, max_len, ws, out, scale, q_len, parents)
 
     def algo_bytes(self, total_tokens):
         return lib.b2_span_attn_algo_bytes(C.byref(self.cfg), int(total_tokens))
