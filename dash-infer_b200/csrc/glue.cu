@@ -217,6 +217,15 @@ __global__ void __launch_bounds__(128) embedding_kernel(__nv_bfloat16* __restric
     *reinterpret_cast<uint4*>(out + (size_t)b * hidden + i) = *reinterpret_cast<const uint4*>(table + (size_t)id * hidden + i);
 }
 
+// Order of greedy sampling (torch.argmax's): NaN ranks above every number; among equal values or among NaNs the lower
+// index wins.  (v, i) beats (best, bi) under that order.  The start (-inf, INT_MAX) loses to any element, so every row of
+// n >= 1 elements yields an index in [0, n).
+__device__ __forceinline__ bool argmax_beats(float v, int i, float best, int bi) {
+  const bool vn = v != v, bn = best != best;
+  if (vn != bn) return vn;
+  return (!vn && v > best) || ((vn || v == best) && i < bi);
+}
+
 // greedy sampling: lowest index among the maxima (bit-exact index contract)
 template <bool H>
 __global__ void __launch_bounds__(1024) argmax_kernel(int64_t* __restrict__ ids_out, float* __restrict__ vals_out,
@@ -231,13 +240,13 @@ __global__ void __launch_bounds__(1024) argmax_kernel(int64_t* __restrict__ ids_
   int bi = 0x7fffffff;
   for (int i = threadIdx.x; i < n; i += 1024) {
     const float v = Ft<H>::to_f(row[i]);
-    if (v > best || (v == best && i < bi)) { best = v; bi = i; }
+    if (argmax_beats(v, i, best, bi)) { best = v; bi = i; }
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
     const float ov = __shfl_xor_sync(0xffffffffu, best, o);
     const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-    if (ov > best || (ov == best && oi < bi)) { best = ov; bi = oi; }
+    if (argmax_beats(ov, oi, best, bi)) { best = ov; bi = oi; }
   }
   if ((threadIdx.x & 31) == 0) { sv[threadIdx.x >> 5] = best; si[threadIdx.x >> 5] = bi; }
   __syncthreads();
@@ -248,7 +257,7 @@ __global__ void __launch_bounds__(1024) argmax_kernel(int64_t* __restrict__ ids_
     for (int o = 16; o > 0; o >>= 1) {
       const float ov = __shfl_xor_sync(0xffffffffu, best, o);
       const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-      if (ov > best || (ov == best && oi < bi)) { best = ov; bi = oi; }
+      if (argmax_beats(ov, oi, best, bi)) { best = ov; bi = oi; }
     }
     if (threadIdx.x == 0) {
       ids_out[b] = bi + id_offset;
@@ -297,7 +306,8 @@ __global__ void spec_accept_kernel(int32_t* accepted, int32_t* path, int64_t* ne
   new_lens[b] = ol + q_len;
 }
 
-// vocab-split lm_head: pick the global winner among the ranks' (max, argmax) pairs; ties -> lowest rank == lowest vocab id
+// vocab-split lm_head: pick the global winner among the ranks' (max, argmax) pairs under argmax_beats' order; ties (equal
+// values, or NaN on several ranks) -> lowest rank == lowest vocab id
 __global__ void argmax_merge_kernel(int64_t* ids_out, const float* vals, const int64_t* ids, int nranks, int batch) {
   pdl_wait();
   pdl_launch_dependents();
@@ -307,7 +317,7 @@ __global__ void argmax_merge_kernel(int64_t* ids_out, const float* vals, const i
   int64_t bid = ids[b];
   for (int r = 1; r < nranks; ++r) {
     const float v = vals[(size_t)r * batch + b];
-    if (v > best) { best = v; bid = ids[(size_t)r * batch + b]; }
+    if (argmax_beats(v, 0, best, 0)) { best = v; bid = ids[(size_t)r * batch + b]; }
   }
   ids_out[b] = bid;
 }
@@ -315,6 +325,9 @@ __global__ void argmax_merge_kernel(int64_t* ids_out, const float* vals, const i
 }  // namespace b2
 
 using namespace b2;
+
+// the vector loads and stores of the kernels above: 16 bytes (uint4) for rmsnorm / binary / embedding, 8 (uint2) for rotary
+static bool aligned(const void* p, uintptr_t bytes) { return ((uintptr_t)p & (bytes - 1)) == 0; }
 
 #define B2_LAUNCH_CHECK(name, call)            \
   do {                                         \
@@ -341,6 +354,7 @@ extern "C" {
 int b2_rmsnorm_ft(void* y, const void* x, const void* gamma, int rows, int cols, float eps, int ft, void* stream) {
   if (!y || !x || !gamma || rows <= 0 || cols <= 0) return B2_ERR_PARAM;
   if (cols % 8 || (ft != B2_DT_BF16 && ft != B2_DT_F16)) return B2_ERR_UNSUPPORTED;
+  if (!aligned(y, 16) || !aligned(x, 16) || !aligned(gamma, 16)) return B2_ERR_UNSUPPORTED;
   if (ft == B2_DT_F16)
     B2_LAUNCH_CHECK("rmsnorm", launch(rmsnorm_kernel<true>, dim3(rows), dim3(256), 0, (cudaStream_t)stream, true, (__nv_bfloat16*)y,
                                       (const __nv_bfloat16*)x, (const __nv_bfloat16*)gamma, cols, eps));
@@ -365,7 +379,7 @@ int b2_quant_fp8(void* y, int64_t ldy, float* scale, float* tile_sums, const voi
 int b2_rotary(void* qkv, const int32_t* pos, int batch, int n_heads, int n_groups, int head_size, const b2_rope_cfg* rope,
               void* stream) {
   if (!qkv || !pos || !rope || batch <= 0) return B2_ERR_PARAM;
-  if (head_size != 128 || (rope->rotary_dim != 128 && rope->rotary_dim != 64)) return B2_ERR_UNSUPPORTED;
+  if (head_size != 128 || (rope->rotary_dim != 128 && rope->rotary_dim != 64) || !aligned(qkv, 8)) return B2_ERR_UNSUPPORTED;
   const int warps = batch * (n_heads + n_groups);
   B2_LAUNCH_CHECK("rotary", launch(rotary_kernel, dim3((warps + 3) / 4), dim3(128), 0, (cudaStream_t)stream, true,
                                    (__nv_bfloat16*)qkv, pos, batch, n_heads, n_groups, rope->rotary_dim, log2f(rope->base)));
@@ -375,6 +389,7 @@ int b2_rotary(void* qkv, const int32_t* pos, int batch, int n_heads, int n_group
 int b2_binary_ft(void* out, const void* a, const void* b, int64_t n, int op, int ft, void* stream) {
   if (!out || !a || !b || n <= 0) return B2_ERR_PARAM;
   if ((op != B2_BIN_ADD && op != B2_BIN_MUL) || (ft != B2_DT_BF16 && ft != B2_DT_F16)) return B2_ERR_UNSUPPORTED;
+  if (!aligned(out, 16) || !aligned(a, 16) || !aligned(b, 16)) return B2_ERR_UNSUPPORTED;
   const int64_t blocks = (n + 2047) / 2048;
   if (ft == B2_DT_F16)
     B2_LAUNCH_CHECK("binary", launch(binary_kernel<true>, dim3((unsigned)blocks), dim3(256), 0, (cudaStream_t)stream, true,
@@ -390,7 +405,7 @@ int b2_binary(void* out, const void* a, const void* b, int64_t n, int op, void* 
 
 int b2_embedding(void* out, const void* table, const int64_t* ids, int batch, int hidden, void* stream) {
   if (!out || !table || !ids || batch <= 0 || hidden <= 0) return B2_ERR_PARAM;
-  if (hidden % 8) return B2_ERR_UNSUPPORTED;
+  if (hidden % 8 || !aligned(out, 16) || !aligned(table, 16)) return B2_ERR_UNSUPPORTED;
   B2_LAUNCH_CHECK("embedding", launch(embedding_kernel, dim3(batch), dim3(128), 0, (cudaStream_t)stream, true, (__nv_bfloat16*)out,
                                       (const __nv_bfloat16*)table, ids, hidden));
   return B2_OK;
@@ -398,7 +413,7 @@ int b2_embedding(void* out, const void* table, const int64_t* ids, int batch, in
 
 int b2_argmax_ft(int64_t* ids_out, float* vals_out, const void* logits, int batch, int n, int64_t ld, int64_t id_offset, int ft,
                  void* stream) {
-  if (!ids_out || !logits || batch <= 0 || n <= 0) return B2_ERR_PARAM;
+  if (!ids_out || !logits || batch <= 0 || n <= 0 || ld < n) return B2_ERR_PARAM;
   if (ft != B2_DT_BF16 && ft != B2_DT_F16) return B2_ERR_UNSUPPORTED;
   if (ft == B2_DT_F16)
     B2_LAUNCH_CHECK("argmax", launch(argmax_kernel<true>, dim3(batch), dim3(1024), 0, (cudaStream_t)stream, true, ids_out, vals_out,

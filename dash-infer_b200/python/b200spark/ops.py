@@ -411,6 +411,8 @@ def quant_fp8(x, gamma=None, eps=1e-6, out=None):
 
 
 def rotary(qkv, pos, n_heads, n_groups, base=1e6, rotary_dim=128):
+    if qkv.dtype != torch.bfloat16:  # b2_rotary is bf16 only (fp16 models rotate in the fused cache append)
+        raise TypeError(f"rotary: qkv must be bfloat16, got {qkv.dtype}")
     r = RopeCfg(float(base), int(rotary_dim), 0)
     check(lib.b2_rotary(_ptr(qkv), _ptr(pos), qkv.shape[0], n_heads, n_groups, 128, C.byref(r), _stream()), "b2_rotary")
     return qkv
@@ -437,6 +439,8 @@ def argmax(logits, out=None):
 
 
 def argmax_shard(logits, id_offset, ids_out, vals_out):
+    if logits.dtype != torch.bfloat16:  # b2_argmax_shard is bf16 only
+        raise TypeError(f"argmax_shard: logits must be bfloat16, got {logits.dtype}")
     B, n = logits.shape
     check(lib.b2_argmax_shard(_ptr(ids_out), _ptr(vals_out), _ptr(logits), B, n, logits.stride(0), int(id_offset), _stream()),
           "b2_argmax_shard")
