@@ -92,6 +92,12 @@ struct KVTraits {
   static constexpr int PARAM = kTile * PARAM_ROW;                      // K (or V) {zero, scale} of a stage
   static constexpr int STAGE = 2 * TILE + 2 * PARAM;
   static constexpr int kStages = QM == B2_KV_NONE ? 2 : (QM == B2_KV_U4 ? 4 : 3);  // default ring depth (B2_ATTN_STAGES)
+  // tile_compute_q rounds P' = P * s_v * 2^kPExp to fp16.  Without the power of two a small V scale puts P' among the fp16
+  // subnormals (spacing 2^-24), whose error relative to the output grows as V shrinks.  The exponent keeps s_v 2^kPExp
+  // below 65504 for per-row max|v| <= 4096 (u4: s_v <= 8192 / 15, i8: 8192 / 255, fp8: 4096 / 448); l carries the same
+  // factor, so o / l is what it would be without it, bit for bit.
+  static constexpr int kPExp = QM == B2_KV_U4 ? 6 : (QM == B2_KV_I8 ? 10 : (QM == B2_KV_FP8 ? 12 : 0));
+  static constexpr float kPScale = static_cast<float>(1 << kPExp);
   // byte offset of row rowi's {zero, scale} in a span of n_rows = n_groups * span_len rows
   __device__ __forceinline__ static size_t param_offset(size_t n_rows, size_t rowi) { return n_rows * ROW + rowi * PARAM_ROW; }
   __device__ __forceinline__ static int swz(int row, int c) { return QM == B2_KV_U4 ? c ^ ((row >> 1) & 3) : c ^ (row & 7); }
@@ -441,8 +447,8 @@ __device__ __forceinline__ void tile_compute_q(const uint8_t* st, int warp, int 
     // and the 16-byte param chunk of an odd-length tail covers one unwritten token): their V params must not reach
     // the arithmetic (0 * NaN), so they are forced to zero exactly like the scores are forced to -inf
     const bool live0 = wtok + nt * 8 + 2 * t < mask.tok1, live1 = wtok + nt * 8 + 2 * t + 1 < mask.tok1;
-    vz[nt][0] = live0 ? vp.x : 0.f; vs[nt][0] = live0 ? vp.y : 0.f;
-    vz[nt][1] = live1 ? vp.z : 0.f; vs[nt][1] = live1 ? vp.w : 0.f;
+    vz[nt][0] = live0 ? vp.x : 0.f; vs[nt][0] = live0 ? vp.y * T::kPScale : 0.f;
+    vz[nt][1] = live1 ? vp.z : 0.f; vs[nt][1] = live1 ? vp.w * T::kPScale : 0.f;
 #pragma unroll
     for (int cc = 0; cc < 4; ++cc) {
       const int tok = wtok + nt * 8 + 2 * t + (cc & 1);
@@ -463,7 +469,7 @@ __device__ __forceinline__ void tile_compute_q(const uint8_t* st, int warp, int 
     for (int cc = 0; cc < 4; ++cc) {
       const float pv = exp2f(sc[nt][cc] - msub[cc >> 1]);
       psum[cc >> 1] += pv;
-      pq[cc] = pv * vs[nt][cc & 1];  // fold the V scale into the probability
+      pq[cc] = pv * vs[nt][cc & 1];  // fold the V scale (times 2^kPExp) into the probability
     }
     pa[2 * nt] = pack_f16x2(pq[0], pq[1]);
     pa[2 * nt + 1] = pack_f16x2(pq[2], pq[3]);
@@ -855,11 +861,11 @@ __global__ void __launch_bounds__(kAttnThreads) span_attn_kernel(const AttnArgs<
         }
       }
     }
-    if (t == 0) {
+    if (t == 0) {  // quantized: o carries the 2^kPExp folded into P', and l takes it here (exact), so o / l is unchanged
       mrg_ml[(warp * 16 + gq) * 2] = mrow[0];
-      mrg_ml[(warp * 16 + gq) * 2 + 1] = lrow[0];
+      mrg_ml[(warp * 16 + gq) * 2 + 1] = T::kCodesF16 ? lrow[0] * T::kPScale : lrow[0];
       mrg_ml[(warp * 16 + gq + 8) * 2] = mrow[1];
-      mrg_ml[(warp * 16 + gq + 8) * 2 + 1] = lrow[1];
+      mrg_ml[(warp * 16 + gq + 8) * 2 + 1] = T::kCodesF16 ? lrow[1] * T::kPScale : lrow[1];
     }
     __syncthreads();
     // thread d = tid handles column d of every head row

@@ -223,6 +223,11 @@ int b2_span_attn_destroy(b2_span_attn_t handle);
 size_t b2_span_attn_workspace_bytes(b2_span_attn_t handle, int batch, int max_len);
 
 /* out [batch, n_heads*head_size] FT = softmax(qk_scale * q K^T) V over the first new_lens[b] tokens.
+ * I8 / U4 / FP8: the MMAs run in fp16, so |q| < 65504 after Q's conversion to fp16, and each probability times its
+ * token's V scale is rounded to fp16 with a per-mode power of two folded in.  Accuracy window: for V rows (before
+ * quantization) with per-row max|v| in [2^-12, 2^12] the output meets the attention error envelope (probabilities far
+ * below the row's maximum may still round as fp16 subnormals; their error stays inside the envelope).  Above per-row
+ * max|v| ~ 2^12.8 the rounded products can overflow to inf and the output is undefined.
  * new_lens: device int32 [batch] (including the token appended this step).  max_len bounds every
  * new_lens[b] (only sizes the workspace check; a loose bound is fine).
  * workspace >= workspace_bytes(batch,max_len), 16B aligned, contents undefined on entry/exit. */
