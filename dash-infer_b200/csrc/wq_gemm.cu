@@ -18,7 +18,8 @@
 //     in shared memory and every CTA sums and finishes its share of the tile through distributed shared memory (slice order:
 //     deterministic).  Fallback (narrow shapes, forced splits, the fused all-reduce): fp32 partials in the caller's workspace,
 //     the last CTA of an n-group (device counter) sums them in fixed order.  Either way: fused bias / activation / residual /
-//     SwiGLU, optionally a self-contained RMSNorm prologue (b2_gemm_fuse).
+//     SwiGLU, optionally a self-contained RMSNorm (b2_gemm_fuse): the kernel normalises its own activations, nothing comes
+//     from the producer (the RMSNorm hand-off of batches >= 17 belongs to the wgmma kernel, wq_gemm_tc.cu).
 //   * the 16-bit type of activations / outputs / scales is a template parameter (Ft<H>: bf16 or fp16; fp16 uses 128 + q).
 //
 // Roofline: HBM-bound; algorithmic bytes/launch = K*N*wbits/8 + 4*G*N + 2*M*(K+N).
@@ -58,15 +59,13 @@ struct GemmParams {
   int nst_log2;     // log2(pipeline stages)
   int act;
   float alpha;
-  // optional RMSNorm fusion (b2_gemm_fuse)
-  const float* norm_sumsq;
-  const __nv_bfloat16* norm_gamma;
-  int norm_parts;
   int cluster;    // 1: the S k-slices of a tile are one thread-block cluster; partial tiles are summed through distributed
                   //    shared memory (no workspace, no counters)
-  int norm_self;  // 1: the kernel takes the row statistics itself while staging the activations (K == hidden)
+  // optional self-contained RMSNorm (b2_gemm_fuse): the kernel takes the row statistics itself while staging the
+  // activations (K == hidden)
+  int norm_self;
+  const __nv_bfloat16* norm_gamma;
   float norm_inv_hidden, norm_eps;
-  float* sumsq_out;
   // optional fused all-reduce of the output over tensor-parallel ranks (b2_gemm_wq_run_allreduce)
   int comm_on;
   CommDev comm;
@@ -144,8 +143,15 @@ B2_TRACE_DECL(g_gemv_tr)
 extern "C" int b2_debug_trace_gemv(unsigned long long* host_out) { return (int)cudaMemcpyFromSymbol(host_out, g_gemv_tr, sizeof(g_gemv_tr)); }
 #endif
 
+// CTAs per SM each instantiation is compiled for (registers <= 65536 / (kThreads * n)).  make_plan sizes the split-K from
+// the occupancy, so this fixes the plans, and with them the summation order of every result; left to ptxas, the register
+// budget (and the occupancy) moves with unrelated edits of the kernel body.
+template <int W, int MT, bool G, bool H>
+constexpr int kMinCtasPerSm = MT == 1 ? ((W == 8 && (G || H)) || (W == 4 && G) ? 3 : 4)
+                                      : (W == 16 ? (H ? 3 : 4) : W == 4 && !H ? (G ? 2 : 4) : 3);
+
 template <int WBITS, int MT, bool GROUPED, bool H>
-__global__ void __launch_bounds__(kThreads) wq_gemm_kernel(const GemmParams p) {
+__global__ void __launch_bounds__(kThreads, (kMinCtasPerSm<WBITS, MT, GROUPED, H>)) wq_gemm_kernel(const GemmParams p) {
   using T = WTraits<WBITS>;
   using F = Ft<H>;  // bf16 / fp16 activations, outputs, bias, residual
   constexpr int MP = 8 * MT;
@@ -171,8 +177,9 @@ __global__ void __launch_bounds__(kThreads) wq_gemm_kernel(const GemmParams p) {
   float* fs = reinterpret_cast<float*>(grow + XS);           // [MP][kBN] partial tile
   float* suma = fs + MP * kBN;                                // [MP][groups per chunk] (or [MP])
   const int gpc = GROUPED ? p.xt / gt : 1;                    // groups per chunk
-  float* sinv = suma + MP * gpc;                              // [MP] rsqrt(mean square) of the activation rows (norm fusion)
-  float* srs = sinv + MP;                                     // [MP] 1/rms of the rows (self-contained norm), else unused
+  float* sumsq = suma + MP * gpc;  // [MP] self-contained norm: sum x^2 of the rows over this CTA's k-slice (all of K once
+                                   //      the workspace reducer has added the slices)
+  float* srs = sumsq + MP;         // [MP] self-contained norm: 1/rms of the rows
   uint64_t* full = reinterpret_cast<uint64_t*>((reinterpret_cast<uintptr_t>(srs + MP + 4) + 7) & ~uintptr_t(7));
   uint64_t* empty = full + NST;
   uint64_t* xbar = empty + NST;  // activation rows of a chunk landed (bulk copies)
@@ -239,17 +246,6 @@ __global__ void __launch_bounds__(kThreads) wq_gemm_kernel(const GemmParams p) {
   pdl_wait();  // activations / workspace / counters belong to the previous kernels from here on
   if (tr0) B2_TR(g_gemv_tr, 3);
 
-  if (p.norm_sumsq) {  // LayerNormNoBeta statistics from the producer's per-tile partial sums (fixed order)
-    for (int m = warp; m < MP; m += kWarps) {
-      float ss = 0.f;
-      if (m < p.M)
-        for (int i = lane; i < p.norm_parts; i += 32) ss += __ldcg(p.norm_sumsq + (size_t)i * p.M + m);
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
-      if (lane == 0) sinv[m] = rsqrtf(ss * p.norm_inv_hidden + p.norm_eps);
-    }
-    named_bar_sync(1, kWarps * 32);
-  }
   const uint32_t w_ring = smem_u32(ring);
   // this thread's rows (16*warp + g, +8) inside the [chunk][row ^ swz][16B] tile image
   const int wc = WBITS == 4 ? (t >> 1) : (WBITS == 8 ? t : 2 * t);
@@ -280,17 +276,7 @@ __global__ void __launch_bounds__(kThreads) wq_gemm_kernel(const GemmParams p) {
           float sacc = 0.f;
           for (int v = v0 + lane; v < v0 + gvec; v += 32) {
             uint4 val = make_uint4(0, 0, 0, 0);
-            if (mrow && kbase + v * 8 < p.K) {
-              val = *reinterpret_cast<const uint4*>(arow + v * 8);
-              if (p.norm_sumsq) {  // same fp32 op order and rounding as rmsnorm_kernel: (x * inv) * gamma -> bf16
-                const uint4 gv = *reinterpret_cast<const uint4*>(p.norm_gamma + kbase + v * 8);
-                const float inv = sinv[m];
-                val.x = F::pack(F::lo(val.x) * inv * F::lo(gv.x), F::hi(val.x) * inv * F::hi(gv.x));
-                val.y = F::pack(F::lo(val.y) * inv * F::lo(gv.y), F::hi(val.y) * inv * F::hi(gv.y));
-                val.z = F::pack(F::lo(val.z) * inv * F::lo(gv.z), F::hi(val.z) * inv * F::hi(gv.z));
-                val.w = F::pack(F::lo(val.w) * inv * F::lo(gv.w), F::hi(val.w) * inv * F::hi(gv.w));
-              }
-            }
+            if (mrow && kbase + v * 8 < p.K) val = *reinterpret_cast<const uint4*>(arow + v * 8);
             *reinterpret_cast<uint4*>(xrow + v * 16) = val;
             sacc += (F::lo(val.x) + F::hi(val.x)) + (F::lo(val.y) + F::hi(val.y)) +
                     (F::lo(val.z) + F::hi(val.z)) + (F::lo(val.w) + F::hi(val.w));
@@ -350,14 +336,6 @@ __global__ void __launch_bounds__(kThreads) wq_gemm_kernel(const GemmParams p) {
                   val.z = F::pack(x4 * F::lo(gv.z), x5 * F::hi(gv.z));
                   val.w = F::pack(x6 * F::lo(gv.w), x7 * F::hi(gv.w));
                   *reinterpret_cast<uint4*>(xrow + v * 16) = val;
-                } else if (p.norm_sumsq) {  // same fp32 op order and rounding as rmsnorm_kernel: (x * inv) * gamma -> bf16
-                  const uint4 gv = *reinterpret_cast<const uint4*>(p.norm_gamma + kbase + v * 8);
-                  const float inv = sinv[m];
-                  val.x = F::pack(F::lo(val.x) * inv * F::lo(gv.x), F::hi(val.x) * inv * F::hi(gv.x));
-                  val.y = F::pack(F::lo(val.y) * inv * F::lo(gv.y), F::hi(val.y) * inv * F::hi(gv.y));
-                  val.z = F::pack(F::lo(val.z) * inv * F::lo(gv.z), F::hi(val.z) * inv * F::hi(gv.z));
-                  val.w = F::pack(F::lo(val.w) * inv * F::lo(gv.w), F::hi(val.w) * inv * F::hi(gv.w));
-                  *reinterpret_cast<uint4*>(xrow + v * 16) = val;
                 }
               } else {
                 *reinterpret_cast<uint4*>(xrow + v * 16) = val;  // k >= K
@@ -376,7 +354,7 @@ __global__ void __launch_bounds__(kThreads) wq_gemm_kernel(const GemmParams p) {
         if (p.norm_self) {
 #pragma unroll
           for (int o = 16; o > 0; o >>= 1) ssq += __shfl_xor_sync(0xffffffffu, ssq, o);
-          if (lane == 0) sinv[m] = (xc0 == 0 ? 0.f : sinv[m]) + ssq;
+          if (lane == 0) sumsq[m] = (xc0 == 0 ? 0.f : sumsq[m]) + ssq;
         }
       }
     }
@@ -450,11 +428,11 @@ __global__ void __launch_bounds__(kThreads) wq_gemm_kernel(const GemmParams p) {
     cluster_arrive();
     cluster_wait();
     if (tr0) B2_TR(g_gemv_tr, 8);
-    const uint32_t fs_a = smem_u32(fs), sinv_a = smem_u32(sinv);
+    const uint32_t fs_a = smem_u32(fs), sumsq_a = smem_u32(sumsq);
     if (p.norm_self) {
       if (ctid < MP) {
         float ss = 0.f;
-        for (int r = 0; r < p.S; ++r) ss += ld_dsmem_f(dsmem_addr(sinv_a + ctid * 4, r));
+        for (int r = 0; r < p.S; ++r) ss += ld_dsmem_f(dsmem_addr(sumsq_a + ctid * 4, r));
         srs[ctid] = rsqrtf(ss * p.norm_inv_hidden + p.norm_eps);
       }
       named_bar_sync(1, kWarps * 32);
@@ -471,8 +449,7 @@ __global__ void __launch_bounds__(kThreads) wq_gemm_kernel(const GemmParams p) {
       }
       return a;
     };
-    const bool gather = p.comm_on || p.sumsq_out != nullptr;  // epilogues that need the whole tile in one CTA
-    if (!gather) {
+    if (!p.comm_on) {  // the fused all-reduce needs the whole tile in one CTA: gathered below
       if (p.act == B2_ACT_SWIGLU) {
         for (int i = s + p.S * ctid; i < p.M * 16; i += p.S * kWarps * 32) {
           const int m = i >> 4, cg = i & 15;
@@ -524,7 +501,7 @@ __global__ void __launch_bounds__(kThreads) wq_gemm_kernel(const GemmParams p) {
       if (tr0) B2_TR(g_gemv_tr, 11);
       return;
     }
-    // gather: slice 0 collects the whole tile and runs the single-CTA epilogue below
+    // fused all-reduce: slice 0 collects the whole tile and runs the exchange below
     if (s == 0) {
       for (int i = ctid; i < p.M * 32; i += kWarps * 32) {
         const float4 q = slice_sum(i * 4);
@@ -539,7 +516,7 @@ __global__ void __launch_bounds__(kThreads) wq_gemm_kernel(const GemmParams p) {
     for (int i = ctid * 4; i < p.M * kBN; i += kWarps * 32 * 4)
       *reinterpret_cast<float4*>(wsu + i) = *reinterpret_cast<const float4*>(fs + i);
     float* wsq = p.ws + (size_t)p.NG * p.S * MPK;  // [NG][S][MP] sum x^2 of each k-slice (self-contained norm)
-    if (p.norm_self && ctid < p.M) wsq[((size_t)ng * p.S + s) * MP + ctid] = sinv[ctid];
+    if (p.norm_self && ctid < p.M) wsq[((size_t)ng * p.S + s) * MP + ctid] = sumsq[ctid];
     __threadfence();
     named_bar_sync(1, kWarps * 32);
     if (tr0) B2_TR(g_gemv_tr, 7);
@@ -581,8 +558,8 @@ __global__ void __launch_bounds__(kThreads) wq_gemm_kernel(const GemmParams p) {
         ssq_h += __shfl_xor_sync(0xffffffffu, ssq_h, o);
       }
       if (lane == 0) {
-        sinv[warp] = ssq_l;
-        if (MP > kWarps) sinv[warp + kWarps] = ssq_h;
+        sumsq[warp] = ssq_l;
+        if (MP > kWarps) sumsq[warp + kWarps] = ssq_h;
       }
     }
     if (ctid == 0) p.counters[ng] = 0;  // re-arm for the next launch / graph replay
@@ -591,7 +568,7 @@ __global__ void __launch_bounds__(kThreads) wq_gemm_kernel(const GemmParams p) {
   }
 
   if (p.norm_self && !p.cluster) {  // sum x^2 -> 1/rms, one thread per row (the cluster path already has it)
-    if (ctid < MP) srs[ctid] = rsqrtf(sinv[ctid] * p.norm_inv_hidden + p.norm_eps);
+    if (ctid < MP) srs[ctid] = rsqrtf(sumsq[ctid] * p.norm_inv_hidden + p.norm_eps);
     named_bar_sync(1, kWarps * 32);
   }
   // ---- final: alpha (x 1/rms of the row), bias, activation, residual, bf16 store (coalesced along n)
@@ -708,27 +685,8 @@ __global__ void __launch_bounds__(kThreads) wq_gemm_kernel(const GemmParams p) {
       cp[0] = F::from_f(v0);
       if (has1) cp[1] = F::from_f(v1);
     }
-    if (p.sumsq_out) {  // keep what was actually stored (bf16-rounded) for the row statistics below
-      fs[m * kBN + np * 2] = F::to_f(F::from_f(v0));
-      fs[m * kBN + np * 2 + 1] = has1 ? F::to_f(F::from_f(v1)) : 0.f;
-    }
   }
   if (ng == 0 && ctid == 0) B2_TR(g_gemv_tr, 11);
-  if (p.sumsq_out) {  // per-tile sum of squares of the output rows, for the next op's fused RMSNorm
-    named_bar_sync(1, kWarps * 32);
-    for (int m = warp; m < p.M; m += kWarps) {
-      float ss = 0.f;
-#pragma unroll
-      for (int i = 0; i < kBN / 32; ++i) {
-        const int c = lane + 32 * i;
-        const float v = (ng * kBN + c) < p.N ? fs[m * kBN + c] : 0.f;
-        ss += v * v;
-      }
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
-      if (lane == 0) p.sumsq_out[(size_t)ng * p.M + m] = ss;
-    }
-  }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1207,26 +1165,32 @@ static int run_impl(b2_gemm_wq_t h, const void* A, int64_t lda, void* C, int64_t
                     const void* residual, int activation, float alpha, void* workspace, size_t workspace_bytes,
                     const b2_gemm_fuse* fuse, const CommDev* comm, void* stream_) {
   if (!h || !A || !C || M <= 0) return B2_ERR_PARAM;
-  const bool norm_self = fuse && !fuse->norm_sumsq && fuse->norm_gamma;
-  const bool fused = fuse && (fuse->norm_sumsq || fuse->sumsq_out || norm_self || fuse->xg_out);
-  if (fused && use_tc(h, M) && !comm) {
-    // ---- batches >= 17: the hand-off form only (pre-scaled activations in; scaled copy + statistics out)
+  const bool tc = use_tc(h, M) && !comm;  // wgmma path, 64 rows per launch (else the mma.sync GEMV, 16 rows per launch)
+  // ---- RMSNorm fusion: the fields of b2_gemm_fuse that are set name one of two forms, each checked here once; every other
+  //      combination is B2_ERR_UNSUPPORTED.
+  //        self-contained: norm_gamma alone, on the mma.sync GEMV (M <= 16)
+  //        hand-off, on the wgmma path: consumer norm_sumsq (no norm_gamma) and / or producer xg_out + sumsq_out + gamma_out
+  bool norm_self = false, handoff = false;
+  if (fuse) {
     const bool cons = fuse->norm_sumsq != nullptr, prod = fuse->xg_out != nullptr;
-    if (norm_self || (cons && fuse->norm_gamma) || (fuse->sumsq_out && !prod)) return B2_ERR_UNSUPPORTED;
-    if (cons && (fuse->norm_parts <= 0 || fuse->norm_hidden <= 0)) return B2_ERR_PARAM;
-    if (prod) {
-      if (!fuse->sumsq_out || !fuse->gamma_out || h->pair || activation != B2_ACT_NONE) return B2_ERR_PARAM;
-      // the statistics come out of the vectorised residual epilogue: 8-byte aligned rows everywhere
-      if ((h->d.N & 3) || (ldc & 3) || (fuse->ldxg & 3) || (reinterpret_cast<uintptr_t>(C) & 7) ||
-          (reinterpret_cast<uintptr_t>(fuse->xg_out) & 7) || (reinterpret_cast<uintptr_t>(fuse->gamma_out) & 7) ||
-          (residual && (reinterpret_cast<uintptr_t>(residual) & 7)) || (bias && (reinterpret_cast<uintptr_t>(bias) & 7)))
-        return B2_ERR_UNSUPPORTED;
+    norm_self = fuse->norm_gamma && !cons;
+    handoff = cons || prod || fuse->sumsq_out;
+    if (norm_self) {
+      if (tc || M > kGemvMaxM || handoff) return B2_ERR_UNSUPPORTED;
+      if (fuse->norm_hidden != h->d.K) return B2_ERR_PARAM;  // the row statistics span exactly this GEMM's K
+      if (reinterpret_cast<uintptr_t>(fuse->norm_gamma) & 15) return B2_ERR_UNSUPPORTED;  // bulk-copied by slices
+    } else if (handoff) {
+      if (!tc || fuse->norm_gamma || (fuse->sumsq_out && !prod)) return B2_ERR_UNSUPPORTED;
+      if (cons && (fuse->norm_parts <= 0 || fuse->norm_hidden <= 0)) return B2_ERR_PARAM;
+      if (prod) {
+        if (!fuse->sumsq_out || !fuse->gamma_out || h->pair || activation != B2_ACT_NONE) return B2_ERR_PARAM;
+        // the statistics come out of the vectorised residual epilogue: 8-byte aligned rows everywhere
+        if ((h->d.N & 3) || (ldc & 3) || (fuse->ldxg & 3) || (reinterpret_cast<uintptr_t>(C) & 7) ||
+            (reinterpret_cast<uintptr_t>(fuse->xg_out) & 7) || (reinterpret_cast<uintptr_t>(fuse->gamma_out) & 7) ||
+            (residual && (reinterpret_cast<uintptr_t>(residual) & 7)) || (bias && (reinterpret_cast<uintptr_t>(bias) & 7)))
+          return B2_ERR_UNSUPPORTED;
+      }
     }
-  } else {
-    if (norm_self && (fuse->norm_hidden != h->d.K || comm)) return B2_ERR_PARAM;  // the row statistics span exactly this GEMM's K
-    if (norm_self && (reinterpret_cast<uintptr_t>(fuse->norm_gamma) & 15)) return B2_ERR_UNSUPPORTED;  // bulk-copied by slices
-    if (fused && (M > 16 || (h->pair && fuse->sumsq_out) || fuse->xg_out)) return B2_ERR_UNSUPPORTED;
-    if (fuse && fuse->norm_sumsq && (!fuse->norm_gamma || fuse->norm_parts <= 0 || fuse->norm_hidden <= 0)) return B2_ERR_PARAM;
   }
   if (!h->packed) return B2_ERR_RUNTIME;
   if (M > h->d.max_m) return B2_ERR_LIMIT;
@@ -1238,7 +1202,7 @@ static int run_impl(b2_gemm_wq_t h, const void* A, int64_t lda, void* C, int64_t
   if (workspace_bytes < b2_gemm_wq_workspace_bytes(h, M)) return B2_ERR_PARAM;
   cudaStream_t stream = (cudaStream_t)stream_;
   const bool grouped = h->group_tiles > 0;
-  if (use_tc(h, M) && !comm) {  // decode batches 17..: wgmma path, 64 rows per launch
+  if (tc) {
     TcParams p;
     p.A = (const __nv_bfloat16*)A; p.lda = lda;
     p.C = (__nv_bfloat16*)C; p.ldc = ldc;
@@ -1248,7 +1212,7 @@ static int run_impl(b2_gemm_wq_t h, const void* A, int64_t lda, void* C, int64_t
     p.act = activation; p.alpha = alpha;
     p.group_tiles = h->group_tiles;
     p.group_k = h->group_k; p.ngroups = h->G;
-    if (fused) {
+    if (handoff) {
       p.norm_ld = M;
       if (fuse->norm_sumsq) {
         p.norm_sumsq = fuse->norm_sumsq; p.norm_parts = fuse->norm_parts;
@@ -1264,7 +1228,7 @@ static int run_impl(b2_gemm_wq_t h, const void* A, int64_t lda, void* C, int64_t
   }
   // ---- dense bf16 weights at batches <= 16: no global split-K (wq_gemv2.cu), unless a fusion only the split-K kernel
   //      implements is asked for (fp16 handles: the split-K kernel)
-  if (h->d.wbits == 16 && M <= kGemvMaxM && !fused && !comm && h->d.ft == B2_DT_BF16) {
+  if (h->d.wbits == 16 && M <= kGemvMaxM && !norm_self && !comm && h->d.ft == B2_DT_BF16) {
     Gemv2Params p;
     p.packed = (const uint8_t*)h->packed;
     p.A = (const __nv_bfloat16*)A; p.lda = lda;
@@ -1307,14 +1271,11 @@ static int run_impl(b2_gemm_wq_t h, const void* A, int64_t lda, void* C, int64_t
     p.nst_log2 = pl.nst_log2;
     p.act = activation;
     p.alpha = alpha;
-    p.norm_sumsq = fuse ? fuse->norm_sumsq : nullptr;
-    p.norm_gamma = fuse ? (const __nv_bfloat16*)fuse->norm_gamma : nullptr;
-    p.norm_parts = fuse ? fuse->norm_parts : 0;
-    p.norm_self = norm_self ? 1 : 0;
     p.cluster = pl.cluster ? 1 : 0;
-    p.norm_inv_hidden = fuse && fuse->norm_hidden > 0 ? 1.0f / (float)fuse->norm_hidden : 0.f;
-    p.norm_eps = fuse ? fuse->norm_eps : 0.f;
-    p.sumsq_out = fuse ? fuse->sumsq_out : nullptr;
+    p.norm_self = norm_self ? 1 : 0;
+    p.norm_gamma = norm_self ? (const __nv_bfloat16*)fuse->norm_gamma : nullptr;
+    p.norm_inv_hidden = norm_self ? 1.0f / (float)fuse->norm_hidden : 0.f;
+    p.norm_eps = norm_self ? fuse->norm_eps : 0.f;
     p.comm_on = comm ? 1 : 0;
     if (comm) p.comm = *comm;
     else memset(&p.comm, 0, sizeof(p.comm));

@@ -122,7 +122,7 @@ class _RefView:
 
 class DecodeStack:
     def __init__(self, cfg, batch, max_len, wbits=4, group=-1, kv="none", span=128, seed=1234, device="cuda",
-                 keep_ref=False, layers=None, tp_rank=0, tp_size=1, tp_group=None, fuse_swiglu=True, fuse_norm=False,
+                 keep_ref=False, layers=None, tp_rank=0, tp_size=1, tp_group=None, fuse_swiglu=True,
                  collective=None, comm=None, dtype=torch.bfloat16, q_len=1, tree=False):
         """tp_size > 1: the reference's tensor-parallel layout (QKV/gate/up column split, o/down row split + all-reduce,
         vocab-split lm_head + B-element all-gather); every rank builds the SAME full synthetic weights from `seed` and
@@ -219,26 +219,7 @@ class DecodeStack:
             self.all_val = torch.empty(tp, batch, dtype=torch.float32, device=device)
         self.graph = None
         self.set_batch(batch)
-        # RMSNorm fusion (decode batches <= 16, TP = 1): the row-parallel GEMVs emit per-tile sums of squares, their
-        # consumers normalise while staging activations; only layer 0's first norm stays a stand-alone kernel.
-        # Off by default: it removes 2 launches/layer but lengthens every GEMV's dependent chain (statistics load + barrier
-        # before staging).
-        self.fuse_norm = fuse_norm and tp == 1 and rows <= 16
-        if self.fuse_norm:
-            self.ssq_o = torch.zeros(self.layers[0]["o"].op.sumsq_parts(), rows, dtype=torch.float32, device=device)
-            self.ssq_d = torch.zeros(self.layers[0]["down"].op.sumsq_parts(), rows, dtype=torch.float32, device=device)
-        # Self-contained RMSNorm fusion (any TP): the column-parallel GEMVs (qkv, gate/up) stage bf16(x * gamma), collect
-        # sum x^2 in the same pass and scale their reduced tile by 1/rms — two launches per layer disappear.  Every CTA
-        # repeats the normalisation of its k-slice of every live row, so the saving shrinks with the batch.  Default: batches <= 2.
-        self.norm_self = (os.environ.get("B2_NORM_SELF", "1") != "0" and not self.fuse_norm
-                          and (group == -1 or group % 64 == 0))  # other group sizes run on the wgmma kernel at every batch
-        self.norm_self_max_b = int(os.environ.get("B2_NORM_SELF_MAX_B", "2"))
-        # RMSNorm hand-off between the wgmma GEMMs (batches >= 17, TP = 1): o_proj / down_proj also write the next
-        # norm's input scaled by its gamma plus per-tile row statistics; qkv / gate+up / lm_head scale their result rows by
-        # 1/rms.  Only layer 0's first norm stays a stand-alone kernel (2 launches per layer fewer).
-        self.norm_handoff = (os.environ.get("B2_NORM_HANDOFF", "1") != "0" and tp == 1 and not self.fuse_norm
-                             and (group == -1 or wbits == 4))
-        if self.norm_handoff and rows >= 17:
+        if self._norm_placement(rows) == "handoff":  # per-tile row statistics of o_proj / down_proj, [tiles][R] per step
             self._ssq_o = torch.zeros(self.layers[0]["o"].op.sumsq_parts() * rows, dtype=torch.float32, device=device)
             self._ssq_d = torch.zeros(self.layers[0]["down"].op.sumsq_parts() * rows, dtype=torch.float32, device=device)
         self.launches_per_step = 0
@@ -258,7 +239,6 @@ class DecodeStack:
         if self.tree:
             self.parents, self.path = self._parents[:b], self._path[:b]
         self.graph = None
-        assert not getattr(self, "fuse_norm", False) or b == self.Bmax, "the fused-norm statistics are laid out for one batch"
 
     # ------------------------------------------------------------------ cache fill
     def set_context(self, ctx, seed=4321):
@@ -320,15 +300,31 @@ class DecodeStack:
         else:
             self.comm.allreduce(t, out=out if out is not None else t)
 
+    def _norm_placement(self, R):
+        """Where a step of R activation rows runs its RMSNorms.
+        "self": qkv and gate/up normalise their own input (b2_gemm_fuse, self-contained form): they stage bf16(x * gamma),
+          collect sum x^2 in the same pass and scale their reduced tile by 1/rms, so two launches per layer disappear.
+          Every CTA repeats the normalisation of its k-slice of every live row, so it pays at R <= 2 only.  It needs the
+          mma.sync GEMV at R rows, which group sizes that are not a multiple of 64 never take.
+        "handoff": o_proj / down_proj also write the next norm's input scaled by its gamma plus per-tile row statistics;
+          qkv, gate/up and lm_head take that input and scale their result rows by 1/rms.  Only layer 0's first norm stays
+          a stand-alone kernel (two launches per layer fewer).  It needs the wgmma GEMM (R >= 17; per-channel or int4
+          weights) and a whole hidden state per rank (TP = 1).
+        "standalone": b2_rmsnorm before each consumer, everywhere else (R 3..16, TP > 1 at R >= 17, ...)."""
+        g = self.group_size
+        if R <= 2 and (g == -1 or g % 64 == 0):
+            return "self"
+        if R >= 17 and self.tp == 1 and (g == -1 or self.wbits == 4):
+            return "handoff"
+        return "standalone"
+
     def _step_ops(self):
         cfg, ws = self.cfg, self.ws
         H = cfg.hidden
-        fn = self.fuse_norm
         T = self.q_len
-        R = self.B * T  # activation rows: the fusion thresholds follow them
-        ns = self.norm_self and R <= min(16, self.norm_self_max_b)
-        nh = self.norm_handoff and R >= 17
-        if nh:
+        R = self.B * T  # activation rows
+        norm = self._norm_placement(R)
+        if norm == "handoff":
             ssq_o = self._ssq_o[:self._ssq_o.numel() // self.Bmax * self.B].view(-1, R)
             ssq_d = self._ssq_d[:self._ssq_d.numel() // self.Bmax * self.B].view(-1, R)
         # the step form of append + attention: single token, chain of T tokens, or draft tree
@@ -336,24 +332,19 @@ class DecodeStack:
         n = 0
         ops.embedding(self.embed, self.ids if T == 1 else self.tokens.view(-1), out=self.x); n += 1
         for li, L in enumerate(self.layers):
-            if fn and li > 0:  # x and its row statistics come from the previous layer's down_proj
-                L["qkv"](self.x, ws, out=self.qkv, norm_in=(self.ssq_d, L["g1"], H, cfg.eps)); n += 1
-            elif ns:
+            if norm == "self":
                 L["qkv"](self.x, ws, out=self.qkv, norm_in=(None, L["g1"], H, cfg.eps)); n += 1
-            elif nh and li > 0:  # xn = bf16(x * g1) and the row statistics were written by the previous layer's down_proj
+            elif norm == "handoff" and li > 0:  # xn = bf16(x * g1) and the row statistics were written by the previous layer's down_proj
                 L["qkv"](self.xn, ws, out=self.qkv, norm_in=(ssq_d, None, H, cfg.eps)); n += 1
             else:
                 ops.rmsnorm(self.x, L["g1"], cfg.eps, out=self.xn); n += 1
                 L["qkv"](self.xn, ws, out=self.qkv); n += 1
             ops._cache_append(L["cache"], self.qkv, self.lens_old, q_out=self.q, rope=self.rope, **form); n += 1
             self.attn._run(self.q, L["cache"], self.lens_new, self.max_len, ws, out=self.ao, **form); n += 1
-            if fn:
-                L["o"](self.ao, ws, out=self.x, residual=self.x, sumsq_out=self.ssq_o); n += 1
-                mlp_in, nin = self.x, (self.ssq_o, L["g2"], H, cfg.eps)
-            elif ns:
+            if norm == "self":
                 n = self._row_parallel(L["o"], self.ao, n)
                 mlp_in, nin = self.x, (None, L["g2"], H, cfg.eps)
-            elif nh:
+            elif norm == "handoff":
                 L["o"](self.ao, ws, out=self.x, residual=self.x, sumsq_out=ssq_o, xg_out=(self.xn, L["g2"])); n += 1
                 mlp_in, nin = self.xn, (ssq_o, None, H, cfg.eps)
             else:
@@ -366,16 +357,12 @@ class DecodeStack:
                 L["gate"](mlp_in, ws, out=self.gate, act=ACT_SILU, norm_in=nin); n += 1
                 L["up"](mlp_in, ws, out=self.up, norm_in=nin); n += 1
                 ops.binary(self.gate, self.up, BIN_MUL, out=self.gate); n += 1
-            if fn:
-                L["down"](self.gate, ws, out=self.x, residual=self.x, sumsq_out=self.ssq_d); n += 1
-            elif nh:
+            if norm == "handoff":
                 g_next = self.layers[li + 1]["g1"] if li + 1 < len(self.layers) else self.gf
                 L["down"](self.gate, ws, out=self.x, residual=self.x, sumsq_out=ssq_d, xg_out=(self.xn, g_next)); n += 1
             else:
                 n = self._row_parallel(L["down"], self.gate, n)
-        if fn:
-            self.lm_head(self.x, ws, out=self.logits, norm_in=(self.ssq_d, self.gf, H, cfg.eps)); n += 1
-        elif nh:
+        if norm == "handoff":
             self.lm_head(self.xn, ws, out=self.logits, norm_in=(ssq_d, None, H, cfg.eps)); n += 1
         else:
             ops.rmsnorm(self.x, self.gf, cfg.eps, out=self.xn); n += 1

@@ -86,9 +86,12 @@ class GemmWQ:
         return lib.b2_gemm_wq_sumsq_parts(self.h)
 
     def __call__(self, a, ws, out=None, act=ACT_NONE, alpha=1.0, residual=None, norm_in=None, sumsq_out=None, xg_out=None):
-        """norm_in = (sumsq [parts, M] fp32 or None, gamma [K] bf16, hidden, eps): fused RMSNorm prologue;
-        sumsq_out [sumsq_parts(), M] fp32: per-tile row sums of squares of the output (for the next op's norm_in).
-        Batches >= 17: norm_in = (sumsq, None, hidden, eps) with `a` = the producer's xg_out (already scaled by gamma)."""
+        """Fused RMSNorm (b2_gemm_fuse), two forms:
+        M <= 16, self-contained: norm_in = (None, gamma [K], K, eps) — the GEMV normalises its own activations.
+        M >= 17, hand-off on the wgmma path: the producer (o_proj / down_proj with residual) takes
+        sumsq_out [sumsq_parts(), M] fp32 and xg_out = (xg [M, N], gamma_out [N]) and also writes xg = FT(out * gamma_out)
+        and per-tile row sums of squares; the consumer takes a = xg and norm_in = (sumsq, None, hidden, eps).
+        Any other combination fails with B2_ERR_UNSUPPORTED."""
         if self.pair:
             act = _lib.ACT_SWIGLU
         M = a.numel() // a.shape[-1]

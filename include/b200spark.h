@@ -115,31 +115,28 @@ size_t b2_gemm_wq_workspace_bytes(b2_gemm_wq_t handle, int M);
 int b2_gemm_wq_run(b2_gemm_wq_t handle, const void* A, int64_t lda, void* C, int64_t ldc, int M,
                    const void* bias, const void* residual, int activation, float alpha,
                    void* workspace, size_t workspace_bytes, void* stream);
-/* RMSNorm fusion around the GEMV (decode batches <= 16; "next" row f2 of SURVEY.md §8): the producer of a hidden
- * state (o_proj / down_proj with residual) also emits, per 128-channel tile, the sum of squares of each output row
- * (sumsq_out [tiles][M], tiles = b2_gemm_wq_sumsq_parts); the consumer applies LayerNormNoBeta on the fly while staging
- * its activations: a_norm[m,k] = A[m,k] * rsqrt(sum_p norm_sumsq[p][m] / norm_hidden + eps) * gamma[k], rounded to FT
- * exactly like the stand-alone b2_rmsnorm.  Either half may be NULL.  These two forms exist for M <= 16 (B2_ERR_UNSUPPORTED
- * above; batches >= 17 have the hand-off form described with the struct).
- * Self-contained form (norm_sumsq == NULL, norm_gamma != NULL, norm_hidden == K): the consumer needs nothing from its
- * producer — it stages bf16(A[m,k] * gamma[k]), collects sum_k A[m,k]^2 over its own k-slice in the same pass (the split-K
- * reducer adds the slices), and multiplies the reduced fp32 tile by rsqrt(sum / K + eps) before alpha / bias / activation:
+/* RMSNorm fusion ("next" row f2 of SURVEY.md §8), two forms named by the fields that are set; any other combination
+ * (norm_sumsq with norm_gamma, sumsq_out without xg_out, a form on the other kernel's batches) is B2_ERR_UNSUPPORTED.
+ * Self-contained form, batches <= 16 (norm_gamma only, norm_hidden == K): the GEMV needs nothing from its producer — it
+ * stages bf16(A[m,k] * gamma[k]), collects sum_k A[m,k]^2 over its own k-slice in the same pass (the split-K reducer adds
+ * the slices), and multiplies the reduced fp32 tile by rsqrt(sum / K + eps) before alpha / bias / activation:
  *   C = act(alpha * inv_rms[m] * sum_k bf16(A[m,k] gamma[k]) W[k,n] + bias)   — one bf16 rounding per activation, like the
  * stand-alone norm, at a different point of the product.  Every CTA repeats the normalisation of its k-slice of every live
- * row, so it pays at tiny batches only: the decode stack uses it at batches <= 2 (FT(x) stands for bf16 or fp16). */
+ * row, so it pays at tiny batches only: the decode stack uses it at batches <= 2 (FT(x) stands for bf16 or fp16).
+ * Hand-off form, batches >= 17 (int4 group sizes that are not a multiple of 64: every batch): see the struct. */
 typedef struct {
-  const float* norm_sumsq; /* [norm_parts][M] or NULL */
-  const void* norm_gamma;  /* [K] FT */
+  const float* norm_sumsq; /* hand-off consumer: [norm_parts][M], or NULL */
+  const void* norm_gamma;  /* self-contained form: [K] FT, or NULL */
   int32_t norm_parts;
   int32_t norm_hidden;
   float norm_eps;
   int32_t reserved;
-  float* sumsq_out;        /* [b2_gemm_wq_sumsq_parts(handle)][M] or NULL */
-  /* Batches >= 17 (wgmma path): the hand-off form.  The producer (o_proj / down_proj with residual) writes, besides C and
-   * sumsq_out, xg_out[m, n] = FT(C[m, n] * gamma_out[n]) — the next RMSNorm's input already scaled by its gamma; the consumer
-   * is called with A = xg, norm_sumsq = the producer's sumsq_out, norm_gamma = NULL, and multiplies its fp32 result rows by
-   * rsqrt(sum_p norm_sumsq[p][m] / norm_hidden + eps) (the factor is linear in the row).  Two RMSNorm launches per layer
-   * disappear; the statistics are taken from the values as stored (FT), like the stand-alone norm reads them. */
+  float* sumsq_out;        /* hand-off producer: [b2_gemm_wq_sumsq_parts(handle)][M], or NULL */
+  /* Hand-off form (wgmma path).  The producer (o_proj / down_proj with residual) writes, besides C, per-tile row sums of
+   * squares (sumsq_out) and xg_out[m, n] = FT(C[m, n] * gamma_out[n]) — the next RMSNorm's input already scaled by its gamma;
+   * the consumer (A = xg, norm_sumsq = the producer's sumsq_out, norm_gamma = NULL) multiplies its fp32 result rows by
+   * rsqrt(sum_p norm_sumsq[p][m] / norm_hidden + eps).  A call may be both.  Two RMSNorm launches per layer disappear; the
+   * statistics are taken from the values as stored (FT), like the stand-alone norm reads them. */
   void* xg_out;            /* [M, ldxg] FT or NULL (requires sumsq_out and gamma_out) */
   const void* gamma_out;   /* [N] FT */
   int64_t ldxg;
