@@ -23,6 +23,7 @@
 //   * the 16-bit type of activations / outputs / scales is a template parameter (Ft<H>: bf16 or fp16; fp16 uses 128 + q).
 //
 // Roofline: HBM-bound; algorithmic bytes/launch = K*N*wbits/8 + 4*G*N + 2*M*(K+N).
+#include <algorithm>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -774,7 +775,7 @@ struct b2_gemm_wq {
   bool own_sz = false;
   unsigned* counters = nullptr;
   Plan plans[2];  // MT = 1, 2
-  int tc_S = 0;   // split-K of the wgmma path (0 = not planned)
+  int tc_grid = 0, tc_rounds = 0, tc_S = 1, tc_h = 0;  // schedule of the wgmma path (TcSched; tc_grid 0 = not planned)
   bool pair = false;  // gate/up pair image (SwiGLU epilogue): physical channels = 2 * N
   int device = 0;
 };
@@ -1034,31 +1035,46 @@ static bool use_tc(const b2_gemm_wq* h, int M) {
   return M >= kTcMinM && (h->group_tiles == 0 || h->d.wbits == 4);
 }
 
+// The wgmma path's schedule (TcSched), once per handle.  At most as many n-groups as SMs: S = min(SMs / n-groups, KT / 4,
+// B2_GEMM_TC_MAX_SPLIT) equal k-slices per n-group, one CTA each (B2_GEMM_TC_PERSIST=0: also above that, S = 1).  More
+// n-groups than SMs: one CTA per SM, whole n-groups in rounds, and the NR left over each cut in two at a multiple of 4 k-tiles
+// near KT / 2, a head on CTA b < NR and a tail on CTA NR + b: the gate+up pair's 296 n-groups (132 SMs) run 2 rounds plus
+// 28 tiles on 64 CTAs instead of 3 rounds on 32.  The tail continues the head's accumulator chain, so the results are those
+// of whole n-groups bit for bit.  B2_GEMM_TC_MAX_SPLIT=1 splits no n-group.
 static void make_tc_plan(b2_gemm_wq* h) {
-  if (h->tc_S > 0) return;
-  const int ctas = env_int("B2_GEMM_TC_CTAS_PER_SM", 1);
-  auto split_for = [&](int slots, int smax) {
-    int S = slots / h->NG;
-    if (S > h->KT / 4) S = h->KT / 4;
-    if (S > smax) S = smax;
-    return S < 1 ? 1 : S;
-  };
-  h->tc_S = split_for(ctas * sm_count(), env_int("B2_GEMM_TC_MAX_SPLIT", 6));
+  if (h->tc_grid > 0) return;
+  const int sms = sm_count(), NG = h->NG, KT = h->KT;
+  const int smax = std::max(1, env_int("B2_GEMM_TC_MAX_SPLIT", 6));
+  if (NG <= sms || !env_int("B2_GEMM_TC_PERSIST", 1)) {
+    h->tc_S = std::max(1, std::min({sms / NG, KT / 4, smax}));
+    h->tc_grid = NG * h->tc_S;
+    h->tc_rounds = 0;
+    h->tc_h = 0;
+    return;
+  }
+  const int NR = NG % sms;
+  h->tc_S = 1;
+  h->tc_grid = sms;
+  h->tc_rounds = NG / sms;
+  h->tc_h = (NR > 0 && smax > 1 && 2 * NR <= sms) ? KT / 2 / 4 * 4 : 0;
 }
 
-// workspace of the wgmma path: the split-K partial tiles of one launch (kTcMaxM rows)
+// workspace of the wgmma path: the k-slices' partial tiles, or the parked heads, of one launch (kTcMaxM rows)
 static size_t tc_workspace_bytes(b2_gemm_wq* h) {
   make_tc_plan(h);
-  return h->tc_S <= 1 ? 16 : (size_t)h->NG * h->tc_S * kTcMaxM * kBN * sizeof(float) + 16;
+  if (h->tc_S > 1) return (size_t)h->NG * h->tc_S * kTcMaxM * kBN * sizeof(float) + 16;
+  if (h->tc_h > 0) return (size_t)(h->NG - h->tc_rounds * h->tc_grid) * kTcCarryFloats * sizeof(float) + 16;
+  return 16;
 }
 
 // The wgmma kernel over M rows, kTcMaxM per launch.  p holds the caller's operands for row 0 (A, C, residual and the per-row
 // fp8 / RMSNorm arrays, offset here for every launch); the image, its params and the split-K plan come from the handle.
 static int run_tc(b2_gemm_wq* h, TcParams p, int M, cudaStream_t stream) {
   make_tc_plan(h);
-  if (h->tc_S > 1 && !p.ws) return B2_ERR_PARAM;
+  if ((h->tc_S > 1 || h->tc_h > 0) && !p.ws) return B2_ERR_PARAM;
   p.packed = (const uint8_t*)h->packed; p.sz = h->sz; p.counters = h->counters;
-  p.N = h->d.N; p.K = h->d.K; p.Np = h->Np; p.KT = h->KT; p.NG = h->NG; p.S = h->tc_S;
+  p.N = h->d.N; p.K = h->d.K; p.Np = h->Np; p.KT = h->KT; p.NG = h->NG;
+  p.grid = h->tc_grid; p.rounds = h->tc_rounds; p.S = h->tc_S; p.h = h->tc_h;
   const int64_t a_row = p.a_scale ? p.lda : 2 * p.lda;  // bytes per activation row (fp8: lda counts bytes)
   for (int m0 = 0; m0 < M; m0 += kTcMaxM) {
     TcParams q = p;

@@ -60,9 +60,10 @@ struct TcParams {
   int64_t ldc;
   const __nv_bfloat16* bias;
   const __nv_bfloat16* residual;
-  float* ws;
+  float* ws;              // [NG][S] partial tiles of the k-slices, or [NR][kTcCarryFloats] parked heads (TcSched)
   unsigned* counters;
-  int M, N, K, Np, KT, NG, S;
+  int M, N, K, Np, KT, NG;
+  int grid, rounds, S, h;  // the work schedule (TcSched)
   int act;
   float alpha;
   // fp8 activations (A8 instantiation): A is fp8-e4m3 in the b2 fp8 activation layout (lda in bytes), per-token scale [M] and
@@ -83,6 +84,39 @@ struct TcParams {
   int group_tiles = 0;    // > 0: sub-channel weights (GROUPED instantiation), k-tiles per quantization group; sz is [G][Np]
   int group_k = 0, ngroups = 1;  // group_k > 0: a group size that is no multiple of 64 (a multiple of 8, >= 32): 8 consecutive
                                  // k — one word of the image — never straddle a group, so the params are looked up per word
+};
+
+// The wgmma kernel's work schedule (planned by make_tc_plan, walked by wq_gemm_tc_kernel).  While there are at most as many
+// n-groups as CTAs, CTA b takes k-slice b % S of n-group b / S (S equal slices; the last slice to arrive sums the partials in
+// slice order).  Otherwise each of the grid CTAs takes `rounds` whole n-groups, b + j * grid, and each of the NR = NG - nfull
+// n-groups left over is cut in two at k-tile h: CTA b < NR runs the head [0, h) of n-group nfull + b first and parks its
+// raw accumulators; CTA NR + b runs the tail [h, KT) last, starting from them, so every output is the one k-ordered fp32
+// chain of a whole n-group, bit for bit.  A tail that starts before its head has parked runs the whole n-group instead: no
+// CTA waits for another.  h = 0: CTA b < NR runs leftover n-group nfull + b whole.
+struct TcSeg {
+  int ng, kt0, kt1;  // k-tiles [kt0, kt1) of n-group ng
+  int part, parts;   // k-slice `part` of `parts` (parts == 1: the CTA finishes the n-group)
+  int carry;         // 1: head (parks its accumulators), 2: tail (starts from them if they are there)
+};
+constexpr int kTcCarryFloats = 256 * 32 + 64 * 4;  // a parked head: 32 accumulators per consumer thread, 4 row sums per row
+struct TcSched {
+  int NG, KT, grid, rounds, S, h, b, nfull, NR;
+  __host__ __device__ TcSched(int NG_, int KT_, int grid_, int rounds_, int S_, int h_, int b_)
+      : NG(NG_), KT(KT_), grid(grid_), rounds(rounds_), S(S_), h(h_), b(b_), nfull(rounds_ * grid_), NR(NG_ - rounds_ * grid_) {}
+  __host__ __device__ int count() const {
+    return rounds == 0 ? 1 : rounds + (b < NR ? 1 : 0) + (h > 0 && b >= NR && b < 2 * NR ? 1 : 0);
+  }
+  __host__ __device__ TcSeg seg(int i) const {
+    if (rounds == 0) {
+      const int ng = b / S, s = b - ng * S;
+      return TcSeg{ng, s * KT / S, (s + 1) * KT / S, s, S, 0};
+    }
+    const int head = b < NR ? 1 : 0;
+    if (head && i == 0) return TcSeg{nfull + b, 0, h > 0 ? h : KT, 0, 1, h > 0 ? 1 : 0};
+    const int j = i - head;
+    if (j < rounds) return TcSeg{j * grid + b, 0, KT, 0, 1, 0};
+    return TcSeg{nfull + b - NR, h, KT, 0, 1, 2};
+  }
 };
 
 // GEMV for dense bf16 weights without global split-K (wq_gemv2.cu)

@@ -21,9 +21,11 @@
 //   epilogue    : the consumers apply s * (acc - (16+z) * sum a) to their accumulators and park the fp32 tile in the drained
 //                 activation ring; then ALL 384 threads do the split-K partial store / last-CTA reduction and the final
 //                 alpha/bias/activation/residual (or SwiGLU) with 16-byte reads and 8-byte bf16x4 stores.
-//   persistent  : when there are more (n-group, k-split) units than SMs (gate+up pair, lm_head) one CTA per SM walks
-//                 several units; barriers and ring phases carry over and the next unit's first weight stages are issued
-//                 before the epilogue (MULTI instantiation).
+//   schedule    : one CTA per SM; the launch's tiles are spread evenly over them (TcSched, wq_gemm_shared.cuh): whole
+//                 n-groups in rounds while there are more n-groups than CTAs (MULTI instantiation: gate+up pair, lm_head),
+//                 each n-group left over cut in two k-ordered halves on two CTAs, the second starting from the first's
+//                 accumulators; else equal k-slices.  A CTA walks its segments with the barriers and ring phases carried
+//                 over; the next segment's first weight stages are issued before the epilogue.
 //
 //   variants    : GROUPED (sub-channel int4: the scale is applied to the weights at dequantization; group sizes that do not
 //                 divide the 64-k tile look their params up per 8-k word), A8 (fp8 activations, e4m3 wgmma), H (fp16
@@ -130,7 +132,7 @@ __device__ __forceinline__ uint32_t nib4_to_e4m3(uint32_t w_rot3, uint32_t qsh, 
   return r;
 }
 
-// MULTI: a CTA walks several units (more units than SMs); the single-unit instantiation folds the unit loop away
+// MULTI: more n-groups than CTAs, a CTA walks whole n-groups and at most one head and one tail; else one k-slice
 // A8: fp8-e4m3 activations (b2_gemm_wq_run_fp8, int4 weights only): the int4 codes become exact e4m3 bytes, the MMAs are
 // e4m3 x e4m3 with K = 32 (half the MMAs of the bf16 path), an activation tile is 128 k wide.
 // GROUPED: sub-channel weights (GPTQ g128 ...): the (scale, zero) of a channel changes every group_tiles k-tiles, so the affine
@@ -170,7 +172,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) wq_gemm_tc_kernel(const TcParam
   __shared__ int s_is_last;
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int nunits = p.NG * p.S;
+  const TcSched sch(p.NG, p.KT, (int)gridDim.x, p.rounds, p.S, p.h, (int)blockIdx.x);
+  const int nseg = MULTI ? sch.count() : 1;  // MULTI: whole n-groups, a head first / a tail last; else one k-slice
+  auto segment = [&](int i) { return sch.seg(i); };
+  __shared__ unsigned s_carry;
 
   if (tid == 0) {
     for (int i = 0; i < NSW; ++i) { mbar_init(&wfull[i], 1); mbar_init(&wfree[i], 8); }
@@ -180,24 +185,35 @@ __global__ void __launch_bounds__(kTcThreads, 1) wq_gemm_tc_kernel(const TcParam
   __syncthreads();
   pdl_launch_dependents();
 
-  // Persistent over work units (n-group, k-split): unit = blockIdx.x, += gridDim.x.  Barriers and the ring phases carry over;
-  // g = gbase + st is the stage index since kernel start.  Stage g uses weight slot g % NSW and X slot g % NSX.
-  int w_pre = 0;  // weight stages of the current unit already issued during the previous unit's tail (producer thread only)
-  const int my_units = !MULTI ? 1 : ((int)blockIdx.x < nunits) ? (nunits - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x : 0;
-  // The MMA width (N32: m64n32 for batches <= 32) is fixed once per launch: the whole unit loop is compiled once per width.
-  // A width chosen inside it would leave two main loops in one unit loop, and ptxas then serializes the MMAs of the
+  // The CTA walks its segments (TcSched).  Barriers and the ring phases carry over; g = gbase + st is the stage index since
+  // kernel start.  Stage g uses weight slot g % NSW and X slot g % NSX.
+  int w_pre = 0;  // weight stages of the current segment already issued during the previous one's tail (producer thread only)
+  // The MMA width (N32: m64n32 for batches <= 32) is fixed once per launch: the whole segment loop is compiled once per width.
+  // A width chosen inside it would leave two main loops in one segment loop, and ptxas then serializes the MMAs of the
   // persistent instantiations for lack of registers.
   auto body = [&](auto n32) {
   constexpr bool N32 = decltype(n32)::value;
-  for (int uit = 0; uit < my_units; ++uit) {
-  const int unit = (int)blockIdx.x + uit * (int)gridDim.x;
-  const int ng = unit / p.S;
-  const int s = unit - ng * p.S;
-  const int kt0 = (int)((int64_t)s * p.KT / p.S), kt1 = (int)((int64_t)(s + 1) * p.KT / p.S);
+  int gbase = 0;  // stages of the earlier segments
+  for (int si = 0; si < nseg; ++si) {
+  const TcSeg sg = segment(si);
+  const int ng = sg.ng, kt1 = sg.kt1;
+  // a tail starts from its head's parked accumulators if they are there (the head's arrival makes the count 1), else it runs
+  // the whole n-group.  Counters and workspace belong to the previous kernels until pdl_wait.
+  bool carry_in = false;
+  if (MULTI && sg.carry == 2) {
+    pdl_wait();
+    if (tid == 0) {
+      s_carry = atomicAdd(&p.counters[ng], 1u);
+      if (s_carry == 1u) p.counters[ng] = 0;  // both have arrived: re-arm for the next launch / graph replay
+      __threadfence();
+    }
+    __syncthreads();
+    carry_in = s_carry == 1u;
+  }
+  const int kt0 = sg.carry == 2 && !carry_in ? 0 : sg.kt0;
+  const float* carry_src = p.ws + (size_t)(ng - sch.nfull) * kTcCarryFloats;
   const int nt = kt1 - kt0;
-  const int nst = (nt + TPS - 1) / TPS;  // pipeline stages of this unit
-  // stages before this unit.  A CTA only walks several units when S == 1, where every unit has the same stage count
-  const int gbase = MULTI ? uit * nst : 0;
+  const int nst = (nt + TPS - 1) / TPS;  // pipeline stages of this segment
   if (warp == 8) {
     // ===================== weight producer (does not wait for the previous kernel) =====================
     if (lane == 0) {
@@ -209,14 +225,12 @@ __global__ void __launch_bounds__(kTcThreads, 1) wq_gemm_tc_kernel(const TcParam
       };
       const uint8_t* wsrc = p.packed + ((size_t)ng * p.KT + kt0) * TILE_BYTES;
       for (int st = w_pre; st < nst; ++st) issue(gbase + st, wsrc + (size_t)st * WSTAGE, min(TPS, nt - st * TPS) * TILE_BYTES);
-      // head of the next unit: its first stages stream in while this unit drains and runs its epilogue
+      // head of the next segment: its first stages stream in while this one drains and runs its epilogue
       w_pre = 0;
-      const int nu = unit + gridDim.x;
-      if (MULTI && nu < nunits) {
-        const int ng2 = nu / p.S, s2 = nu - ng2 * p.S;
-        const int k0 = (int)((int64_t)s2 * p.KT / p.S), k1 = (int)((int64_t)(s2 + 1) * p.KT / p.S);
-        const int nt2 = k1 - k0, nst2 = (nt2 + TPS - 1) / TPS;
-        const uint8_t* wsrc2 = p.packed + ((size_t)ng2 * p.KT + k0) * TILE_BYTES;
+      if (si + 1 < nseg && segment(si + 1).carry != 2) {  // a tail's first k-tile is only known when it starts
+        const TcSeg s2 = segment(si + 1);
+        const int nt2 = s2.kt1 - s2.kt0, nst2 = (nt2 + TPS - 1) / TPS;
+        const uint8_t* wsrc2 = p.packed + ((size_t)s2.ng * p.KT + s2.kt0) * TILE_BYTES;
         w_pre = min(NSW, nst2);
         for (int st = 0; st < w_pre; ++st)
           issue(gbase + nst + st, wsrc2 + (size_t)st * WSTAGE, min(TPS, nt2 - st * TPS) * TILE_BYTES);
@@ -248,6 +262,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) wq_gemm_tc_kernel(const TcParam
     // ===================== row sums of the landed activation tiles (row = xt) =====================
     const int xt = tid - 320;  // 0..63
     float r0 = 0.f, r1 = 0.f, r2 = 0.f, r3 = 0.f;
+    if (carry_in) {
+      const float4 r = __ldcg(reinterpret_cast<const float4*>(carry_src + 256 * 32) + xt);
+      r0 = r.x; r1 = r.y; r2 = r.z; r3 = r.w;
+    }
     if (A8) {  // the quantizer already summed every 64-k tile of every row: add this unit's tiles; stage the token scales
       pdl_wait();
       if (xt < p.M) {
@@ -287,6 +305,8 @@ __global__ void __launch_bounds__(kTcThreads, 1) wq_gemm_tc_kernel(const TcParam
     }
     suma[xt] = (r0 + r1) + (r2 + r3);
     asm volatile("bar.sync 3, 320;" ::: "memory");  // hand the sums to the consumers
+    if (MULTI && sg.carry == 1)  // a head parks its running sums behind the accumulators (the ring is drained now)
+      reinterpret_cast<float4*>(xring)[256 * 32 / 4 + xt] = make_float4(r0, r1, r2, r3);
   } else {
     // ===================== consumers: dequantize into wgmma A fragments, MMA, accumulators -> smem tile =====================
     const int wg = warp >> 2, g8 = lane >> 2, t4 = lane & 3;
@@ -311,6 +331,13 @@ __global__ void __launch_bounds__(kTcThreads, 1) wq_gemm_tc_kernel(const TcParam
     float d[32], dt[32];
 #pragma unroll
     for (int i = 0; i < 32; ++i) d[i] = dt[i] = 0.f;
+    if (carry_in) {
+#pragma unroll
+      for (int i = 0; i < 32; i += 4) {
+        const float4 v = __ldcg(reinterpret_cast<const float4*>(carry_src + tid * 32 + i));
+        d[i] = v.x; d[i + 1] = v.y; d[i + 2] = v.z; d[i + 3] = v.w;
+      }
+    }
     int prev_xs = -1;
     for (int st = 0; st < nst; ++st) {
       const int g = gbase + st;
@@ -454,6 +481,11 @@ __global__ void __launch_bounds__(kTcThreads, 1) wq_gemm_tc_kernel(const TcParam
     // ---------------- accumulators -> fp32 tile in shared memory: [m][128 n] over the drained activation ring ----------------
     asm volatile("bar.sync 3, 320;" ::: "memory");  // row sums ready; every MMA of both warpgroups has completed
     float* fs = reinterpret_cast<float*>(xring);
+    if (MULTI && sg.carry == 1) {  // a head parks its raw accumulators
+#pragma unroll
+      for (int i = 0; i < 32; i += 4)
+        reinterpret_cast<float4*>(fs + tid * 32)[i / 4] = make_float4(d[i], d[i + 1], d[i + 2], d[i + 3]);
+    } else {
 #pragma unroll
     for (int j = 0; j < 8; ++j) {  // n8 block j of the accumulator: batch rows m = 8j + 2t (+1), channels rr0 / rr1
       const int m = 8 * j + 2 * t4;
@@ -465,6 +497,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) wq_gemm_tc_kernel(const TcParam
       fs[(m + 1) * kBN + rr0] = sz0.x * s1 * (d[4 * j + 1] - zz0 * sa1);
       fs[m * kBN + rr1] = sz1.x * s0 * (d[4 * j + 2] - zz1 * sa0);
       fs[(m + 1) * kBN + rr1] = sz1.x * s1 * (d[4 * j + 3] - zz1 * sa1);
+    }
     }
   }
 
@@ -478,33 +511,41 @@ __global__ void __launch_bounds__(kTcThreads, 1) wq_gemm_tc_kernel(const TcParam
     const int units = p.M * (kBN / 4);  // float4 units, index = m * 32 + nq
     constexpr int MPK4 = kTcNM * kBN / 4;
     bool finalize = true;
-    if (p.S > 1) {
-      float4* wsu = reinterpret_cast<float4*>(p.ws) + ((size_t)ng * p.S + s) * MPK4;
+    if (MULTI && sg.carry == 1) {  // a head: accumulators and row sums to the workspace, then count its arrival
+      float4* dst = reinterpret_cast<float4*>(p.ws + (size_t)(ng - sch.nfull) * kTcCarryFloats);
+      for (int i = tid; i < kTcCarryFloats / 4; i += T) dst[i] = fs4[i];
+      __threadfence();
+      __syncthreads();
+      if (tid == 0 && atomicAdd(&p.counters[ng], 1u) == 1u) p.counters[ng] = 0;  // the tail ran whole already: re-arm
+      finalize = false;
+    } else if (sg.parts > 1) {  // k-slice sg.part of sg.parts: partial tile to slot ng * S + part
+      const size_t slots = (size_t)ng * p.S;
+      float4* wsu = reinterpret_cast<float4*>(p.ws) + (slots + sg.part) * MPK4;
       for (int i = tid; i < units; i += T) wsu[i] = fs4[i];
       __threadfence();
       __syncthreads();
       if (tid == 0) {
         const unsigned prev = atomicAdd(&p.counters[ng], 1u);
-        s_is_last = (prev == (unsigned)(p.S - 1));
+        s_is_last = (prev == (unsigned)(sg.parts - 1));
       }
       __syncthreads();
       finalize = s_is_last != 0;
       if (finalize) {
         __threadfence();
-        // fixed-order sum over the S partials (deterministic); 2 units x 8 partials = 16 independent 16-byte loads in
-        // flight per thread, so the reduction is a few L2 round trips
-        const float4* wsg = reinterpret_cast<const float4*>(p.ws) + (size_t)ng * p.S * MPK4;
+        // fixed-order sum over the partials in k order (deterministic, whichever CTA arrives last); 2 units x 8 partials =
+        // 16 independent 16-byte loads in flight per thread, so the reduction is a few L2 round trips
+        const float4* wsg = reinterpret_cast<const float4*>(p.ws) + slots * MPK4;
         for (int i0 = tid; i0 < units; i0 += 2 * T) {
           float4 a[2];
           a[0] = a[1] = make_float4(0.f, 0.f, 0.f, 0.f);
-          for (int s0 = 0; s0 < p.S; s0 += 8) {
+          for (int s0 = 0; s0 < sg.parts; s0 += 8) {
             float4 b[2][8];
 #pragma unroll
             for (int g = 0; g < 2; ++g)
 #pragma unroll
               for (int u = 0; u < 8; ++u) {
                 const int i = i0 + g * T;
-                b[g][u] = (s0 + u < p.S && i < units) ? __ldcg(wsg + (size_t)(s0 + u) * MPK4 + i) : make_float4(0.f, 0.f, 0.f, 0.f);
+                b[g][u] = (s0 + u < sg.parts && i < units) ? __ldcg(wsg + (size_t)(s0 + u) * MPK4 + i) : make_float4(0.f, 0.f, 0.f, 0.f);
               }
 #pragma unroll
             for (int g = 0; g < 2; ++g)
@@ -621,9 +662,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) wq_gemm_tc_kernel(const TcParam
     }
   }
 
-  if (MULTI) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy tile writes before the next unit's TMA writes
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy tile writes before the next segment's TMA writes
   __syncthreads();  // the tile in the X ring is free again
-  }  // unit loop
+  gbase += nst;
+  }  // segment loop
   };
   if (p.nm == 32)
     body(std::true_type{});
@@ -668,11 +710,7 @@ cudaError_t tc_launch(int wbits, bool fp16, TcParams p, cudaStream_t stream) {
           CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
     return cudaErrorInvalidValue;
 
-  // persistent: one CTA per SM walks the (n-group, k-split) units; B2_GEMM_TC_PERSIST=0 launches one CTA per unit
-  static const int persist = env_int("B2_GEMM_TC_PERSIST", 1);
-  const int units = p.NG * p.S;
-  const int cap = sm_count();
-  const int grid = (persist && units > cap) ? cap : units;
+  const int grid = p.grid;
   const bool grouped = p.group_tiles > 0 || p.group_k > 0;
   // instantiations: fp8 activations with int4 weights and bf16 outputs; sub-channel weights with int4 only
   if ((a8 && (wbits != 4 || fp16)) || (grouped && !a8 && wbits != 4)) return cudaErrorNotSupported;
@@ -682,7 +720,7 @@ cudaError_t tc_launch(int wbits, bool fp16, TcParams p, cudaStream_t stream) {
       const cudaError_t e = raise_smem_limit((const void*)kern, (int)smem);
       return e != cudaSuccess ? e : launch(kern, dim3(grid), dim3(kTcThreads), smem, stream, true, p, amap);
     };
-    return with_flag(units > grid, [&](auto MULTI) {
+    return with_flag(p.NG > grid, [&](auto MULTI) {
       if constexpr (W == 4) {
         if (a8) return go(wq_gemm_tc_kernel<4, MULTI, true>);
       }
