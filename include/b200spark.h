@@ -123,7 +123,11 @@ int b2_gemm_wq_run(b2_gemm_wq_t handle, const void* A, int64_t lda, void* C, int
  *   C = act(alpha * inv_rms[m] * sum_k bf16(A[m,k] gamma[k]) W[k,n] + bias)   — one bf16 rounding per activation, like the
  * stand-alone norm, at a different point of the product.  Every CTA repeats the normalisation of its k-slice of every live
  * row, so it pays at tiny batches only: the decode stack uses it at batches <= 2 (FT(x) stands for bf16 or fp16).
- * Hand-off form, batches >= 17 (int4 group sizes that are not a multiple of 64: every batch): see the struct. */
+ * Hand-off form, batches >= 17 (int4 group sizes that are not a multiple of 64: every batch): see the struct.
+ * Range: both forms stage FT(x * gamma) before normalising.  In fp16 a row with max|x * gamma| > 65504 stages inf, where
+ * b2_rmsnorm stays finite; keep fp16 rows below that.  On N(0,1) rows with one channel at 64 sigma, both forms stay inside the
+ * fp64 RMSNorm -> GEMM envelope wherever checked: RMS 2^-16 (the lowest checked) up to 2^12 in bf16, up to that overflow in
+ * fp16 (H100 SXM, tests/test_norm_exact_gpu.py). */
 typedef struct {
   const float* norm_sumsq; /* hand-off consumer: [norm_parts][M], or NULL */
   const void* norm_gamma;  /* self-contained form: [K] FT, or NULL */

@@ -242,8 +242,9 @@ def act_bound(x, y, act):
     ax, ay = np.abs(x), np.abs(y)
     if act in EXACT_ACTS:
         return np.zeros_like(ay)
-    if act in (ACT_SILU, ACT_SIGMOID):      # x / (1 + __expf(-x)), 1 / (1 + __expf(-x)): relative to y
-        return (2 * (3 + 1.2 * ax) + 4) * U24 * ay
+    if act in (ACT_SILU, ACT_SIGMOID):      # x / (1 + __expf(-x)), 1 / (1 + __expf(-x)): relative to y; below
+        E = (2 * (3 + 1.2 * ax) + 4) * U24 * ay  # x = -88.72 (-x log2 e >= 128) __expf(-x) is inf and the result zero
+        return np.where(x < -88.72, np.maximum(E, ay), E)
     if act == ACT_TANH:                     # tanhf
         return 6 * U24 * ay
     if act == ACT_GELU_ERF:                 # x * 0.5 * (1 + erff(x * c)): erff's absolute error and the rounding of x * c
@@ -503,9 +504,10 @@ def gemv2_cb(case, M, sms=H100_SMS, forced=0):
     return cb
 
 
-def launches(case, M, env=None, sms=H100_SMS, a8=False):
+def launches(case, M, env=None, sms=H100_SMS, a8=False, norm_self=False):
     """The kernel launches of one b2_gemm_wq_run call (run_impl / run_tc): a list of dicts with the kernel's name as the
-    profiler shows it, its rows and the facts that select a code path (wgmma: nm, MULTI, tc_S)."""
+    profiler shows it, its rows and the facts that select a code path (wgmma: nm, MULTI, tc_S).  norm_self: the
+    self-contained RMSNorm form, which only the split-K GEMV implements (dense bf16 included)."""
     env = env or {}
     H = "true" if case.ft == "fp16" else "false"
     out = []
@@ -526,7 +528,7 @@ def launches(case, M, env=None, sms=H100_SMS, a8=False):
             out.append(dict(path="tc", kernel=f"wq_gemm_tc_kernel<{case.wbits}, {'true' if multi else 'false'}, false, {G}, {H}>",
                             m0=m0, rows=rows, nm=32 if rows <= 32 else 64, multi=multi, S=S))
         return out
-    if case.wbits == 16 and case.ft == "bf16" and M <= GEMV_MAX_M and env.get("B2_GEMV2", "1") != "0":
+    if case.wbits == 16 and case.ft == "bf16" and M <= GEMV_MAX_M and not norm_self and env.get("B2_GEMV2", "1") != "0":
         cb = gemv2_cb(case, M, sms, int(env.get("B2_GEMV2_CB", 0)))
         if cb is not None:
             return [dict(path="gemv2", kernel=f"wq_gemv2_kernel<{1 if M <= 8 else 2}>", m0=0, rows=M, cb=cb)]
