@@ -302,6 +302,27 @@ struct Ft<true> {
   }
 };
 
+// ---- per-head RMSNorm of one 128-wide head row held 4 consecutive values per lane (QKLayerNormNoBeta; the stand-alone
+// b2_qk_rmsnorm and the fused form of the span-cache append both call this, so they cannot drift apart):
+//   ss = the lane's 4 squares summed in order, then an xor butterfly over 16, 8, 4, 2, 1 (a fixed order: deterministic);
+//   rs = rsqrtf(ss * (1/128) + eps);  x[i] <- FT((x[i] * rs) * gamma[4 lane + i]), one FT rounding (returned widened).
+// The squares of 16-bit values are exact in fp32.  gamma: 128 FT values, 8-byte aligned; a lane reads its own 4 only.
+template <bool H>
+__device__ __forceinline__ void head_rmsnorm(float (&x)[4], const __nv_bfloat16* gamma, float eps, int lane) {
+  using F = Ft<H>;
+  float ss = x[0] * x[0];
+  ss += x[1] * x[1];
+  ss += x[2] * x[2];
+  ss += x[3] * x[3];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
+  const float rs = rsqrtf(ss * (1.f / 128.f) + eps);
+  const uint2 g = *reinterpret_cast<const uint2*>(gamma + lane * 4);
+  const float gv[4] = {F::lo(g.x), F::hi(g.x), F::lo(g.y), F::hi(g.y)};
+#pragma unroll
+  for (int i = 0; i < 4; ++i) x[i] = F::to_f(F::from_f((x[i] * rs) * gv[i]));
+}
+
 template <int ACT>
 __device__ __forceinline__ float apply_act(float x) {
   // csrc/core/kernel/cuda/hie/cuda_activation.hpp (reference formulas, fp32)

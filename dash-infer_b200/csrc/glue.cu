@@ -181,6 +181,32 @@ __global__ void __launch_bounds__(128) rotary_kernel(__nv_bfloat16* __restrict__
   *reinterpret_cast<uint2*>(ptr) = make_uint2(pack_bf16x2(x[0], x[1]), pack_bf16x2(x[2], x[3]));
 }
 
+// QKLayerNormNoBeta (b2_qk_rmsnorm): one warp per (row, head) of x [rows, ld]; heads [0, n_heads) normalised with q_gamma,
+// [n_heads, n_heads + n_groups) with k_gamma (head_rmsnorm), the V heads copied unless y == x
+template <bool H>
+__global__ void __launch_bounds__(128) qk_rmsnorm_kernel(__nv_bfloat16* y, const __nv_bfloat16* x, int64_t ld, int64_t warps,
+                                                         int n_heads, int n_groups, const __nv_bfloat16* q_gamma,
+                                                         const __nv_bfloat16* k_gamma, float eps) {
+  using F = Ft<H>;
+  pdl_wait();
+  pdl_launch_dependents();
+  const int lane = threadIdx.x & 31;
+  const int slots = n_heads + 2 * n_groups;
+  const int64_t wid = (int64_t)blockIdx.x * 4 + (threadIdx.x >> 5);
+  if (wid >= warps) return;
+  const int64_t row = wid / slots;
+  const int h = (int)(wid - row * slots);
+  const size_t off = (size_t)row * ld + (size_t)h * 128 + lane * 4;
+  const uint2 raw = *reinterpret_cast<const uint2*>(x + off);
+  if (h >= n_heads + n_groups) {
+    if (y != x) *reinterpret_cast<uint2*>(y + off) = raw;
+    return;
+  }
+  float v[4] = {F::lo(raw.x), F::hi(raw.x), F::lo(raw.y), F::hi(raw.y)};
+  head_rmsnorm<H>(v, h < n_heads ? q_gamma : k_gamma, eps, lane);
+  *reinterpret_cast<uint2*>(y + off) = make_uint2(F::pack(v[0], v[1]), F::pack(v[2], v[3]));
+}
+
 template <bool H>
 __global__ void __launch_bounds__(256) binary_kernel(__nv_bfloat16* __restrict__ out, const __nv_bfloat16* __restrict__ a,
                                                      const __nv_bfloat16* __restrict__ b, int64_t n, int op) {
@@ -383,6 +409,22 @@ int b2_rotary(void* qkv, const int32_t* pos, int batch, int n_heads, int n_group
   const int warps = batch * (n_heads + n_groups);
   B2_LAUNCH_CHECK("rotary", launch(rotary_kernel, dim3((warps + 3) / 4), dim3(128), 0, (cudaStream_t)stream, true,
                                    (__nv_bfloat16*)qkv, pos, batch, n_heads, n_groups, rope->rotary_dim, log2f(rope->base)));
+  return B2_OK;
+}
+
+int b2_qk_rmsnorm(void* y, const void* x, int rows, int64_t ld, int n_heads, int n_groups, int head_size, const b2_qk_norm* norm,
+                  int ft, void* stream) {
+  if (!y || !x || !norm || !norm->q_gamma || !norm->k_gamma || rows <= 0 || n_heads <= 0 || n_groups <= 0) return B2_ERR_PARAM;
+  if (head_size != 128 || (ft != B2_DT_BF16 && ft != B2_DT_F16)) return B2_ERR_UNSUPPORTED;
+  if (ld < (int64_t)(n_heads + 2 * n_groups) * 128) return B2_ERR_PARAM;
+  if ((ld & 3) || !aligned(y, 8) || !aligned(x, 8) || !aligned(norm->q_gamma, 8) || !aligned(norm->k_gamma, 8)) return B2_ERR_UNSUPPORTED;
+  const int64_t warps = (int64_t)rows * (n_heads + 2 * n_groups);
+  if (warps > (int64_t)1 << 31) return B2_ERR_LIMIT;
+  const dim3 grid((unsigned)((warps + 3) / 4)), block(128);
+  const auto kern = ft == B2_DT_F16 ? qk_rmsnorm_kernel<true> : qk_rmsnorm_kernel<false>;
+  B2_LAUNCH_CHECK("qk_rmsnorm", launch(kern, grid, block, 0, (cudaStream_t)stream, true, (__nv_bfloat16*)y, (const __nv_bfloat16*)x,
+                                       ld, warps, n_heads, n_groups, (const __nv_bfloat16*)norm->q_gamma,
+                                       (const __nv_bfloat16*)norm->k_gamma, norm->eps));
   return B2_OK;
 }
 

@@ -1078,6 +1078,15 @@ struct AppendParams {
   int q_len;       // multi-token forms: rows per sequence
   const int32_t* parents;  // tree form: the draft tree of each sequence (format: AttnTreeParams)
 };
+// The per-head Q/K RMSNorm form (cache_append_kernel<..., QKN = true>) takes these fields on top, like AttnTokParams: the
+// kernels without the norm keep their parameter block and code.
+struct AppendNormParams : AppendParams {
+  const __nv_bfloat16* q_gamma;  // [128] FT, 8-byte aligned
+  const __nv_bfloat16* k_gamma;
+  float eps;
+};
+template <bool QKN>
+using AppendArgs = std::conditional_t<QKN, AppendNormParams, AppendParams>;
 
 // Where row `row` of qkv / q_out goes: its sequence b, the slot it is written to and its rotary position.
 // MT = false: row b is sequence b, at position old_lens[b].  MT = true: row b*q_len + t is token t of sequence b, at position
@@ -1093,8 +1102,10 @@ __device__ __forceinline__ void append_row(const AppendParams& p, int row, int& 
   }
 }
 
-template <int QM, bool H, bool MT = false, bool TREE = false>
-__global__ void __launch_bounds__(128) cache_append_kernel(const AppendParams p) {
+// QKN: each q and k head row is first normalised (head_rmsnorm with q_gamma / k_gamma) and rounded to FT, like the
+// reference's QKLayerNormNoBeta writes an FT tensor for its Rotary; V rows are not.
+template <int QM, bool H, bool MT = false, bool TREE = false, bool QKN = false>
+__global__ void __launch_bounds__(128) cache_append_kernel(const AppendArgs<QKN> p) {
   using F = Ft<H>;
   pdl_wait();
   pdl_launch_dependents();
@@ -1109,6 +1120,9 @@ __global__ void __launch_bounds__(128) cache_append_kernel(const AppendParams p)
   int b, wpos, pos;
   append_row<MT, TREE>(p, row, b, wpos, pos);
   const bool is_v = slot >= p.n_heads + p.n_groups;
+  if constexpr (QKN) {
+    if (!is_v) head_rmsnorm<H>(x, slot < p.n_heads ? p.q_gamma : p.k_gamma, p.eps, lane);  // warp-uniform branch
+  }
 
   if (p.rope && !is_v) {
     // NeoX rotate-half over the first rotary_dim dims: out[i] = x[i]cos - x[i+h]sin ; out[i+h] = x[i+h]cos + x[i]sin
@@ -1473,12 +1487,16 @@ static int append_check(const b2_span_cfg* cfg, bool args_ok, int form, int q_le
   return B2_OK;
 }
 
-// q_len rows per sequence (1 in the single-token form), the nodes of the draft tree `parents` in the tree form
+// q_len rows per sequence (1 in the single-token form), the nodes of the draft tree `parents` in the tree form; norm: the
+// per-head Q/K RMSNorm before rotary (validated by the caller), or NULL
 static int cache_append_launch(const b2_span_cfg* cfg, void* const* k_spans, void* const* v_spans, void* q_out, const void* qkv,
                                const int32_t* old_lens, const int32_t* parents, int form, int batch, int q_len,
-                               const b2_rope_cfg* rope, void* stream_) {
+                               const b2_rope_cfg* rope, void* stream_, const b2_qk_norm* norm = nullptr) {
   if (rope && (rope->rotary_dim != 128 && rope->rotary_dim != 64)) return B2_ERR_UNSUPPORTED;
-  AppendParams p;
+  AppendNormParams p;  // each kernel takes the base it needs (AppendArgs)
+  p.q_gamma = norm ? (const __nv_bfloat16*)norm->q_gamma : nullptr;
+  p.k_gamma = norm ? (const __nv_bfloat16*)norm->k_gamma : nullptr;
+  p.eps = norm ? norm->eps : 0.f;
   p.parents = parents;
   p.k_spans = k_spans; p.v_spans = v_spans;
   p.q_out = (__nv_bfloat16*)q_out; p.qkv = (const __nv_bfloat16*)qkv; p.old_lens = old_lens;
@@ -1493,7 +1511,9 @@ static int cache_append_launch(const b2_span_cfg* cfg, void* const* k_spans, voi
   const cudaError_t e = with_kv_mode(cfg->quant_mode, [&](auto QM) {
     return with_flag(cfg->ft == B2_DT_F16, [&](auto H) {
       return with_step_form(form, [&](auto MT, auto TREE) {
-        return launch(cache_append_kernel<QM, H, MT, TREE>, grid, block, 0, (cudaStream_t)stream_, true, p);
+        return with_flag(norm != nullptr, [&](auto QKN) {
+          return launch(cache_append_kernel<QM, H, MT, TREE, QKN>, grid, block, 0, (cudaStream_t)stream_, true, p);
+        });
       });
     });
   });
@@ -1524,6 +1544,17 @@ int b2_span_cache_append_tree(const b2_span_cfg* cfg, void* const* k_spans, void
                               void* stream_) {
   if (int st = append_check(cfg, k_spans && v_spans && q_out && qkv && old_lens && parents && batch > 0, 2, q_len)) return st;
   return cache_append_launch(cfg, k_spans, v_spans, q_out, qkv, old_lens, parents, 2, batch, q_len, rope, stream_);
+}
+
+int b2_span_cache_append_qknorm(const b2_span_cfg* cfg, void* const* k_spans, void* const* v_spans, void* q_out, const void* qkv,
+                                const int32_t* old_lens, const int32_t* parents, int batch, int q_len, const b2_rope_cfg* rope,
+                                const b2_qk_norm* norm, void* stream_) {
+  const int form = parents ? 2 : (q_len == 1 ? 0 : 1);
+  if (int st = append_check(cfg, k_spans && v_spans && q_out && qkv && old_lens && batch > 0, form, q_len)) return st;
+  if (cfg->head_size != kHead) return B2_ERR_UNSUPPORTED;  // head 64 (span_attn64.cu) has no Q/K norm
+  if (!norm || !norm->q_gamma || !norm->k_gamma) return B2_ERR_PARAM;
+  if (((uintptr_t)norm->q_gamma & 7) || ((uintptr_t)norm->k_gamma & 7)) return B2_ERR_UNSUPPORTED;
+  return cache_append_launch(cfg, k_spans, v_spans, q_out, qkv, old_lens, parents, form, batch, q_len, rope, stream_, norm);
 }
 
 int b2_span_cache_compact(const b2_span_cfg* cfg, void* const* const* k_tables, void* const* const* v_tables, int n_layers,

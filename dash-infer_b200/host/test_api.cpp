@@ -7,6 +7,7 @@
 
 #include "allreduce_op.h"
 #include "gemm_lowp_gpu.h"
+#include "qk_layernorm_op.h"
 #include "span_attn_op_cuda.h"
 
 using namespace allspark;
@@ -219,6 +220,51 @@ int as_test_span_attn(int batch, int steps, int n_heads, int n_groups, int span_
     return cudaGetLastError() == cudaSuccess ? 0 : -3;
   } catch (const std::exception& e) {
     AS_LOG_ERROR("as_test_span_attn: %s", e.what());
+    return -1;
+  }
+}
+
+// QKLayerNormNoBeta on a rank of an nranks-way tensor-parallel context: attributes num_heads / multi_query_group_num are the
+// whole model's, the op divides them.  x_host / out_host [batch][(nH/nranks + 2 nG') * head_dim] in the test dtype, nG' as
+// the op derives it; q_gamma_host / k_gamma_host [head_dim].
+int as_test_qk_layernorm(int nranks, int batch, int num_heads, int groups, int head_dim, float eps, const void* x_host,
+                         const void* q_gamma_host, const void* k_gamma_host, void* out_host) {
+  try {
+    CUDAContext ctx;
+    ctx.SetDtype(g_test_ft);
+    ctx.SetRank(0, nranks);
+    const int nH = num_heads / nranks, nG = groups != 1 ? groups / nranks : 1;
+    const int64_t W = (int64_t)(nH + 2 * nG) * head_dim;
+    TensorMap tensors, weights, weights_buffer;
+    auto add = [&](TensorMap& m, const std::string& name, Shape s, const void* src) {
+      auto t = std::make_shared<AsTensor>(name, DeviceType::CUDA, g_test_ft, DataMode::DENSE, s);
+      t->CopyDataFrom(src, t->GetSizeInByte(), DeviceType::CPU);
+      m[name] = t;
+    };
+    add(tensors, "qkv", Shape{batch, 1, W}, x_host);
+    add(weights, "q_norm.weight", Shape{head_dim}, q_gamma_host);
+    add(weights, "k_norm.weight", Shape{head_dim}, k_gamma_host);
+    OperatorProto proto;
+    proto.op_type_ = "QKLayerNormNoBeta"; proto.op_name_ = "decoder.layer.0.attention.qk_norm";
+    proto.inputs_.push_back({"qkv"}); proto.outputs_.push_back({"qkv_normed"});
+    proto.weights_.push_back({"q_norm.weight"}); proto.weights_.push_back({"k_norm.weight"});
+    proto.SetAttr<float>("eps", eps);
+    proto.SetAttr<int>("num_heads", num_heads);
+    proto.SetAttr<int>("multi_query_group_num", groups);
+    auto op = OpFactory::getInstance().GetOperator({"QKLayerNormNoBeta", DeviceType::CUDA})();
+    AsStatus st = op->InitV2(proto, ctx, weights, weights_buffer, &tensors, nullptr);
+    if (st != AsStatus::ALLSPARK_SUCCESS) return (int)st;
+    st = op->Reshape();
+    if (st != AsStatus::ALLSPARK_SUCCESS) return (int)st;
+    st = op->Forward();
+    if (st != AsStatus::ALLSPARK_SUCCESS) return (int)st;
+    ctx.Synchronize();
+    auto out = tensors["qkv_normed"];
+    if (out->GetShape().Count() != (int64_t)batch * W) return -2;
+    out->CopyDataTo(out_host, out->GetSizeInByte(), DeviceType::CPU);
+    return cudaGetLastError() == cudaSuccess ? 0 : -3;
+  } catch (const std::exception& e) {
+    AS_LOG_ERROR("as_test_qk_layernorm: %s", e.what());
     return -1;
   }
 }

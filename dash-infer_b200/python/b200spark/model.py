@@ -31,6 +31,7 @@ class ModelConfig:
     rope_base: float = 1e6
     eps: float = 1e-6
     qkv_bias: bool = True
+    qk_norm: bool = False  # Qwen3: per-head RMSNorm of the q and k heads before rotary (QKLayerNormNoBeta), head 128 only
 
 
 QWEN2_7B = ModelConfig("Qwen2-7B", 3584, 28, 4, 18944, 28, 152064)
@@ -38,6 +39,10 @@ LLAMA3_8B = ModelConfig("Llama-3-8B", 4096, 32, 8, 14336, 32, 128256, rope_base=
 QWEN2_72B = ModelConfig("Qwen2-72B", 8192, 64, 8, 29568, 80, 152064)
 QWEN2_05B = ModelConfig("Qwen2-0.5B", 896, 14, 2, 4864, 24, 151936, head=64)   # config C0: the CPU-parity anchor
 TINY = ModelConfig("tiny-2L", 512, 8, 2, 1024, 2, 1024)
+# Qwen3 dense models (shapes of the published config.json files): no QKV bias, per-head Q/K norm, head_dim 128 carried
+# explicitly — n_heads * head differs from hidden for 0.6B (16 x 128 = 2048 against 1024), so o_proj's K is not hidden
+QWEN3_8B = ModelConfig("Qwen3-8B", 4096, 32, 8, 12288, 36, 151936, qkv_bias=False, qk_norm=True)
+QWEN3_06B = ModelConfig("Qwen3-0.6B", 1024, 16, 8, 3072, 28, 151936, qkv_bias=False, qk_norm=True)  # full-depth parity anchor
 
 KV_MODES = {"none": KV_NONE, "bf16": KV_NONE, "i8": KV_I8, "u4": KV_U4, "fp8": KV_FP8}
 
@@ -140,6 +145,7 @@ class DecodeStack:
         assert 1 <= q_len <= 16 and (q_len == 1 or (tp_size == 1 and cfg.head == 128)), \
             "multi-token steps: q_len <= 16, single GPU, head size 128"
         assert not tree or (q_len > 1 and tp_size == 1 and cfg.head == 128), "draft trees: q_len > 1, single GPU, head size 128"
+        assert not cfg.qk_norm or cfg.head == 128, "per-head Q/K norm: head size 128"
         self.dtype = _DT = dtype
         self.q_len, self.tree = q_len, tree
         rows = batch * q_len  # activation rows of a step
@@ -166,9 +172,15 @@ class DecodeStack:
         col_i = ("cols", TP.col_range_even(I, r, tp)) if tp > 1 else None
         row = ("rows", r, tp) if tp > 1 else None
         self.embed = synth_weight(cfg.vocab, H, gen, device, std=1.0)
+        # the Q/K norm gammas come from their own generator, so a stack with qk_norm=False gets identical weights otherwise;
+        # every rank keeps them whole (they are per head, shared by all heads)
+        gen_qk = torch.Generator(device=device).manual_seed(seed + 1) if cfg.qk_norm else None
         self.layers = []
         for _ in range(self.n_layers):
             L = {}
+            if cfg.qk_norm:
+                L["qn"] = (1.0 + 0.1 * torch.randn(hd, generator=gen_qk, device=device)).to(_DT)
+                L["kn"] = (1.0 + 0.1 * torch.randn(hd, generator=gen_qk, device=device)).to(_DT)
             L["g1"] = (1.0 + 0.1 * torch.randn(H, generator=gen, device=device)).to(_DT)
             L["qkv"] = QuantLinear(H, (nH + 2 * nG) * hd, wbits, group, gen, device, rows, bias=cfg.qkv_bias, keep_ref=keep_ref,
                                    shard=col_qkv)
@@ -339,7 +351,8 @@ class DecodeStack:
             else:
                 ops.rmsnorm(self.x, L["g1"], cfg.eps, out=self.xn); n += 1
                 L["qkv"](self.xn, ws, out=self.qkv); n += 1
-            ops._cache_append(L["cache"], self.qkv, self.lens_old, q_out=self.q, rope=self.rope, **form); n += 1
+            ops._cache_append(L["cache"], self.qkv, self.lens_old, q_out=self.q, rope=self.rope,
+                              qk_norm=(L["qn"], L["kn"], cfg.eps) if cfg.qk_norm else None, **form); n += 1
             self.attn._run(self.q, L["cache"], self.lens_new, self.max_len, ws, out=self.ao, **form); n += 1
             if norm == "self":
                 n = self._row_parallel(L["o"], self.ao, n)

@@ -7,7 +7,7 @@ import ctypes as C
 import torch
 
 from . import _lib
-from ._lib import (ACT_NONE, BIN_ADD, BIN_MUL, DT_BF16, DT_I8, DT_U8, KV_I8, KV_NONE, KV_U4, GemmDesc, GemmFuse, RopeCfg,
+from ._lib import (ACT_NONE, BIN_ADD, BIN_MUL, DT_BF16, DT_I8, DT_U8, KV_I8, KV_NONE, KV_U4, GemmDesc, GemmFuse, QkNorm, RopeCfg,
                    SpanCfg, check, lib)
 
 
@@ -239,11 +239,32 @@ class SpanCache:
         return pool[off: off + self.span_bytes]
 
 
-def _cache_append(cache, qkv, old_lens, q_out=None, rope=None, q_len=None, parents=None):
+def _qk_norm(norm, dtype, device):
+    """(q_gamma, k_gamma, eps) -> QkNorm; the gammas are [128] contiguous tensors of the model FT on the activations' device"""
+    q_gamma, k_gamma, eps = norm
+    for g in (q_gamma, k_gamma):
+        assert g.shape == (128,) and g.dtype == dtype and g.is_contiguous() and g.device == device, \
+            "qk_norm gammas: contiguous [128] tensors of the model dtype on the activations' device"
+    return QkNorm(q_gamma.data_ptr(), k_gamma.data_ptr(), float(eps), 0)
+
+
+def qk_rmsnorm(x, n_heads, n_groups, q_gamma, k_gamma, eps=1e-6, out=None):
+    """QKLayerNormNoBeta (b2_qk_rmsnorm): x [rows, >= (n_heads + 2 n_groups) * 128] FT, row stride x.stride(0); the q and k
+    heads of each row are RMS-normalised per head with q_gamma / k_gamma [128], the V heads copied.  out may be x."""
+    out = torch.empty_strided(x.shape, x.stride(), dtype=x.dtype, device=x.device) if out is None else out
+    assert x.dim() == 2 and x.stride(-1) == 1 and out.shape == x.shape and out.stride() == x.stride() and out.dtype == x.dtype
+    nrm = _qk_norm((q_gamma, k_gamma, eps), x.dtype, x.device)
+    check(lib.b2_qk_rmsnorm(_ptr(out), _ptr(x), x.shape[0], x.stride(0), int(n_heads), int(n_groups), 128, C.byref(nrm), _ft(x),
+                            _stream()), "b2_qk_rmsnorm")
+    return out
+
+
+def _cache_append(cache, qkv, old_lens, q_out=None, rope=None, q_len=None, parents=None, qk_norm=None):
     """Append one step's rows to the span cache (+ optional fused rotary).  q_len None: row b of qkv is sequence b, written at
     position old_lens[b].  q_len: row b*q_len + t is token t of sequence b, written at position old_lens[b] + t; with parents
     (int32 [B, q_len]) it is node t of sequence b's draft tree, written at slot old_lens[b] + t with rotary position
-    old_lens[b] + depth(t)."""
+    old_lens[b] + depth(t).  qk_norm = (q_gamma, k_gamma, eps): the per-head Q/K RMSNorm before rotary
+    (b2_span_cache_append_qknorm), every step form."""
     cfg = cache.cfg
     rows = qkv.shape[0]
     assert rows % (q_len or 1) == 0 and (parents is None or (q_len and parents.dtype == torch.int32 and parents.is_contiguous()))
@@ -252,7 +273,11 @@ def _cache_append(cache, qkv, old_lens, q_out=None, rope=None, q_len=None, paren
     r = RopeCfg(float(rope[0]), int(rope[1]), 0) if rope is not None else None
     head = (C.byref(cfg), _ptr(cache.k_tab), _ptr(cache.v_tab), _ptr(q_out), _ptr(qkv), _ptr(old_lens))
     tail = (C.byref(r) if r is not None else None, _stream())
-    if q_len is None:
+    if qk_norm is not None:
+        nrm = _qk_norm(qk_norm, qkv.dtype, qkv.device)
+        check(lib.b2_span_cache_append_qknorm(*head, _ptr(parents), rows // (q_len or 1), int(q_len or 1), tail[0], C.byref(nrm),
+                                              tail[1]), "b2_span_cache_append_qknorm")
+    elif q_len is None:
         check(lib.b2_span_cache_append(*head, rows, *tail), "b2_span_cache_append")
     elif parents is None:
         check(lib.b2_span_cache_append_tokens(*head, rows // q_len, int(q_len), *tail), "b2_span_cache_append_tokens")

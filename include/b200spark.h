@@ -26,6 +26,8 @@
  *   b2_rmsnorm, b2_rotary, b2_binary, b2_embedding, b2_argmax ("next" rows, SURVEY.md §8f)
  *                         LayerNormNoBeta / Rotary / Binary / EmbeddingT5 / GenerateOp(top_k=1)
  *                           csrc/core/kernel/cuda/layernorm.cu:86, rotary.cu:23, binary.cu
+ *   b2_qk_rmsnorm, b2_span_cache_append_qknorm
+ *                         QKLayerNormNoBeta (Qwen3, qwen_v30.py)  csrc/core/kernel/cuda/layernorm.cu:259-304
  */
 #ifndef B200SPARK_H_
 #define B200SPARK_H_
@@ -278,6 +280,28 @@ int b2_span_attn_run_tree(b2_span_attn_t handle, void* out, const void* q, const
                           const void* const* v_spans, const int32_t* new_lens, const int32_t* parents, int batch, int q_len,
                           int max_len, void* workspace, size_t workspace_bytes, float qk_scale, void* stream);
 
+/* ---- Per-head Q/K RMSNorm (Qwen3: the reference's QKLayerNormNoBeta operator, qwen_v30.py; arithmetic of its
+ * batch_layernorm_nobeta_kernel, layernorm.cu:259-304).  Head 128 only.  For each q head and each k head of a row, with x
+ * the 128 stored FT values of that head:
+ *   ss = sum x^2 in fp32: each lane of a warp sums its 4 consecutive squares in order, then an xor butterfly over
+ *        16, 8, 4, 2, 1 (a fixed order, so results are deterministic);
+ *   rs = rsqrtf(ss * (1/128) + eps);   y = FT((x * rs) * gamma), one FT rounding.
+ * q heads use q_gamma, k heads k_gamma (both shared by all heads of their kind). */
+typedef struct {
+  const void* q_gamma; /* [head_size] FT, 8-byte aligned */
+  const void* k_gamma; /* [head_size] FT, 8-byte aligned */
+  float eps;
+  int32_t reserved;
+} b2_qk_norm;
+/* b2_span_cache_append / _tokens / _tree with the per-head norm applied to the q and k rows as they are loaded, before the
+ * fused rotary (which rounds to FT again, as without the norm); V rows are stored as given.  parents == NULL: the
+ * single-token form (q_len 1) or the chain form (q_len > 1); otherwise the tree form.  The span bytes, {zero, scale} and
+ * q_out equal those of b2_qk_rmsnorm followed by the matching entry point without the norm, bit for bit.  NULL norm or
+ * gamma: B2_ERR_PARAM; a misaligned gamma or head_size != 128: B2_ERR_UNSUPPORTED; q_len and batch as the other appends. */
+int b2_span_cache_append_qknorm(const b2_span_cfg* cfg, void* const* k_spans, void* const* v_spans, void* q_out,
+                                const void* qkv, const int32_t* old_lens, const int32_t* parents, int batch, int q_len,
+                                const b2_rope_cfg* rope, const b2_qk_norm* norm, void* stream);
+
 /* =====================================================================================
  * Glue ops of the decode graph ("next" rows): element-wise / norm / lookup, FT = bf16.
  * ===================================================================================== */
@@ -294,6 +318,13 @@ int b2_argmax_ft(int64_t* ids_out, float* vals_out /* or NULL */, const void* lo
 /* in-place NeoX rotary on the q and k heads of qkv [batch, (nH+2nG)*head]; position = pos[b] */
 int b2_rotary(void* qkv, const int32_t* pos, int batch, int n_heads, int n_groups, int head_size,
               const b2_rope_cfg* rope, void* stream);
+/* QKLayerNormNoBeta (arithmetic: b2_qk_norm): x, y [rows, ld] FT.  Per row, heads [0, n_heads) and [n_heads,
+ * n_heads + n_groups) are normalised; the V heads [n_heads + n_groups, n_heads + 2 n_groups) are copied unless y == x; the
+ * columns beyond are untouched.  y may be x (any other overlap is undefined).  head_size 128 and ft B2_DT_BF16 / B2_DT_F16
+ * (else B2_ERR_UNSUPPORTED); ld >= (n_heads + 2 n_groups) * 128 (else B2_ERR_PARAM); x, y and the gammas 8-byte aligned and
+ * ld a multiple of 4 (else B2_ERR_UNSUPPORTED). */
+int b2_qk_rmsnorm(void* y, const void* x, int rows, int64_t ld, int n_heads, int n_groups, int head_size,
+                  const b2_qk_norm* norm, int ft, void* stream);
 /* out = a (op) b, n elements; op = B2_BIN_ADD / B2_BIN_MUL */
 int b2_binary(void* out, const void* a, const void* b, int64_t n, int op, void* stream);
 /* out[b,:] = table[ids[b],:] */
