@@ -323,6 +323,15 @@ __device__ __forceinline__ void head_rmsnorm(float (&x)[4], const __nv_bfloat16*
   for (int i = 0; i < 4; ++i) x[i] = F::to_f(F::from_f((x[i] * rs) * gv[i]));
 }
 
+// Order of greedy sampling (torch.argmax's): NaN ranks above every number; among equal values or among NaNs the lower
+// index wins.  (v, i) beats (best, bi) under that order.  The start (-inf, INT_MAX) loses to any element, so every row of
+// n >= 1 elements yields an index in [0, n).  b2_argmax and the top-N of b2_logprobs both rank by it.
+__device__ __forceinline__ bool argmax_beats(float v, int i, float best, int bi) {
+  const bool vn = v != v, bn = best != best;
+  if (vn != bn) return vn;
+  return (!vn && v > best) || ((vn || v == best) && i < bi);
+}
+
 template <int ACT>
 __device__ __forceinline__ float apply_act(float x) {
   // csrc/core/kernel/cuda/hie/cuda_activation.hpp (reference formulas, fp32)

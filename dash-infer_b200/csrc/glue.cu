@@ -243,15 +243,6 @@ __global__ void __launch_bounds__(128) embedding_kernel(__nv_bfloat16* __restric
     *reinterpret_cast<uint4*>(out + (size_t)b * hidden + i) = *reinterpret_cast<const uint4*>(table + (size_t)id * hidden + i);
 }
 
-// Order of greedy sampling (torch.argmax's): NaN ranks above every number; among equal values or among NaNs the lower
-// index wins.  (v, i) beats (best, bi) under that order.  The start (-inf, INT_MAX) loses to any element, so every row of
-// n >= 1 elements yields an index in [0, n).
-__device__ __forceinline__ bool argmax_beats(float v, int i, float best, int bi) {
-  const bool vn = v != v, bn = best != best;
-  if (vn != bn) return vn;
-  return (!vn && v > best) || ((vn || v == best) && i < bi);
-}
-
 // greedy sampling: lowest index among the maxima (bit-exact index contract)
 template <bool H>
 __global__ void __launch_bounds__(1024) argmax_kernel(int64_t* __restrict__ ids_out, float* __restrict__ vals_out,

@@ -128,7 +128,7 @@ class _RefView:
 class DecodeStack:
     def __init__(self, cfg, batch, max_len, wbits=4, group=-1, kv="none", span=128, seed=1234, device="cuda",
                  keep_ref=False, layers=None, tp_rank=0, tp_size=1, tp_group=None, fuse_swiglu=True,
-                 collective=None, comm=None, dtype=torch.bfloat16, q_len=1, tree=False):
+                 collective=None, comm=None, dtype=torch.bfloat16, q_len=1, tree=False, logprobs=0):
         """tp_size > 1: the reference's tensor-parallel layout (QKV/gate/up column split, o/down row split + all-reduce,
         vocab-split lm_head + B-element all-gather); every rank builds the SAME full synthetic weights from `seed` and
         keeps its shard, exactly like the reference splits an already-quantized checkpoint.
@@ -138,7 +138,12 @@ class DecodeStack:
         tree=True (with q_len = T > 1): the T rows of a sequence are the nodes of a draft tree.  self.parents [B, T] int32
         (tree format: include/b200spark.h) is filled by the caller next to self.tokens before each step; the step appends
         and attends in tree form, accepts the longest greedy path and compacts the path's cache rows in every layer.
-        step() returns (pred [B, T], accepted [B], path [B, T]); the emitted tokens are pred[b, path[b, :accepted[b]]]."""
+        step() returns (pred [B, T], accepted [B], path [B, T]); the emitted tokens are pred[b, path[b, :accepted[b]]].
+        logprobs = N (0 <= N <= 10): the step also returns log-probabilities on the device (b2_logprobs; TP > 1: per-rank
+        records, one all-gather, b2_logprobs_merge) in place of the argmax, with the same ids and launch count: self.tok_lp
+        [B*T] fp32 (the logprob of each row's own argmax), self.top_ids [B*T, N] int64 and self.top_lp [B*T, N] fp32 (the N
+        most likely tokens, argmax order).  Every row of a multi-token or tree step gets them; the logprob of an emitted token
+        is tok_lp at its row: row b*T + u for the token pred[b, u] (u = path[b, j] in a tree).  N = 0 runs today's step."""
         global _DT
         assert dtype in (torch.bfloat16, torch.float16) and (dtype == torch.bfloat16 or (tp_size == 1 and cfg.head == 128)), \
             "fp16: single GPU, head size 128 (the communicator and the head-64 kernels are bf16)"
@@ -146,6 +151,8 @@ class DecodeStack:
             "multi-token steps: q_len <= 16, single GPU, head size 128"
         assert not tree or (q_len > 1 and tp_size == 1 and cfg.head == 128), "draft trees: q_len > 1, single GPU, head size 128"
         assert not cfg.qk_norm or cfg.head == 128, "per-head Q/K norm: head size 128"
+        assert 0 <= logprobs <= ops._lib.MAX_TOP_LOGPROBS, "logprobs: 0 .. 10 alternatives"
+        self.logprobs = logprobs
         self.dtype = _DT = dtype
         self.q_len, self.tree = q_len, tree
         rows = batch * q_len  # activation rows of a step
@@ -221,14 +228,23 @@ class DecodeStack:
                           qkv=torch.empty(rows, (nHl + 2 * nGl) * hd, **bf), q=torch.empty(rows, nHl * hd, **bf),
                           ao=torch.empty(rows, nHl * hd, **bf), gate=torch.empty(rows, self.I_l, **bf),
                           up=torch.empty(rows, self.I_l, **bf), logits=torch.empty(rows, self.vocab_l, **bf))
+        if logprobs:
+            self._bufs.update(tok_lp=torch.empty(rows, dtype=torch.float32, device=device),
+                              top_ids=torch.empty(rows, logprobs, dtype=torch.int64, device=device),
+                              top_lp=torch.empty(rows, logprobs, dtype=torch.float32, device=device))
         if tp > 1:
+            rec = ops.logprobs_partial_bytes(logprobs) if logprobs else 0
+            if logprobs:  # one record per row and rank (b2_logprobs_shard), all-gathered as bytes
+                self._bufs["loc_rec"] = torch.empty(batch, rec, dtype=torch.uint8, device=device)
+                self._all_rec = torch.empty(tp * batch * rec, dtype=torch.uint8, device=device)
             if self.collective != "nccl" and self.comm is None:
-                self.comm = ops.Comm(tp_rank, tp, max(batch * H * 2, 4096)).connect_group(tp_group)
+                self.comm = ops.Comm(tp_rank, tp, max(batch * H * 2, 4096, batch * rec)).connect_group(tp_group)
             self._bufs["part"] = torch.empty(batch, H, **bf)             # row-split partial sums (all-reduced)
-            self.loc_ids = torch.empty(batch, dtype=torch.int64, device=device)
-            self.loc_val = torch.empty(batch, dtype=torch.float32, device=device)
-            self.all_ids = torch.empty(tp, batch, dtype=torch.int64, device=device)
-            self.all_val = torch.empty(tp, batch, dtype=torch.float32, device=device)
+            if not logprobs:  # the argmax path's per-rank (max, argmax) pairs
+                self.loc_ids = torch.empty(batch, dtype=torch.int64, device=device)
+                self.loc_val = torch.empty(batch, dtype=torch.float32, device=device)
+                self.all_ids = torch.empty(tp, batch, dtype=torch.int64, device=device)
+                self.all_val = torch.empty(tp, batch, dtype=torch.float32, device=device)
         self.graph = None
         self.set_batch(batch)
         if self._norm_placement(rows) == "handoff":  # per-tile row statistics of o_proj / down_proj, [tiles][R] per step
@@ -250,6 +266,9 @@ class DecodeStack:
             self.tokens, self.pred, self.accepted = self._tokens[:b], self._pred[:b], self._accepted[:b]
         if self.tree:
             self.parents, self.path = self._parents[:b], self._path[:b]
+        if self.logprobs and self.tp > 1:
+            rec = self._all_rec.numel() // (self.tp * self.Bmax)
+            self.all_rec = self._all_rec[:self.tp * b * rec].view(self.tp, b * rec)
         self.graph = None
 
     # ------------------------------------------------------------------ cache fill
@@ -380,7 +399,15 @@ class DecodeStack:
         else:
             ops.rmsnorm(self.x, self.gf, cfg.eps, out=self.xn); n += 1
             self.lm_head(self.xn, ws, out=self.logits); n += 1
-        if T > 1:
+        if self.logprobs and self.tp == 1:  # the argmax ids and the log-probabilities in one launch
+            ids = self.pred.view(-1) if T > 1 else self.next_ids
+            ops.logprobs(self.logits, self.logprobs, out=(ids, self.tok_lp, self.top_ids, self.top_lp)); n += 1
+        elif self.logprobs:  # vocab-split: per-rank records, one all-gather of them, the merge
+            ops.logprobs_shard(self.logits, self.logprobs, self.tp_rank * self.vocab_l, out=self.loc_rec); n += 1
+            self._gather_records()
+            n += self.collective != "nccl"
+            ops.logprobs_merge(self.all_rec, self.logprobs, out=(self.next_ids, self.tok_lp, self.top_ids, self.top_lp)); n += 1
+        elif T > 1:
             ops.argmax(self.logits, out=self.pred.view(-1)); n += 1
         elif self.tp == 1:
             ops.argmax(self.logits, out=self.next_ids); n += 1
@@ -408,6 +435,14 @@ class DecodeStack:
         qchunks = ((R + 15) // 16 if (self.group_size != -1 and self.wbits != 4) else hchunks) if R > 16 else 1
         n += (qchunks - 1) * (4 if self.fuse_swiglu else 5) * len(self.layers) + (hchunks - 1)
         self.launches_per_step = n
+
+    def _gather_records(self):
+        """all-gather the per-rank logprob records (opaque bytes) of the vocab-split lm_head"""
+        if self.collective == "nccl":
+            import torch.distributed as dist
+            dist.all_gather_into_tensor(self.all_rec, self.loc_rec.view(-1), group=self.tp_group)
+        else:
+            self.comm.allgather(self.loc_rec, self.all_rec)
 
     def step(self):
         """q_len 1: returns next_ids [B].  q_len > 1: one verify step, returns (pred [B, T], accepted [B]); the step's
@@ -449,7 +484,9 @@ class DecodeStack:
         def ops_():
             for _ in range(2 * len(self.layers)):
                 self._allreduce(self.part)
-            if self.collective == "nccl":
+            if self.logprobs:
+                self._gather_records()
+            elif self.collective == "nccl":
                 dist_.all_gather_into_tensor(self.all_val, self.loc_val, group=self.tp_group)
                 dist_.all_gather_into_tensor(self.all_ids, self.loc_ids, group=self.tp_group)
             else:

@@ -481,6 +481,71 @@ def argmax_merge(all_vals, all_ids, out):
     return out
 
 
+def _lp_outputs(rows, n_top, device, out):
+    """(ids [rows] int64, tok_lp [rows] fp32, top_ids [rows, n_top] int64 or None, top_lp [rows, n_top] fp32 or None)"""
+    if out is not None:
+        ids, tok_lp, top_ids, top_lp = out
+    else:
+        ids = torch.empty(rows, dtype=torch.int64, device=device)
+        tok_lp = torch.empty(rows, dtype=torch.float32, device=device)
+        top_ids = torch.empty(rows, n_top, dtype=torch.int64, device=device) if n_top else None
+        top_lp = torch.empty(rows, n_top, dtype=torch.float32, device=device) if n_top else None
+    for t, dt, shape in ((ids, torch.int64, (rows,)), (tok_lp, torch.float32, (rows,)), (top_ids, torch.int64, (rows, n_top)),
+                         (top_lp, torch.float32, (rows, n_top))):
+        assert t is None or (t.dtype == dt and t.is_contiguous() and tuple(t.shape) == shape), \
+            f"logprobs outputs: {shape} {dt} contiguous"
+    assert (top_ids is None) == (n_top == 0) and (top_lp is None) == (n_top == 0)
+    return ids, tok_lp, top_ids, top_lp
+
+
+def _tok_ids(tok_ids, rows):
+    assert tok_ids is None or (tok_ids.dtype == torch.int64 and tok_ids.is_contiguous() and tok_ids.numel() == rows)
+    return _ptr(tok_ids)
+
+
+def logprobs(logits, n_top, tok_ids=None, out=None):
+    """Log-probabilities of the rows of logits [rows, n] FT (b2_logprobs; any row stride): returns (ids, tok_lp, top_ids,
+    top_lp) — the argmax ids (== argmax()), the logprob of tok_ids[r] (of the top-1 without tok_ids), and the top n_top
+    (0 <= n_top <= 10) ids and logprobs in argmax order (None when n_top == 0).  out: the four tensors to write (ids or
+    tok_lp may be None)."""
+    rows, n = logits.shape
+    assert logits.stride(-1) == 1
+    ids, tok_lp, top_ids, top_lp = _lp_outputs(rows, n_top, logits.device, out)
+    check(lib.b2_logprobs(_ptr(ids), _ptr(tok_lp), _ptr(top_ids), _ptr(top_lp), _tok_ids(tok_ids, rows), _ptr(logits), rows, n,
+                          logits.stride(0), int(n_top), _ft(logits), _stream()), "b2_logprobs")
+    return ids, tok_lp, top_ids, top_lp
+
+
+def logprobs_partial_bytes(n_top):
+    return lib.b2_logprobs_partial_bytes(int(n_top))
+
+
+def logprobs_shard(logits, n_top, id_offset, tok_ids=None, out=None):
+    """The vocab-split form's first half (b2_logprobs_shard): logits [rows, n] hold vocab ids id_offset .. id_offset + n - 1;
+    returns the rows' partial records, uint8 [rows, logprobs_partial_bytes(n_top)] (opaque bytes for an all-gather)."""
+    rows, n = logits.shape
+    assert logits.stride(-1) == 1
+    if out is None:
+        out = torch.empty(rows, logprobs_partial_bytes(n_top), dtype=torch.uint8, device=logits.device)
+    assert out.dtype == torch.uint8 and out.is_contiguous() and out.numel() == rows * logprobs_partial_bytes(n_top)
+    check(lib.b2_logprobs_shard(_ptr(out), _tok_ids(tok_ids, rows), _ptr(logits), rows, n, logits.stride(0), int(id_offset),
+                                int(n_top), _ft(logits), _stream()), "b2_logprobs_shard")
+    return out
+
+
+def logprobs_merge(all_partials, n_top, out=None):
+    """The second half (b2_logprobs_merge): all_partials uint8 [nranks, rows * bytes] (or [nranks, rows, bytes]), the ranks'
+    records as all-gathered; returns logprobs()' outputs over the whole vocabulary."""
+    nranks, rb = all_partials.shape[0], logprobs_partial_bytes(n_top)
+    rows = all_partials[0].numel() // rb
+    assert all_partials.dtype == torch.uint8 and all_partials.is_contiguous()
+    assert rows > 0 and all_partials[0].numel() == rows * rb, "records of another n_top: %d bytes per rank" % all_partials[0].numel()
+    ids, tok_lp, top_ids, top_lp = _lp_outputs(rows, n_top, all_partials.device, out)
+    check(lib.b2_logprobs_merge(_ptr(ids), _ptr(tok_lp), _ptr(top_ids), _ptr(top_lp), _ptr(all_partials), nranks, rows, int(n_top),
+                                _stream()), "b2_logprobs_merge")
+    return ids, tok_lp, top_ids, top_lp
+
+
 def lens_add(lens, delta):
     check(lib.b2_lens_add(_ptr(lens), lens.numel(), int(delta), _stream()), "b2_lens_add")
     return lens

@@ -343,6 +343,46 @@ int b2_argmax_shard(int64_t* ids_out, float* vals_out, const void* logits, int b
  * pairs were all-gathered ([nranks][batch] each).  With rank r holding vocab ids [r*n, (r+1)*n), it equals b2_argmax of the
  * whole row. */
 int b2_argmax_merge(int64_t* ids_out, const float* all_vals, const int64_t* all_ids, int nranks, int batch, void* stream);
+/* Log-probabilities of the decode step (logprobs / top_logprobs of a greedy step), on the device, CUDA-graph replayable.
+ * A row runs on one CTA, or on a cluster of 8 CTAs when n > 32768 (a function of n alone: the same bits at every batch).
+ * logits FT [rows, ld] (ft = B2_DT_BF16 / B2_DT_F16), the first n columns of each row; columns n .. ld-1 are ignored.  Per
+ * row, with every value widened to fp32 exactly:
+ *   m = the row maximum;  s = sum_i expf(x_i - m) in fp32;  lp_i = (x_i - m) - logf(s)  (lse = m + logf(s)).
+ *   top_ids[r][k], top_lp[r][k] (k < n_top, 0 <= n_top <= B2_MAX_TOP_LOGPROBS): the first n_top entries in argmax order (NaN
+ *   first, then descending value, the lower index on ties), so top_ids[r][0] == ids_out[r] == b2_argmax's id bit for bit.
+ *   When n_top > n the slots past n hold id -1 and lp -inf.
+ *   tok_lp[r] = lp at tok_ids[r] when tok_ids is given, else at the top-1.  An id outside [0, n) gives NaN (never read).
+ * Non-finite rows follow torch.log_softmax(x.double()) cast to fp32: a NaN or a +inf anywhere makes every lp of the row NaN,
+ * an all -inf row gives NaN, -inf entries of a row with a finite maximum give -inf.  The ids follow argmax order all the same.
+ * Accuracy, per element against log_softmax of the widened row in fp64, for a row of finite maximum:
+ *   |lp_i - exact| <= (1 + u)(u |x_i - m| + dL) + u |exact|,  u = 2^-24,
+ *   dL = -log(1 - e_s) + 2^-23 (|L| - log(1 - e_s)),  L = log(sum_i exp(x_i - m)),
+ *   e_s = (sum_i t_i ((1 + 2^-22) exp(u |x_i - m|) (1 + u)^d - 1) + n 2^-148 (1 + u)^d) / sum_i t_i,  t_i = exp(x_i - m),
+ * with d = ceil(n / (1024 C)) + 8 + C additions on a term's way into s, C the CTAs of the row (expf's 2 ulp, the
+ * rounding of x_i - m, the sum, logf's ulp and the final subtraction); the merge adds, per rank, the rounding of m_q - M
+ * and expf's 2 ulp on that rank's scale, and its
+ * fused multiply-add.  A result beyond the fp32 range is -inf.  The reduction order is fixed and there are no atomics:
+ * results are bitwise repeatable.  Unlike the reference, whose logprobs are rounded to FT before its top-k
+ * (generate_impl_gpu.hpp:46-64), these are fp32.
+ * n_top outside [0, 10], n < 1, ld < n, top_ids / top_lp NULL with n_top > 0 or given with n_top == 0, or no output at all:
+ * B2_ERR_PARAM, before any launch. */
+#define B2_MAX_TOP_LOGPROBS 10 /* the reference's engine_max_top_logprobs */
+int b2_logprobs(int64_t* ids_out /* [rows] or NULL */, float* tok_lp /* [rows] or NULL */, int64_t* top_ids, float* top_lp,
+                const int64_t* tok_ids /* [rows] or NULL */, const void* logits, int rows, int n, int64_t ld, int n_top, int ft,
+                void* stream);
+/* Vocab-split form (tensor parallel).  b2_logprobs_shard writes one record of b2_logprobs_partial_bytes(n_top) bytes per row
+ * (partials [rows][bytes], 4-byte aligned): the shard's m and s, its top max(n_top, 1) (value, id + id_offset) padded with
+ * (-inf, INT_MAX), and the token's logit when tok_ids[r] lies in [id_offset, id_offset + n).  The records are opaque bytes
+ * (b2_allgather moves them unchanged).  id_offset >= 0 and id_offset + n < INT_MAX (else B2_ERR_PARAM).
+ * b2_logprobs_merge takes all_partials [nranks][rows][bytes] and writes b2_logprobs' outputs over the whole vocabulary:
+ *   M = max_q m_q,  S = sum_q s_q expf(m_q - M) in rank order (shards with m_q = -inf add nothing),  lp = (x - M) - logf(S);
+ * the top list is taken over the nranks x max(n_top, 1) candidates in argmax order (the lowest id, i.e. the lowest rank, on
+ * ties).  One shard of the whole row followed by the merge equals b2_logprobs bit for bit. */
+size_t b2_logprobs_partial_bytes(int n_top); /* 0 for n_top outside [0, 10] */
+int b2_logprobs_shard(void* partials, const int64_t* tok_ids /* or NULL */, const void* logits, int rows, int n, int64_t ld,
+                      int64_t id_offset, int n_top, int ft, void* stream);
+int b2_logprobs_merge(int64_t* ids_out, float* tok_lp, int64_t* top_ids, float* top_lp, const void* all_partials, int nranks,
+                      int rows, int n_top, void* stream);
 /* lens[b] += delta for b < batch (keeps sequence lengths device-resident under CUDA graphs) */
 int b2_lens_add(int32_t* lens, int batch, int delta, void* stream);
 /* Greedy verification of a multi-token step, on the device (CUDA-graph replayable).  tokens [batch][q_len] int64: column 0
