@@ -40,6 +40,15 @@ inline auto with_kv_mode(int qm, F&& f) {
   return f(std::integral_constant<int, B2_KV_U4>{});
 }
 
+// The argument checks of a scaled-rotary table (b2_rope_table), shared by b2_rotary_table and the table form of the append.
+inline int rope_table_check(const b2_rope_cfg* rope, const b2_rope_table* t) {
+  if (!rope || !t || !t->inv_freq || t->stride < 0) return B2_ERR_PARAM;
+  if (rope->rotary_dim != 128 && rope->rotary_dim != 64) return B2_ERR_UNSUPPORTED;
+  if (t->stride != 0 && t->stride < rope->rotary_dim / 2) return B2_ERR_PARAM;
+  if (((uintptr_t)t->inv_freq & 15) || (t->stride & 3)) return B2_ERR_UNSUPPORTED;  // whole-vector loads of 4 frequencies
+  return B2_OK;
+}
+
 #define B2_CUDA_TRY(expr)                         \
   do {                                            \
     cudaError_t _e = (expr);                      \
@@ -321,6 +330,35 @@ __device__ __forceinline__ void head_rmsnorm(float (&x)[4], const __nv_bfloat16*
   const float gv[4] = {F::lo(g.x), F::hi(g.x), F::lo(g.y), F::hi(g.y)};
 #pragma unroll
   for (int i = 0; i < 4; ++i) x[i] = F::to_f(F::from_f((x[i] * rs) * gv[i]));
+}
+
+// ---- NeoX rotary of one 128-wide q or k head row held 4 consecutive values per lane, with the inverse frequencies read
+// from a caller-given table row (b2_rope_table; the stand-alone b2_rotary_table and the table form of the span-cache append
+// both call this, so they cannot drift apart).  For d = 4 lane + i < rotary_dim, f = d % half:
+//   ang = fl32(pos * inv[f]);  sincosf;  c = fl32(cs * af);  s = fl32(sn * af);
+//   x[i] <- FT(fma(x[i], c, -+fl32(partner * s))), one FT rounding (returned widened); dims >= rotary_dim keep x.
+// The whole warp calls it (it shuffles); rotary_dim is 128 or 64.  inv: 16-byte aligned, so a lane's 4 frequencies
+// (f = 4 lane % half ... + 3) are one vector load.  The products are written as intrinsics so that no FMA contraction can
+// differ between the two callers.
+template <bool H>
+__device__ __forceinline__ void rope_from_table(float (&x)[4], int pos, const float* inv, float af, int rotary_dim, int lane) {
+  using F = Ft<H>;
+  const int half = rotary_dim >> 1;
+  float other[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) other[i] = __shfl_xor_sync(0xffffffffu, x[i], half == 64 ? 16 : 8);
+  if (lane * 4 >= rotary_dim) return;
+  const float4 fr = *reinterpret_cast<const float4*>(inv + ((lane * 4) & (half - 1)));
+  const float fv[4] = {fr.x, fr.y, fr.z, fr.w};
+  const bool lower = lane * 4 < half;  // the same for the lane's 4 dims: half is a multiple of 4
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    float sn, cs;
+    sincosf(__fmul_rn((float)pos, fv[i]), &sn, &cs);
+    const float c = __fmul_rn(cs, af), s = __fmul_rn(sn, af);
+    const float t = __fmul_rn(other[i], s);
+    x[i] = F::to_f(F::from_f(__fmaf_rn(x[i], c, lower ? -t : t)));
+  }
 }
 
 // Order of greedy sampling (torch.argmax's): NaN ranks above every number; among equal values or among NaNs the lower

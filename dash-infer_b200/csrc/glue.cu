@@ -181,6 +181,28 @@ __global__ void __launch_bounds__(128) rotary_kernel(__nv_bfloat16* __restrict__
   *reinterpret_cast<uint2*>(ptr) = make_uint2(pack_bf16x2(x[0], x[1]), pack_bf16x2(x[2], x[3]));
 }
 
+// in-place NeoX rotary from a caller-given frequency table (b2_rotary_table): one warp per (row, q or k head); row b reads
+// the table row inv + b * stride (rope_from_table)
+template <bool H>
+__global__ void __launch_bounds__(128) rotary_table_kernel(__nv_bfloat16* __restrict__ qkv, const int32_t* __restrict__ pos,
+                                                           int batch, int n_heads, int n_groups, int rotary_dim,
+                                                           const float* __restrict__ inv, int64_t stride, float af) {
+  using F = Ft<H>;
+  pdl_wait();
+  pdl_launch_dependents();
+  const int lane = threadIdx.x & 31;
+  const int rot_heads = n_heads + n_groups;
+  const int slots = n_heads + 2 * n_groups;
+  const int wid = blockIdx.x * 4 + (threadIdx.x >> 5);
+  if (wid >= batch * rot_heads) return;
+  const int b = wid / rot_heads, h = wid - b * rot_heads;
+  __nv_bfloat16* ptr = qkv + ((size_t)b * slots + h) * 128 + lane * 4;
+  const uint2 raw = *reinterpret_cast<const uint2*>(ptr);
+  float x[4] = {F::lo(raw.x), F::hi(raw.x), F::lo(raw.y), F::hi(raw.y)};
+  rope_from_table<H>(x, pos[b], inv + (size_t)b * stride, af, rotary_dim, lane);
+  *reinterpret_cast<uint2*>(ptr) = make_uint2(F::pack(x[0], x[1]), F::pack(x[2], x[3]));
+}
+
 // QKLayerNormNoBeta (b2_qk_rmsnorm): one warp per (row, head) of x [rows, ld]; heads [0, n_heads) normalised with q_gamma,
 // [n_heads, n_heads + n_groups) with k_gamma (head_rmsnorm), the V heads copied unless y == x
 template <bool H>
@@ -400,6 +422,19 @@ int b2_rotary(void* qkv, const int32_t* pos, int batch, int n_heads, int n_group
   const int warps = batch * (n_heads + n_groups);
   B2_LAUNCH_CHECK("rotary", launch(rotary_kernel, dim3((warps + 3) / 4), dim3(128), 0, (cudaStream_t)stream, true,
                                    (__nv_bfloat16*)qkv, pos, batch, n_heads, n_groups, rope->rotary_dim, log2f(rope->base)));
+  return B2_OK;
+}
+
+int b2_rotary_table(void* qkv, const int32_t* pos, int batch, int n_heads, int n_groups, int head_size, const b2_rope_cfg* rope,
+                    const b2_rope_table* table, int ft, void* stream) {
+  if (!qkv || !pos || batch <= 0 || n_heads <= 0 || n_groups <= 0) return B2_ERR_PARAM;
+  if (int st = rope_table_check(rope, table)) return st;
+  if (head_size != 128 || (ft != B2_DT_BF16 && ft != B2_DT_F16) || !aligned(qkv, 8)) return B2_ERR_UNSUPPORTED;
+  const int warps = batch * (n_heads + n_groups);
+  const auto kern = ft == B2_DT_F16 ? rotary_table_kernel<true> : rotary_table_kernel<false>;
+  B2_LAUNCH_CHECK("rotary_table", launch(kern, dim3((warps + 3) / 4), dim3(128), 0, (cudaStream_t)stream, true, (__nv_bfloat16*)qkv,
+                                         pos, batch, n_heads, n_groups, rope->rotary_dim, table->inv_freq, table->stride,
+                                         table->attn_factor));
   return B2_OK;
 }
 

@@ -1085,6 +1085,12 @@ struct AppendNormParams : AppendParams {
   const __nv_bfloat16* k_gamma;
   float eps;
 };
+// The scaled-rotary form (cache_append_table_kernel) takes the caller's inverse-frequency table on top (b2_rope_table).
+struct AppendTableParams : AppendNormParams {
+  const float* inv_freq;  // fp32 rows of >= rotary_dim / 2 frequencies, 16-byte aligned
+  int64_t table_stride;   // floats between the rows of consecutive sequences; 0: one shared row
+  float attn_factor;
+};
 template <bool QKN>
 using AppendArgs = std::conditional_t<QKN, AppendNormParams, AppendParams>;
 
@@ -1104,8 +1110,9 @@ __device__ __forceinline__ void append_row(const AppendParams& p, int row, int& 
 
 // QKN: each q and k head row is first normalised (head_rmsnorm with q_gamma / k_gamma) and rounded to FT, like the
 // reference's QKLayerNormNoBeta writes an FT tensor for its Rotary; V rows are not.
-template <int QM, bool H, bool MT = false, bool TREE = false, bool QKN = false>
-__global__ void __launch_bounds__(128) cache_append_kernel(const AppendArgs<QKN> p) {
+// TAB: the rotary reads its frequencies from the caller's table (rope_from_table, always on) instead of computing them.
+template <int QM, bool H, bool MT, bool TREE, bool QKN, bool TAB, typename P>
+__device__ __forceinline__ void cache_append_warp(const P& p) {
   using F = Ft<H>;
   pdl_wait();
   pdl_launch_dependents();
@@ -1124,7 +1131,9 @@ __global__ void __launch_bounds__(128) cache_append_kernel(const AppendArgs<QKN>
     if (!is_v) head_rmsnorm<H>(x, slot < p.n_heads ? p.q_gamma : p.k_gamma, p.eps, lane);  // warp-uniform branch
   }
 
-  if (p.rope && !is_v) {
+  if constexpr (TAB) {
+    if (!is_v) rope_from_table<H>(x, pos, p.inv_freq + (size_t)b * p.table_stride, p.attn_factor, p.rotary_dim, lane);
+  } else if (p.rope && !is_v) {
     // NeoX rotate-half over the first rotary_dim dims: out[i] = x[i]cos - x[i+h]sin ; out[i+h] = x[i+h]cos + x[i]sin
     const int half = p.rotary_dim >> 1;
     float other[4];
@@ -1157,6 +1166,16 @@ __global__ void __launch_bounds__(128) cache_append_kernel(const AppendArgs<QKN>
   uint8_t* span = reinterpret_cast<uint8_t*>(tab[si]);
   const size_t rowi = (size_t)g * p.span_len + ps;
   store_row<QM, H>(span, rowi, p.n_groups * p.span_len, lane, x);
+}
+
+template <int QM, bool H, bool MT = false, bool TREE = false, bool QKN = false>
+__global__ void __launch_bounds__(128) cache_append_kernel(const AppendArgs<QKN> p) {
+  cache_append_warp<QM, H, MT, TREE, QKN, false>(p);
+}
+
+template <int QM, bool H, bool MT, bool TREE, bool QKN>
+__global__ void __launch_bounds__(128) cache_append_table_kernel(const AppendTableParams p) {
+  cache_append_warp<QM, H, MT, TREE, QKN, true>(p);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1488,12 +1507,17 @@ static int append_check(const b2_span_cfg* cfg, bool args_ok, int form, int q_le
 }
 
 // q_len rows per sequence (1 in the single-token form), the nodes of the draft tree `parents` in the tree form; norm: the
-// per-head Q/K RMSNorm before rotary (validated by the caller), or NULL
+// per-head Q/K RMSNorm before rotary (validated by the caller), or NULL; table: the rotary's frequencies (validated by the
+// caller, with rope), or NULL
 static int cache_append_launch(const b2_span_cfg* cfg, void* const* k_spans, void* const* v_spans, void* q_out, const void* qkv,
                                const int32_t* old_lens, const int32_t* parents, int form, int batch, int q_len,
-                               const b2_rope_cfg* rope, void* stream_, const b2_qk_norm* norm = nullptr) {
+                               const b2_rope_cfg* rope, void* stream_, const b2_qk_norm* norm = nullptr,
+                               const b2_rope_table* table = nullptr) {
   if (rope && (rope->rotary_dim != 128 && rope->rotary_dim != 64)) return B2_ERR_UNSUPPORTED;
-  AppendNormParams p;  // each kernel takes the base it needs (AppendArgs)
+  AppendTableParams p;  // each kernel takes the base it needs (AppendArgs)
+  p.inv_freq = table ? table->inv_freq : nullptr;
+  p.table_stride = table ? table->stride : 0;
+  p.attn_factor = table ? table->attn_factor : 1.f;
   p.q_gamma = norm ? (const __nv_bfloat16*)norm->q_gamma : nullptr;
   p.k_gamma = norm ? (const __nv_bfloat16*)norm->k_gamma : nullptr;
   p.eps = norm ? norm->eps : 0.f;
@@ -1512,6 +1536,7 @@ static int cache_append_launch(const b2_span_cfg* cfg, void* const* k_spans, voi
     return with_flag(cfg->ft == B2_DT_F16, [&](auto H) {
       return with_step_form(form, [&](auto MT, auto TREE) {
         return with_flag(norm != nullptr, [&](auto QKN) {
+          if (table) return launch(cache_append_table_kernel<QM, H, MT, TREE, QKN>, grid, block, 0, (cudaStream_t)stream_, true, p);
           return launch(cache_append_kernel<QM, H, MT, TREE, QKN>, grid, block, 0, (cudaStream_t)stream_, true, p);
         });
       });
@@ -1555,6 +1580,20 @@ int b2_span_cache_append_qknorm(const b2_span_cfg* cfg, void* const* k_spans, vo
   if (!norm || !norm->q_gamma || !norm->k_gamma) return B2_ERR_PARAM;
   if (((uintptr_t)norm->q_gamma & 7) || ((uintptr_t)norm->k_gamma & 7)) return B2_ERR_UNSUPPORTED;
   return cache_append_launch(cfg, k_spans, v_spans, q_out, qkv, old_lens, parents, form, batch, q_len, rope, stream_, norm);
+}
+
+int b2_span_cache_append_rope_table(const b2_span_cfg* cfg, void* const* k_spans, void* const* v_spans, void* q_out,
+                                    const void* qkv, const int32_t* old_lens, const int32_t* parents, int batch, int q_len,
+                                    const b2_rope_cfg* rope, const b2_rope_table* table, const b2_qk_norm* norm,
+                                    void* stream_) {
+  const int form = parents ? 2 : (q_len == 1 ? 0 : 1);
+  if (int st = append_check(cfg, k_spans && v_spans && q_out && qkv && old_lens && batch > 0, form, q_len)) return st;
+  if (cfg->head_size != kHead) return B2_ERR_UNSUPPORTED;  // head 64 (span_attn64.cu) has no table form
+  if (int st = rope_table_check(rope, table)) return st;
+  if (norm && (!norm->q_gamma || !norm->k_gamma)) return B2_ERR_PARAM;
+  if (norm && (((uintptr_t)norm->q_gamma & 7) || ((uintptr_t)norm->k_gamma & 7))) return B2_ERR_UNSUPPORTED;
+  return cache_append_launch(cfg, k_spans, v_spans, q_out, qkv, old_lens, parents, form, batch, q_len, rope, stream_, norm,
+                             table);
 }
 
 int b2_span_cache_compact(const b2_span_cfg* cfg, void* const* const* k_tables, void* const* const* v_tables, int n_layers,

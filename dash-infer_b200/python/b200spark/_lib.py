@@ -19,6 +19,7 @@ SYMBOLS = [
     "b2_span_cache_append_tree", "b2_span_attn_run_tree", "b2_spec_accept_tree", "b2_span_cache_compact",
     "b2_rmsnorm", "b2_rotary", "b2_binary", "b2_embedding", "b2_argmax", "b2_argmax_shard", "b2_argmax_merge", "b2_lens_add",
     "b2_rmsnorm_ft", "b2_binary_ft", "b2_argmax_ft", "b2_qk_rmsnorm", "b2_span_cache_append_qknorm",
+    "b2_rotary_table", "b2_span_cache_append_rope_table",
     "b2_logprobs", "b2_logprobs_partial_bytes", "b2_logprobs_shard", "b2_logprobs_merge",
     "b2_comm_create", "b2_comm_destroy", "b2_comm_buffer_bytes", "b2_comm_export", "b2_comm_connect", "b2_comm_connect_pointers",
     "b2_comm_local_buffer", "b2_comm_error", "b2_allreduce", "b2_allgather", "b2_gemm_wq_run_allreduce",
@@ -48,6 +49,10 @@ class RopeCfg(C.Structure):
 
 class QkNorm(C.Structure):
     _fields_ = [("q_gamma", C.c_void_p), ("k_gamma", C.c_void_p), ("eps", C.c_float), ("reserved", C.c_int32)]
+
+
+class RopeTable(C.Structure):
+    _fields_ = [("inv_freq", C.c_void_p), ("stride", C.c_int64), ("attn_factor", C.c_float), ("reserved", C.c_int32)]
 
 
 DT_F32, DT_F16, DT_I8, DT_BF16, DT_U8 = 1, 2, 3, 9, 10
@@ -107,6 +112,9 @@ def _load():
         "b2_span_cache_compact": (i32, [C.POINTER(SpanCfg), vp, vp, i32, vp, vp, vp, i32, i32, vp]),
         "b2_span_cache_append_qknorm": (i32, [C.POINTER(SpanCfg), vp, vp, vp, vp, vp, vp, i32, i32, C.POINTER(RopeCfg),
                                               C.POINTER(QkNorm), vp]),
+        "b2_span_cache_append_rope_table": (i32, [C.POINTER(SpanCfg), vp, vp, vp, vp, vp, vp, i32, i32, C.POINTER(RopeCfg),
+                                                  C.POINTER(RopeTable), C.POINTER(QkNorm), vp]),
+        "b2_rotary_table": (i32, [vp, vp, i32, i32, i32, i32, C.POINTER(RopeCfg), C.POINTER(RopeTable), i32, vp]),
         "b2_qk_rmsnorm": (i32, [vp, vp, i32, i64, i32, i32, i32, C.POINTER(QkNorm), i32, vp]),
         "b2_rmsnorm": (i32, [vp, vp, vp, i32, i32, f32, vp]),
         "b2_rmsnorm_ft": (i32, [vp, vp, vp, i32, i32, f32, i32, vp]),

@@ -32,6 +32,9 @@ class ModelConfig:
     eps: float = 1e-6
     qkv_bias: bool = True
     qk_norm: bool = False  # Qwen3: per-head RMSNorm of the q and k heads before rotary (QKLayerNormNoBeta), head 128 only
+    # a Hugging Face rope_scaling entry (ops.rope_table: linear, yarn, llama3), applied statically: one frequency table for
+    # every position and sequence; None: the unscaled rotary (rope_base^(-2f / head)).  Head 128 only.
+    rope_scaling: dict | None = None
 
 
 QWEN2_7B = ModelConfig("Qwen2-7B", 3584, 28, 4, 18944, 28, 152064)
@@ -43,6 +46,13 @@ TINY = ModelConfig("tiny-2L", 512, 8, 2, 1024, 2, 1024)
 # explicitly — n_heads * head differs from hidden for 0.6B (16 x 128 = 2048 against 1024), so o_proj's K is not hidden
 QWEN3_8B = ModelConfig("Qwen3-8B", 4096, 32, 8, 12288, 36, 151936, qkv_bias=False, qk_norm=True)
 QWEN3_06B = ModelConfig("Qwen3-0.6B", 1024, 16, 8, 3072, 28, 151936, qkv_bias=False, qk_norm=True)  # full-depth parity anchor
+# Long-context rotary scaling as the published model cards enable it.  Qwen2.5 / Qwen3 reach 131072 tokens with YaRN over
+# their native 32768; a Qwen3 stack turns it on with dataclasses.replace(QWEN3_8B, rope_scaling=YARN_4X_32K).
+YARN_4X_32K = {"rope_type": "yarn", "factor": 4.0, "original_max_position_embeddings": 32768}
+QWEN25_7B = ModelConfig("Qwen2.5-7B", 3584, 28, 4, 18944, 28, 152064, rope_scaling=YARN_4X_32K)
+LLAMA31_8B = ModelConfig("Llama-3.1-8B", 4096, 32, 8, 14336, 32, 128256, rope_base=5e5, eps=1e-5, qkv_bias=False,
+                         rope_scaling={"rope_type": "llama3", "factor": 8.0, "low_freq_factor": 1.0, "high_freq_factor": 4.0,
+                                       "original_max_position_embeddings": 8192})
 
 KV_MODES = {"none": KV_NONE, "bf16": KV_NONE, "i8": KV_I8, "u4": KV_U4, "fp8": KV_FP8}
 
@@ -151,6 +161,7 @@ class DecodeStack:
             "multi-token steps: q_len <= 16, single GPU, head size 128"
         assert not tree or (q_len > 1 and tp_size == 1 and cfg.head == 128), "draft trees: q_len > 1, single GPU, head size 128"
         assert not cfg.qk_norm or cfg.head == 128, "per-head Q/K norm: head size 128"
+        assert cfg.rope_scaling is None or cfg.head == 128, "rope scaling: head size 128"
         assert 0 <= logprobs <= ops._lib.MAX_TOP_LOGPROBS, "logprobs: 0 .. 10 alternatives"
         self.logprobs = logprobs
         self.dtype = _DT = dtype
@@ -209,7 +220,9 @@ class DecodeStack:
                                    shard=("cols", TP.col_range_even(cfg.vocab, r, tp)) if tp > 1 else None)
         self.attn = ops.SpanAttn(self.layers[0]["cache"].cfg, rows)
         self.ws = ops.Workspace(device)
-        self.rope = (cfg.rope_base, hd)
+        # rope scaling: one fp32 frequency table on the device, shared by every layer and sequence (every TP rank builds the
+        # same one); without it the append computes base^(-2f / head) itself, as before
+        self.rope = (cfg.rope_base, hd) if cfg.rope_scaling is None else ops.rope_table(cfg.rope_scaling, cfg.rope_base, hd, device)
         # device-resident step state, allocated for the construction batch; set_batch() re-views it for a smaller batch
         self.Bmax = batch
         self._lens_old = torch.zeros(batch, dtype=torch.int32, device=device)

@@ -8,7 +8,7 @@ import torch
 
 from . import _lib
 from ._lib import (ACT_NONE, BIN_ADD, BIN_MUL, DT_BF16, DT_I8, DT_U8, KV_I8, KV_NONE, KV_U4, GemmDesc, GemmFuse, QkNorm, RopeCfg,
-                   SpanCfg, check, lib)
+                   RopeTable, SpanCfg, check, lib)
 
 
 def _stream():
@@ -259,19 +259,113 @@ def qk_rmsnorm(x, n_heads, n_groups, q_gamma, k_gamma, eps=1e-6, out=None):
     return out
 
 
+def rope_table(scaling, base, rotary_dim, device=None):
+    """Inverse frequencies and attention factor of a Hugging Face `rope_scaling` entry: (inv_freq fp32 [rotary_dim / 2],
+    attn_factor), for the table form of the rotary (b2_rope_table: rope=(inv_freq, attn_factor) in _cache_append,
+    table=... in rotary).  Computed in fp64 and rounded to fp32 once.  With d = rotary_dim, f = 0 .. d/2 - 1 and
+    theta_f = base^(-2f / d) (the unscaled frequencies):
+
+    None, {"rope_type": "default"}: inv_f = theta_f, attn_factor 1.
+    linear (factor s): inv_f = theta_f / s.
+    yarn (factor s, original_max_position_embeddings L; beta_fast 32, beta_slow 1, attention_factor, mscale,
+      mscale_all_dim, truncate optional, as in transformers' _compute_yarn_parameters):
+        corr(r) = d ln(L / (2 pi r)) / (2 ln base);  low = floor(corr(beta_fast)), high = ceil(corr(beta_slow)) (no
+        floor / ceil with truncate False), clamped to low >= 0, high <= d - 1;
+        ramp_f = clamp((f - low) / (high - low), 0, 1) (high += 0.001 when high == low);  e_f = 1 - ramp_f;
+        inv_f = (theta_f / s) (1 - e_f) + theta_f e_f
+      so frequencies below low keep theta_f and those from high on are interpolated by s.  attn_factor = the dict's
+      attention_factor, else mscale(s, mscale) / mscale(s, mscale_all_dim) when both are given, else mscale(s) with
+      mscale(s, m=1) = 0.1 m ln(s) + 1 (1 for s <= 1).
+    llama3 (factor s, low_freq_factor a, high_freq_factor c, original_max_position_embeddings L):
+        wavelength w_f = 2 pi / theta_f;  w_f > L / a: inv_f = theta_f / s;  w_f < L / c: inv_f = theta_f;  between:
+        g = (L / w_f - a) / (c - a), inv_f = (1 - g) theta_f / s + g theta_f.   attn_factor 1.
+    Any other type (dynamic NTK among them) raises ValueError: the decode stack applies one static table to every
+    position, and dynamic scaling would rotate cached keys and the current query with different frequencies."""
+    import math
+    d = int(rotary_dim)
+    assert d > 0 and d % 2 == 0
+    theta = float(base) ** (-torch.arange(0, d // 2, dtype=torch.float64) * 2.0 / d)
+    sc = dict(scaling or {})
+    kind = sc.get("rope_type", sc.get("type", "default"))
+    af = 1.0
+    if kind == "default":
+        inv = theta
+    elif kind == "linear":
+        inv = theta / float(sc["factor"])
+    elif kind == "yarn":
+        s, L = float(sc["factor"]), float(sc["original_max_position_embeddings"])
+        fast, slow = float(sc.get("beta_fast") or 32), float(sc.get("beta_slow") or 1)
+
+        def corr(r):
+            return d * math.log(L / (r * 2 * math.pi)) / (2 * math.log(base))
+
+        low, high = corr(fast), corr(slow)
+        if sc.get("truncate", True):
+            low, high = math.floor(low), math.ceil(high)
+        low, high = max(low, 0), min(high, d - 1)
+        if low == high:
+            high += 0.001
+        ramp = ((torch.arange(d // 2, dtype=torch.float64) - low) / (high - low)).clamp(0, 1)
+        e = 1 - ramp
+        inv = (theta / s) * (1 - e) + theta * e
+
+        def mscale(x, m=1.0):
+            return 1.0 if x <= 1 else 0.1 * m * math.log(x) + 1.0
+
+        if sc.get("attention_factor") is not None:
+            af = float(sc["attention_factor"])
+        elif sc.get("mscale") and sc.get("mscale_all_dim"):
+            af = mscale(s, float(sc["mscale"])) / mscale(s, float(sc["mscale_all_dim"]))
+        else:
+            af = mscale(s)
+    elif kind == "llama3":
+        s, a, c = float(sc["factor"]), float(sc["low_freq_factor"]), float(sc["high_freq_factor"])
+        L = float(sc["original_max_position_embeddings"])
+        w = 2 * math.pi / theta
+        g = (L / w - a) / (c - a)
+        inv = torch.where(w > L / a, theta / s, torch.where(w < L / c, theta, (1 - g) * theta / s + g * theta))
+    else:
+        raise ValueError(f"rope_table: unsupported rope scaling type {kind!r} (default, linear, yarn, llama3)")
+    inv = inv.to(torch.float32)
+    return (inv.to(device) if device is not None else inv), float(af)
+
+
+def _rope_table(rope, rows, device):
+    """(inv_freq, attn_factor) -> (RopeCfg, RopeTable): inv_freq fp32 [rotary_dim / 2] (one row shared by every sequence) or
+    [rows, >= rotary_dim / 2] (row b for sequence b, stride inv_freq.stride(0)) on the activations' device"""
+    inv, af = rope
+    assert inv.dtype == torch.float32 and inv.device == device and inv.stride(-1) == 1, \
+        "rope table: fp32 inverse frequencies on the activations' device"
+    if inv.dim() == 1:
+        rd, stride = 2 * inv.shape[0], 0
+    else:
+        assert inv.dim() == 2 and inv.shape[0] == rows, "rope table: [rotary_dim / 2] or one row per sequence"
+        rd, stride = 2 * inv.shape[1], inv.stride(0)
+    return RopeCfg(0.0, int(rd), 0), RopeTable(inv.data_ptr(), int(stride), float(af), 0)
+
+
 def _cache_append(cache, qkv, old_lens, q_out=None, rope=None, q_len=None, parents=None, qk_norm=None):
     """Append one step's rows to the span cache (+ optional fused rotary).  q_len None: row b of qkv is sequence b, written at
     position old_lens[b].  q_len: row b*q_len + t is token t of sequence b, written at position old_lens[b] + t; with parents
     (int32 [B, q_len]) it is node t of sequence b's draft tree, written at slot old_lens[b] + t with rotary position
     old_lens[b] + depth(t).  qk_norm = (q_gamma, k_gamma, eps): the per-head Q/K RMSNorm before rotary
-    (b2_span_cache_append_qknorm), every step form."""
+    (b2_span_cache_append_qknorm), every step form.  rope = (base, rotary_dim): the rotary with base^(-2f / rotary_dim);
+    rope = (inv_freq tensor, attn_factor): the scaled rotary from a frequency table (rope_table; one row, or one row per
+    sequence) in every step form, with or without qk_norm (b2_span_cache_append_rope_table)."""
     cfg = cache.cfg
     rows = qkv.shape[0]
     assert rows % (q_len or 1) == 0 and (parents is None or (q_len and parents.dtype == torch.int32 and parents.is_contiguous()))
     if q_out is None:
         q_out = torch.empty(rows, cfg.n_heads * cfg.head_size, dtype=qkv.dtype, device=qkv.device)
-    r = RopeCfg(float(rope[0]), int(rope[1]), 0) if rope is not None else None
     head = (C.byref(cfg), _ptr(cache.k_tab), _ptr(cache.v_tab), _ptr(q_out), _ptr(qkv), _ptr(old_lens))
+    if rope is not None and isinstance(rope[0], torch.Tensor):
+        r, tab = _rope_table(rope, rows // (q_len or 1), qkv.device)
+        nrm = _qk_norm(qk_norm, qkv.dtype, qkv.device) if qk_norm is not None else None
+        check(lib.b2_span_cache_append_rope_table(*head, _ptr(parents), rows // (q_len or 1), int(q_len or 1), C.byref(r),
+                                                  C.byref(tab), C.byref(nrm) if nrm is not None else None, _stream()),
+              "b2_span_cache_append_rope_table")
+        return q_out
+    r = RopeCfg(float(rope[0]), int(rope[1]), 0) if rope is not None else None
     tail = (C.byref(r) if r is not None else None, _stream())
     if qk_norm is not None:
         nrm = _qk_norm(qk_norm, qkv.dtype, qkv.device)
@@ -438,7 +532,15 @@ def quant_fp8(x, gamma=None, eps=1e-6, out=None):
     return out
 
 
-def rotary(qkv, pos, n_heads, n_groups, base=1e6, rotary_dim=128):
+def rotary(qkv, pos, n_heads, n_groups, base=1e6, rotary_dim=128, table=None):
+    """In-place NeoX rotary of the q and k heads of qkv [rows, (n_heads + 2 n_groups) * 128] at positions pos [rows].
+    table = (inv_freq, attn_factor) (rope_table; [rotary_dim / 2], or [rows, >= rotary_dim / 2] with row b for qkv row b):
+    the scaled form b2_rotary_table, bf16 or fp16, base and rotary_dim unused; otherwise b2_rotary, bf16 only."""
+    if table is not None:
+        r, tab = _rope_table(table, qkv.shape[0], qkv.device)
+        check(lib.b2_rotary_table(_ptr(qkv), _ptr(pos), qkv.shape[0], n_heads, n_groups, 128, C.byref(r), C.byref(tab), _ft(qkv),
+                                  _stream()), "b2_rotary_table")
+        return qkv
     if qkv.dtype != torch.bfloat16:  # b2_rotary is bf16 only (fp16 models rotate in the fused cache append)
         raise TypeError(f"rotary: qkv must be bfloat16, got {qkv.dtype}")
     r = RopeCfg(float(base), int(rotary_dim), 0)

@@ -28,6 +28,8 @@
  *                           csrc/core/kernel/cuda/layernorm.cu:86, rotary.cu:23, binary.cu
  *   b2_qk_rmsnorm, b2_span_cache_append_qknorm
  *                         QKLayerNormNoBeta (Qwen3, qwen_v30.py)  csrc/core/kernel/cuda/layernorm.cu:259-304
+ *   b2_rotary_table, b2_span_cache_append_rope_table
+ *                         Rotary with a [batch, head/2] inverse-frequency table  kernel/cuda/rotary.cu:24-80 (static tables)
  */
 #ifndef B200SPARK_H_
 #define B200SPARK_H_
@@ -302,6 +304,34 @@ int b2_span_cache_append_qknorm(const b2_span_cfg* cfg, void* const* k_spans, vo
                                 const void* qkv, const int32_t* old_lens, const int32_t* parents, int batch, int q_len,
                                 const b2_rope_cfg* rope, const b2_qk_norm* norm, void* stream);
 
+/* ---- Scaled rotary (YaRN, Llama-3.1 "llama3", linear, or any other per-frequency scaling): the rotary reads its inverse
+ * frequencies from a caller-given table instead of computing base^(-2f / rotary_dim).  The table IS the caller's definition
+ * of the scaling: the library never computes frequencies for this form (b200spark.ops.rope_table builds the published
+ * Hugging Face tables on the host).  Head 128 only.  With half = rotary_dim / 2 and, for row b, inv = inv_freq + b * stride
+ * (stride 0: one row shared by every sequence; otherwise one row per sequence, the [batch, rotary_dim / 2] layout of the
+ * reference's Rotary op), each q and k head dim d < rotary_dim, f = d % half, is computed in fp32 as
+ *   ang = fl32(pos * inv[f]);  sn, cs = sincosf(ang);  c = fl32(cs * attn_factor);  s = fl32(sn * attn_factor);
+ *   d < half:  t = fl32(x[d + half] * s),  y = FT(fma(x[d], c, -t));
+ *   d >= half: t = fl32(x[d - half] * s),  y = FT(fma(x[d], c, t)),   one FT rounding.
+ * attn_factor is YaRN's mscale (Hugging Face scales the cos / sin caches, so both q and k); 1.0 leaves cs and sn unchanged. */
+typedef struct {
+  const float* inv_freq; /* fp32 [rows][stride] (>= rotary_dim / 2 per row), device, 16-byte aligned, stride % 4 == 0 */
+  int64_t stride;        /* floats between the rows of consecutive sequences; 0 = one shared row */
+  float attn_factor;
+  int32_t reserved;
+} b2_rope_table;
+/* b2_span_cache_append / _tokens / _tree (parents and q_len as b2_span_cache_append_qknorm) with the rotary at the same
+ * positions (old_lens[b] + t, or old_lens[b] + depth(t) in the tree form) computed from the table; the row of token (b, t)
+ * is the table row of sequence b.  norm: the per-head Q/K RMSNorm before the rotary, or NULL.  The span bytes, {zero, scale}
+ * and q_out equal those of b2_rotary_table (same table, per-token rows) followed by the entry point without rotary, bit for
+ * bit.  Errors: NULL rope, table or inv_freq, stride < 0, or 0 < stride < rotary_dim / 2: B2_ERR_PARAM; inv_freq not
+ * 16-byte aligned or stride % 4 != 0, rotary_dim other than 128 or 64, head_size != 128: B2_ERR_UNSUPPORTED; norm as in
+ * b2_span_cache_append_qknorm; q_len and batch as the other appends.  rope->base is not read. */
+int b2_span_cache_append_rope_table(const b2_span_cfg* cfg, void* const* k_spans, void* const* v_spans, void* q_out,
+                                    const void* qkv, const int32_t* old_lens, const int32_t* parents, int batch, int q_len,
+                                    const b2_rope_cfg* rope, const b2_rope_table* table, const b2_qk_norm* norm,
+                                    void* stream);
+
 /* =====================================================================================
  * Glue ops of the decode graph ("next" rows): element-wise / norm / lookup, FT = bf16.
  * ===================================================================================== */
@@ -318,6 +348,10 @@ int b2_argmax_ft(int64_t* ids_out, float* vals_out /* or NULL */, const void* lo
 /* in-place NeoX rotary on the q and k heads of qkv [batch, (nH+2nG)*head]; position = pos[b] */
 int b2_rotary(void* qkv, const int32_t* pos, int batch, int n_heads, int n_groups, int head_size,
               const b2_rope_cfg* rope, void* stream);
+/* b2_rotary with the frequencies of a b2_rope_table (arithmetic and errors there; row b of qkv uses inv_freq + b * stride),
+ * in place, ft = B2_DT_BF16 or B2_DT_F16 (else B2_ERR_UNSUPPORTED); V heads and dims >= rotary_dim are left as they are. */
+int b2_rotary_table(void* qkv, const int32_t* pos, int batch, int n_heads, int n_groups, int head_size,
+                    const b2_rope_cfg* rope, const b2_rope_table* table, int ft, void* stream);
 /* QKLayerNormNoBeta (arithmetic: b2_qk_norm): x, y [rows, ld] FT.  Per row, heads [0, n_heads) and [n_heads,
  * n_heads + n_groups) are normalised; the V heads [n_heads + n_groups, n_heads + 2 n_groups) are copied unless y == x; the
  * columns beyond are untouched.  y may be x (any other overlap is undefined).  head_size 128 and ft B2_DT_BF16 / B2_DT_F16
