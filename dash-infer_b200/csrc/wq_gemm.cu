@@ -776,6 +776,7 @@ struct b2_gemm_wq {
   unsigned* counters = nullptr;
   Plan plans[2];  // MT = 1, 2
   int tc_grid = 0, tc_rounds = 0, tc_S = 1, tc_h = 0;  // schedule of the wgmma path (TcSched; tc_grid 0 = not planned)
+  bool tc_cluster = false;                             // its k-slices run as clusters (TcParams::cluster)
   bool pair = false;  // gate/up pair image (SwiGLU epilogue): physical channels = 2 * N
   int device = 0;
 };
@@ -1041,6 +1042,10 @@ static bool use_tc(const b2_gemm_wq* h, int M) {
 // near KT / 2, a head on CTA b < NR and a tail on CTA NR + b: the gate+up pair's 296 n-groups (132 SMs) run 2 rounds plus
 // 28 tiles on 64 CTAs instead of 3 rounds on 32.  The tail continues the head's accumulator chain, so the results are those
 // of whole n-groups bit for bit.  B2_GEMM_TC_MAX_SPLIT=1 splits no n-group.
+// The S k-slices of an n-group run as one thread-block cluster when all NG clusters are resident at once (one wave; the
+// occupancy query knows how the SMs fall into GPCs): their partial tiles then meet in distributed shared memory, in the
+// same order as through the workspace, so the results do not depend on the choice.  B2_GEMM_TC_CLUSTER=0 keeps the
+// workspace path.  The workspace stays sized for that path, so its size is a function of the schedule alone.
 static void make_tc_plan(b2_gemm_wq* h) {
   if (h->tc_grid > 0) return;
   const int sms = sm_count(), NG = h->NG, KT = h->KT;
@@ -1050,6 +1055,7 @@ static void make_tc_plan(b2_gemm_wq* h) {
     h->tc_grid = NG * h->tc_S;
     h->tc_rounds = 0;
     h->tc_h = 0;
+    h->tc_cluster = h->tc_S > 1 && env_int("B2_GEMM_TC_CLUSTER", 1) && tc_clusters_fit(h->d.wbits, h->tc_S, NG);
     return;
   }
   const int NR = NG % sms;
@@ -1074,7 +1080,7 @@ static int run_tc(b2_gemm_wq* h, TcParams p, int M, cudaStream_t stream) {
   if ((h->tc_S > 1 || h->tc_h > 0) && !p.ws) return B2_ERR_PARAM;
   p.packed = (const uint8_t*)h->packed; p.sz = h->sz; p.counters = h->counters;
   p.N = h->d.N; p.K = h->d.K; p.Np = h->Np; p.KT = h->KT; p.NG = h->NG;
-  p.grid = h->tc_grid; p.rounds = h->tc_rounds; p.S = h->tc_S; p.h = h->tc_h;
+  p.grid = h->tc_grid; p.rounds = h->tc_rounds; p.S = h->tc_S; p.h = h->tc_h; p.cluster = h->tc_cluster ? 1 : 0;
   const int64_t a_row = p.a_scale ? p.lda : 2 * p.lda;  // bytes per activation row (fp8: lda counts bytes)
   for (int m0 = 0; m0 < M; m0 += kTcMaxM) {
     TcParams q = p;
@@ -1121,6 +1127,12 @@ size_t b2_gemm_wq_algo_bytes(b2_gemm_wq_t h, int M) {
 }
 
 int b2_gemm_wq_sumsq_parts(b2_gemm_wq_t h) { return h ? h->NG : 0; }
+
+int b2_gemm_wq_tc_cluster(b2_gemm_wq_t h) {
+  if (!h) return 0;
+  make_tc_plan(h);
+  return h->tc_cluster ? h->tc_S : 1;
+}
 
 int b2_gemm_wq_run(b2_gemm_wq_t h, const void* A, int64_t lda, void* C, int64_t ldc, int M, const void* bias,
                    const void* residual, int activation, float alpha, void* workspace, size_t workspace_bytes,

@@ -64,6 +64,8 @@ struct TcParams {
   unsigned* counters;
   int M, N, K, Np, KT, NG;
   int grid, rounds, S, h;  // the work schedule (TcSched)
+  int cluster = 0;         // 1: the S k-slices of an n-group are one thread-block cluster and sum their partial tiles over
+                           // distributed shared memory (rounds == 0 only; launched by tc_launch as clusters of S CTAs)
   int act;
   float alpha;
   // fp8 activations (A8 instantiation): A is fp8-e4m3 in the b2 fp8 activation layout (lda in bytes), per-token scale [M] and
@@ -87,8 +89,8 @@ struct TcParams {
 };
 
 // The wgmma kernel's work schedule (planned by make_tc_plan, walked by wq_gemm_tc_kernel).  While there are at most as many
-// n-groups as CTAs, CTA b takes k-slice b % S of n-group b / S (S equal slices; the last slice to arrive sums the partials in
-// slice order).  Otherwise each of the grid CTAs takes `rounds` whole n-groups, b + j * grid, and each of the NR = NG - nfull
+// n-groups as CTAs, CTA b takes k-slice b % S of n-group b / S (S equal slices; the partials are summed in slice order by
+// the last slice to arrive, or, when the S slices are one cluster, by every slice for its share of the rows).  Otherwise each of the grid CTAs takes `rounds` whole n-groups, b + j * grid, and each of the NR = NG - nfull
 // n-groups left over is cut in two at k-tile h: CTA b < NR runs the head [0, h) of n-group nfull + b first and parks its
 // raw accumulators; CTA NR + b runs the tail [h, KT) last, starting from them, so every output is the one k-ordered fp32
 // chain of a whole n-group, bit for bit.  A tail that starts before its head has parked runs the whole n-group instead: no
@@ -146,6 +148,8 @@ constexpr int kGemvMaxM = 16;  // batch rows per launch of the mma.sync GEMV ker
 constexpr int kTcMaxM = 64;    // batch rows per wgmma launch
 // sets p.nm; fp16: activations / outputs / bias / residual are fp16 (else bf16)
 cudaError_t tc_launch(int wbits, bool fp16, TcParams p, cudaStream_t stream);
+// whether `clusters` thread-block clusters of S wgmma CTAs are resident at once (one wave) on this device
+bool tc_clusters_fit(int wbits, int S, int clusters);
 
 // Raise a kernel's dynamic shared-memory opt-in to smem, never lower it: an instantiation is shared by handles whose plans
 // need different amounts, and a later handle with a smaller need must not lower the limit under an earlier one's launches.

@@ -19,8 +19,11 @@
 //                 B descriptor reads (out-of-range rows/columns are zero-filled by the TMA unit)
 //   warps 10..11: per-row sums sum_k a[m][k] needed by the zero-point term, read from the landed tiles
 //   epilogue    : the consumers apply s * (acc - (16+z) * sum a) to their accumulators and park the fp32 tile in the drained
-//                 activation ring; then ALL 384 threads do the split-K partial store / last-CTA reduction and the final
-//                 alpha/bias/activation/residual (or SwiGLU) with 16-byte reads and 8-byte bf16x4 stores.
+//                 activation ring; then ALL 384 threads do the split-K reduction and the final alpha/bias/activation/residual
+//                 (or SwiGLU) with 16-byte reads and 8-byte bf16x4 stores.  The k-slices of an n-group are one thread-block
+//                 cluster where they fit in one wave: each CTA sums its share of the rows over the slices' parked tiles
+//                 through distributed shared memory and finishes those rows; else every slice stores its partial tile to
+//                 the workspace and the last to arrive sums and finishes the whole tile.
 //   schedule    : one CTA per SM; the launch's tiles are spread evenly over them (TcSched, wq_gemm_shared.cuh): whole
 //                 n-groups in rounds while there are more n-groups than CTAs (MULTI instantiation: gate+up pair, lm_head),
 //                 each n-group left over cut in two k-ordered halves on two CTAs, the second starting from the first's
@@ -45,6 +48,7 @@ constexpr int kTcNM = 64;            // batch columns per MMA (wgmma N)
 constexpr int kTcNSW = 6;            // weight stages (16 KB each): ~2 us of HBM latency x 25 GB/s/SM needs >= 50 KB in flight
 constexpr int kTcNSX = 3;            // activation stages (32 or 16 KB each)
 constexpr int kTcXTile = kTcNM * 128;  // bytes: NM rows x 64 k bf16
+constexpr int kTcMaxCluster = 8;     // k-slices of a cluster split: the portable cluster size limit
 
 // ---- wgmma wrappers (PTX ISA 8.0, sm_90a): A from registers, B from a shared-memory descriptor, D in registers ----
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
@@ -504,12 +508,16 @@ __global__ void __launch_bounds__(kTcThreads, 1) wq_gemm_tc_kernel(const TcParam
   // ======================= epilogue: all threads =======================
   pdl_wait();  // workspace / counters / C belong to the previous kernels until here
   __syncthreads();  // tile parked
+  const bool cl = !MULTI && p.cluster;
   {
     constexpr int T = kTcThreads;
     const float4* fs4 = reinterpret_cast<const float4*>(xring);
     float4* fs4w = reinterpret_cast<float4*>(xring);
     const int units = p.M * (kBN / 4);  // float4 units, index = m * 32 + nq
     constexpr int MPK4 = kTcNM * kBN / 4;
+    // the tile rows this CTA finishes: r0, r0 + rs, ... (the slices of a cluster share them out; else all of them)
+    const int r0 = cl ? sg.part : 0, rs = cl ? sg.parts : 1;
+    const int rows = (p.M - r0 + rs - 1) / rs;
     bool finalize = true;
     if (MULTI && sg.carry == 1) {  // a head: accumulators and row sums to the workspace, then count its arrival
       float4* dst = reinterpret_cast<float4*>(p.ws + (size_t)(ng - sch.nfull) * kTcCarryFloats);
@@ -518,6 +526,28 @@ __global__ void __launch_bounds__(kTcThreads, 1) wq_gemm_tc_kernel(const TcParam
       __syncthreads();
       if (tid == 0 && atomicAdd(&p.counters[ng], 1u) == 1u) p.counters[ng] = 0;  // the tail ran whole already: re-arm
       finalize = false;
+    } else if (cl) {
+      // split-K inside the cluster: after one cluster barrier every slice's tile is parked.  Each CTA sums its rows over the
+      // S slices through distributed shared memory, from +0 in slice order (the order of the workspace path below, so the
+      // results are the same bit for bit), in place in its own tile — a peer reads only its own rows there — and finishes
+      // them.  No workspace round trip, fence or ticket, and the epilogue of a tile is spread over its S SMs.
+      cluster_arrive();
+      cluster_wait();
+      const uint32_t fs_a = smem_u32(xring);
+      for (int u = tid; u < rows * 32; u += T) {
+        const int i = ((u >> 5) * rs + r0) * 32 + (u & 31);
+        float4 b[kTcMaxCluster];
+#pragma unroll
+        for (int r = 0; r < kTcMaxCluster; ++r)
+          if (r < sg.parts) b[r] = ld_dsmem_f4(dsmem_addr(fs_a + i * 16, r));
+        float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+        for (int r = 0; r < kTcMaxCluster; ++r)
+          if (r < sg.parts) { a.x += b[r].x; a.y += b[r].y; a.z += b[r].z; a.w += b[r].w; }
+        fs4w[i] = a;
+      }
+      cluster_arrive();  // done with the peers' tiles; the matching wait is below, so no CTA leaves while a peer reads it
+      __syncthreads();
     } else if (sg.parts > 1) {  // k-slice sg.part of sg.parts: partial tile to slot ng * S + part
       const size_t slots = (size_t)ng * p.S;
       float4* wsu = reinterpret_cast<float4*>(p.ws) + (slots + sg.part) * MPK4;
@@ -566,10 +596,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) wq_gemm_tc_kernel(const TcParam
       const bool vec_ok = (p.ldc & 3) == 0 && (reinterpret_cast<uintptr_t>(p.C) & 7) == 0;
       if (p.act == B2_ACT_SWIGLU) {
         // tile = [64 gate | 64 up] channels: out[m, 64*ng + c] = silu(gate) * up; unit = 4 outputs
-        const int su = p.M * 16;
+        const int su = rows * 16;
 #pragma unroll 1
-        for (int i = tid; i < su; i += T) {
-          const int m = i >> 4, nq = i & 15;
+        for (int u = tid; u < su; u += T) {
+          const int m = (u >> 4) * rs + r0, nq = u & 15;
           const int nn = ng * 64 + nq * 4;
           if (nn >= p.N) continue;
           const float4 gv = fs4[m * 32 + nq], uv = fs4[m * 32 + 16 + nq];
@@ -592,20 +622,21 @@ __global__ void __launch_bounds__(kTcThreads, 1) wq_gemm_tc_kernel(const TcParam
                  (!p.bias || (reinterpret_cast<uintptr_t>(p.bias) & 7) == 0)) {
         // the decode-path case: no activation; all residual loads of a thread are issued before the first use
         constexpr int UPT = (kTcNM * (kBN / 4) + T - 1) / T;  // units per thread (6)
+        const int ul = rows * 32;                              // this CTA's units: u -> row (u >> 5) * rs + r0
         uint2 res[UPT];
 #pragma unroll
         for (int j = 0; j < UPT; ++j) {
-          const int i = tid + j * T;
-          const int m = i >> 5, nn = ng * kBN + (i & 31) * 4;
+          const int u = tid + j * T;
+          const int m = (u >> 5) * rs + r0, nn = ng * kBN + (u & 31) * 4;
           res[j] = make_uint2(0u, 0u);
-          if (p.residual && i < units && nn < p.N) res[j] = __ldg(reinterpret_cast<const uint2*>(p.residual + (int64_t)m * p.ldc + nn));
+          if (p.residual && u < ul && nn < p.N) res[j] = __ldg(reinterpret_cast<const uint2*>(p.residual + (int64_t)m * p.ldc + nn));
         }
 #pragma unroll
         for (int j = 0; j < UPT; ++j) {
-          const int i = tid + j * T;
-          const int m = i >> 5, nn = ng * kBN + (i & 31) * 4;
+          const int u = tid + j * T;
+          const int m = (u >> 5) * rs + r0, i = m * 32 + (u & 31), nn = ng * kBN + (u & 31) * 4;
           float ssq = 0.f;
-          if (i < units && nn < p.N) {
+          if (u < ul && nn < p.N) {
             const float4 a = fs4[i];
             float v0 = a.x * p.alpha, v1 = a.y * p.alpha, v2 = a.z * p.alpha, v3 = a.w * p.alpha;
             if (p.bias) {
@@ -626,15 +657,15 @@ __global__ void __launch_bounds__(kTcThreads, 1) wq_gemm_tc_kernel(const TcParam
           if (p.xg_out) {  // a warp holds the 32 four-column units of one row (384 = 12 x 32): fixed-order lane reduction
 #pragma unroll
             for (int o = 16; o > 0; o >>= 1) ssq += __shfl_xor_sync(0xffffffffu, ssq, o);
-            if (lane == 0 && i < units) p.sumsq_out[(size_t)ng * p.norm_ld + m] = ssq;
+            if (lane == 0 && u < ul) p.sumsq_out[(size_t)ng * p.norm_ld + m] = ssq;
           }
         }
       } else {
         // generic: any activation / alignment (rolled on purpose: the inlined activation switch is large)
         const float* fs = reinterpret_cast<const float*>(xring);
 #pragma unroll 1
-        for (int i = tid; i < p.M * (kBN / 2); i += T) {
-          const int m = i >> 6, np = i & 63;
+        for (int u = tid; u < rows * (kBN / 2); u += T) {
+          const int m = (u >> 6) * rs + r0, np = u & 63;
           const int nn = ng * kBN + np * 2;
           if (nn >= p.N) continue;
           float v0 = fs[m * kBN + np * 2] * p.alpha, v1 = fs[m * kBN + np * 2 + 1] * p.alpha;
@@ -661,6 +692,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) wq_gemm_tc_kernel(const TcParam
       }
     }
   }
+  if (cl) cluster_wait();  // the peers are done reading this CTA's tile
 
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy tile writes before the next segment's TMA writes
   __syncthreads();  // the tile in the X ring is free again
@@ -679,6 +711,33 @@ static int tc_smem_bytes() {
   const int wstage = tps * Image<WBITS>::kTileBytes;
   const int nsw = WBITS == 16 ? 4 : kTcNSW;
   return 1024 + kTcNSX * tps * kTcXTile + nsw * wstage + kTcNM * 4 + 96 * 8 + 64;  // barrier block: 21 barriers, 64 scales
+}
+
+bool tc_clusters_fit(int wbits, int S, int clusters) {
+  if (S < 2 || S > kTcMaxCluster) return false;
+  return with_wbits(wbits, [&](auto W) {
+    // every instantiation of a weight width has 384 threads, one CTA per SM and the same shared memory: ask for one of them
+    auto kern = wq_gemm_tc_kernel<W, false>;
+    const int smem = tc_smem_bytes<W>();
+    if (raise_smem_limit((const void*)kern, smem) != cudaSuccess) return false;
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3(clusters * S);
+    cfg.blockDim = dim3(kTcThreads);
+    cfg.dynamicSmemBytes = smem;
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeClusterDimension;
+    at[0].val.clusterDim.x = S;
+    at[0].val.clusterDim.y = 1;
+    at[0].val.clusterDim.z = 1;
+    cfg.attrs = at;
+    cfg.numAttrs = 1;
+    int n = 0;
+    if (cudaOccupancyMaxActiveClusters(&n, kern, &cfg) != cudaSuccess) {
+      (void)cudaGetLastError();
+      return false;
+    }
+    return n >= clusters;
+  });
 }
 
 EncodeTiledFn encode_tiled() {
@@ -718,7 +777,9 @@ cudaError_t tc_launch(int wbits, bool fp16, TcParams p, cudaStream_t stream) {
     const size_t smem = (size_t)tc_smem_bytes<W>();
     auto go = [&](auto kern) {
       const cudaError_t e = raise_smem_limit((const void*)kern, (int)smem);
-      return e != cudaSuccess ? e : launch(kern, dim3(grid), dim3(kTcThreads), smem, stream, true, p, amap);
+      if (e != cudaSuccess) return e;
+      return p.cluster ? launch_cluster(kern, dim3(grid), dim3(kTcThreads), smem, stream, true, (unsigned)p.S, p, amap)
+                       : launch(kern, dim3(grid), dim3(kTcThreads), smem, stream, true, p, amap);
     };
     return with_flag(p.NG > grid, [&](auto MULTI) {
       if constexpr (W == 4) {

@@ -12,7 +12,7 @@ SYMBOLS = [
     "b2_status_string", "b2_last_error", "b2_version", "b2_set_pdl",
     "b2_gemm_wq_create", "b2_gemm_wq_destroy", "b2_gemm_wq_packed_bytes", "b2_gemm_wq_prepare_weights",
     "b2_gemm_wq_prepare_swiglu", "b2_gemm_wq_attach_packed", "b2_gemm_wq_workspace_bytes", "b2_gemm_wq_run", "b2_gemm_wq_run_fused", "b2_gemm_wq_sumsq_parts",
-    "b2_gemm_wq_algo_bytes", "b2_quant_fp8", "b2_gemm_wq_run_fp8",
+    "b2_gemm_wq_algo_bytes", "b2_gemm_wq_tc_cluster", "b2_quant_fp8", "b2_gemm_wq_run_fp8",
     "b2_span_bytes", "b2_span_cache_append", "b2_span_context_copy", "b2_span_attn_create", "b2_span_attn_destroy",
     "b2_span_attn_workspace_bytes", "b2_span_attn_run", "b2_span_attn_algo_bytes",
     "b2_span_cache_append_tokens", "b2_span_attn_tokens_workspace_bytes", "b2_span_attn_run_tokens", "b2_spec_accept",
@@ -92,6 +92,7 @@ def _load():
         "b2_gemm_wq_run_fused": (i32, [vp, vp, i64, vp, i64, i32, vp, vp, i32, f32, vp, sz, C.POINTER(GemmFuse), vp]),
         "b2_gemm_wq_sumsq_parts": (i32, [vp]),
         "b2_gemm_wq_algo_bytes": (sz, [vp, i32]),
+        "b2_gemm_wq_tc_cluster": (i32, [vp]),
         "b2_quant_fp8": (i32, [vp, i64, vp, vp, vp, vp, i32, i32, f32, vp]),
         "b2_gemm_wq_run_fp8": (i32, [vp, vp, i64, vp, vp, vp, i64, i32, vp, vp, i32, f32, vp, sz, vp]),
         "b2_span_bytes": (sz, [C.POINTER(SpanCfg)]),

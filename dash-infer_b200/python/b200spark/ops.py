@@ -85,6 +85,9 @@ class GemmWQ:
     def sumsq_parts(self):
         return lib.b2_gemm_wq_sumsq_parts(self.h)
 
+    def tc_cluster(self):
+        return lib.b2_gemm_wq_tc_cluster(self.h)
+
     def __call__(self, a, ws, out=None, act=ACT_NONE, alpha=1.0, residual=None, norm_in=None, sumsq_out=None, xg_out=None):
         """Fused RMSNorm (b2_gemm_fuse), two forms:
         M <= 16, self-contained: norm_in = (None, gamma [K], K, eps) — the GEMV normalises its own activations.

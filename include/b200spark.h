@@ -170,6 +170,9 @@ int b2_gemm_wq_run_fp8(b2_gemm_wq_t handle, const void* A8, int64_t lda_bytes, c
                        void* workspace, size_t workspace_bytes, void* stream);
 /* Algorithmic bytes one run at this M must read from HBM (weights + params + A + C). */
 size_t b2_gemm_wq_algo_bytes(b2_gemm_wq_t handle, int M);
+/* CTAs per thread-block cluster of the batch 17..64 path's k-slices (planned on first use): S when the slices of an
+ * n-group sum their partial tiles in distributed shared memory, 1 when they go through the workspace or there are none. */
+int b2_gemm_wq_tc_cluster(b2_gemm_wq_t handle);
 
 /* =====================================================================================
  * SpanAttention: paged KV cache (spans) append + single-query attention, GQA, KV in FT / int8 / uint4 / fp8-e4m3.

@@ -4,7 +4,8 @@
 
 For every shape and batch it replays, from a CUDA graph, one launch per layer over enough layers' weights to overflow L2,
 times the replays with CUDA events and prints us per launch, GB/s of the bytes the GEMM must move, the grid and the largest
-number of 64-k tiles one CTA streams (tests/tc_schedule.py).  Then it fits time = fixed + rate * tiles over the shapes of each
+number of 64-k tiles one CTA streams (tests/tc_schedule.py; cluster = CTAs per thread-block cluster as the handle planned
+it, 1 for the workspace split-K or no split).  Then it fits time = fixed + rate * tiles over the shapes of each
 batch: the per-launch fixed cost and the per-tile cost of the main loop.  A shape is NAME or NAME=KxN (p: gate/up pair),
 e.g. gate264=3584x16896p.  Writes nothing."""
 import argparse
@@ -107,7 +108,7 @@ def main():
             tiles = pl.max_tiles()
             gbs = hs[0].algo_bytes(M) / (med * 1e-6) / 1e9
             print(f"{name:8s} M={M:3d} K={K:5d} N={N:5d}{'x2' if pair else '  '} layers={len(hs):2d}  {med:7.2f} us "
-                  f"[{lo:.2f}, {hi:.2f}]  {gbs:7.1f} GB/s  grid={pl.grid:3d} rounds={pl.rounds} slices={pl.S} head={pl.h:2d} "
+                  f"[{lo:.2f}, {hi:.2f}]  {gbs:7.1f} GB/s  grid={pl.grid:3d} rounds={pl.rounds} slices={pl.S} cluster={hs[0].tc_cluster()} head={pl.h:2d} "
                   f"max_tiles/CTA={tiles:4d}", flush=True)
             pts.append((tiles, med))
             del hs
