@@ -20,7 +20,7 @@ SYMBOLS = [
     "b2_rmsnorm", "b2_rotary", "b2_binary", "b2_embedding", "b2_argmax", "b2_argmax_shard", "b2_argmax_merge", "b2_lens_add",
     "b2_rmsnorm_ft", "b2_binary_ft", "b2_argmax_ft", "b2_qk_rmsnorm", "b2_span_cache_append_qknorm",
     "b2_rotary_table", "b2_span_cache_append_rope_table",
-    "b2_logprobs", "b2_logprobs_partial_bytes", "b2_logprobs_shard", "b2_logprobs_merge",
+    "b2_logprobs", "b2_logprobs_partial_bytes", "b2_logprobs_shard", "b2_logprobs_merge", "b2_sample",
     "b2_comm_create", "b2_comm_destroy", "b2_comm_buffer_bytes", "b2_comm_export", "b2_comm_connect", "b2_comm_connect_pointers",
     "b2_comm_local_buffer", "b2_comm_error", "b2_allreduce", "b2_allgather", "b2_gemm_wq_run_allreduce",
 ]
@@ -63,6 +63,7 @@ KV_NONE, KV_I8, KV_U4 = 0, 1, 2
 KV_FP8 = 3  # extension (not a span::QuantMode value): fp8-e4m3 KV cache, head 128 only
 COMM_HANDLE_BYTES = 64
 MAX_TOP_LOGPROBS = 10  # B2_MAX_TOP_LOGPROBS
+SAMPLE_MAX_N = 262144  # B2_SAMPLE_MAX_N
 
 
 class B2Error(RuntimeError):
@@ -132,6 +133,7 @@ def _load():
         "b2_logprobs_partial_bytes": (sz, [i32]),
         "b2_logprobs_shard": (i32, [vp, vp, vp, i32, i32, i64, i64, i32, i32, vp]),
         "b2_logprobs_merge": (i32, [vp, vp, vp, vp, vp, i32, i32, i32, vp]),
+        "b2_sample": (i32, [vp, vp, i32, i32, i64, vp, vp, vp, vp, vp, i32, vp]),
         "b2_comm_create": (i32, [C.POINTER(vp), i32, i32, sz]),
         "b2_comm_destroy": (i32, [vp]),
         "b2_comm_buffer_bytes": (sz, [i32, sz]),

@@ -138,7 +138,7 @@ class _RefView:
 class DecodeStack:
     def __init__(self, cfg, batch, max_len, wbits=4, group=-1, kv="none", span=128, seed=1234, device="cuda",
                  keep_ref=False, layers=None, tp_rank=0, tp_size=1, tp_group=None, fuse_swiglu=True,
-                 collective=None, comm=None, dtype=torch.bfloat16, q_len=1, tree=False, logprobs=0):
+                 collective=None, comm=None, dtype=torch.bfloat16, q_len=1, tree=False, logprobs=0, sample=False):
         """tp_size > 1: the reference's tensor-parallel layout (QKV/gate/up column split, o/down row split + all-reduce,
         vocab-split lm_head + B-element all-gather); every rank builds the SAME full synthetic weights from `seed` and
         keeps its shard, exactly like the reference splits an already-quantized checkpoint.
@@ -153,7 +153,14 @@ class DecodeStack:
         records, one all-gather, b2_logprobs_merge) in place of the argmax, with the same ids and launch count: self.tok_lp
         [B*T] fp32 (the logprob of each row's own argmax), self.top_ids [B*T, N] int64 and self.top_lp [B*T, N] fp32 (the N
         most likely tokens, argmax order).  Every row of a multi-token or tree step gets them; the logprob of an emitted token
-        is tok_lp at its row: row b*T + u for the token pred[b, u] (u = path[b, j] in a tree).  N = 0 runs today's step."""
+        is tok_lp at its row: row b*T + u for the token pred[b, u] (u = path[b, j] in a tree).  N = 0 runs today's step.
+        sample=True (q_len 1, one GPU): the step draws next_ids with b2_sample in place of the argmax, with the same launch
+        count.  The per-sequence parameters live on the device, [B] each: self.temperature (fp32, default 1.0), self.top_k
+        (int32, 0 = no limit), self.top_p (fp32, 1.0), self.seeds and self.offsets (int64, 0); set_sampling() writes them in
+        place, so a captured graph stays valid, and every step advances the offsets by 1.  With logprobs = N the step runs
+        b2_sample, then b2_logprobs at the drawn ids (one launch more): tok_lp is the logprob of the sampled token under the
+        model's distribution, before temperature and filtering (as the reference reports it), and top_ids / top_lp the N most
+        likely tokens of that distribution."""
         global _DT
         assert dtype in (torch.bfloat16, torch.float16) and (dtype == torch.bfloat16 or (tp_size == 1 and cfg.head == 128)), \
             "fp16: single GPU, head size 128 (the communicator and the head-64 kernels are bf16)"
@@ -163,7 +170,9 @@ class DecodeStack:
         assert not cfg.qk_norm or cfg.head == 128, "per-head Q/K norm: head size 128"
         assert cfg.rope_scaling is None or cfg.head == 128, "rope scaling: head size 128"
         assert 0 <= logprobs <= ops._lib.MAX_TOP_LOGPROBS, "logprobs: 0 .. 10 alternatives"
-        self.logprobs = logprobs
+        assert not sample or (q_len == 1 and tp_size == 1), \
+            "sample=True: single-token steps (q_len == 1) on one GPU (tp_size == 1); greedy verification stays greedy"
+        self.logprobs, self.sample = logprobs, sample
         self.dtype = _DT = dtype
         self.q_len, self.tree = q_len, tree
         rows = batch * q_len  # activation rows of a step
@@ -229,6 +238,12 @@ class DecodeStack:
         self._lens_new = torch.full((batch,), q_len, dtype=torch.int32, device=device)  # lens_old + q_len
         self._ids = torch.zeros(batch, dtype=torch.int64, device=device)
         self._next_ids = torch.zeros(batch, dtype=torch.int64, device=device)
+        if sample:
+            self._temperature = torch.ones(batch, dtype=torch.float32, device=device)
+            self._top_k = torch.zeros(batch, dtype=torch.int32, device=device)
+            self._top_p = torch.ones(batch, dtype=torch.float32, device=device)
+            self._seeds = torch.zeros(batch, dtype=torch.int64, device=device)
+            self._offsets = torch.zeros(batch, dtype=torch.int64, device=device)
         if q_len > 1:
             self._tokens = torch.zeros(batch, q_len, dtype=torch.int64, device=device)
             self._pred = torch.zeros(batch, q_len, dtype=torch.int64, device=device)
@@ -279,10 +294,21 @@ class DecodeStack:
             self.tokens, self.pred, self.accepted = self._tokens[:b], self._pred[:b], self._accepted[:b]
         if self.tree:
             self.parents, self.path = self._parents[:b], self._path[:b]
+        if self.sample:
+            for k in ("temperature", "top_k", "top_p", "seeds", "offsets"):
+                setattr(self, k, getattr(self, "_" + k)[:b])
         if self.logprobs and self.tp > 1:
             rec = self._all_rec.numel() // (self.tp * self.Bmax)
             self.all_rec = self._all_rec[:self.tp * b * rec].view(self.tp, b * rec)
         self.graph = None
+
+    def set_sampling(self, temperature=None, top_k=None, top_p=None, seeds=None, offsets=None):
+        """Write the sampling parameters of the current batch in place (a scalar or [B] values each; None keeps the value)."""
+        assert self.sample, "set_sampling: the stack was built with sample=False"
+        for k, v in (("temperature", temperature), ("top_k", top_k), ("top_p", top_p), ("seeds", seeds), ("offsets", offsets)):
+            if v is not None:
+                t = getattr(self, k)
+                t.copy_(torch.as_tensor(v, dtype=t.dtype).expand(t.shape))
 
     # ------------------------------------------------------------------ cache fill
     def set_context(self, ctx, seed=4321):
@@ -412,7 +438,12 @@ class DecodeStack:
         else:
             ops.rmsnorm(self.x, self.gf, cfg.eps, out=self.xn); n += 1
             self.lm_head(self.xn, ws, out=self.logits); n += 1
-        if self.logprobs and self.tp == 1:  # the argmax ids and the log-probabilities in one launch
+        if self.sample:  # the drawn ids; with logprobs, the log-probabilities at them (one launch more)
+            ops.sample(self.logits, self.temperature, self.top_k, self.top_p, self.seeds, self.offsets, out=self.next_ids); n += 1
+            if self.logprobs:
+                ops.logprobs(self.logits, self.logprobs, tok_ids=self.next_ids, out=(None, self.tok_lp, self.top_ids, self.top_lp))
+                n += 1
+        elif self.logprobs and self.tp == 1:  # the argmax ids and the log-probabilities in one launch
             ids = self.pred.view(-1) if T > 1 else self.next_ids
             ops.logprobs(self.logits, self.logprobs, out=(ids, self.tok_lp, self.top_ids, self.top_lp)); n += 1
         elif self.logprobs:  # vocab-split: per-rank records, one all-gather of them, the merge
@@ -472,11 +503,14 @@ class DecodeStack:
         """Warm up once eagerly (plans, workspace growth), rewind the lengths, then capture one step."""
         lo, ln = self.lens_old.clone(), self.lens_new.clone()
         tk = self.tokens.clone() if self.q_len > 1 else None  # the accept kernel rewrites column 0
+        off = self.offsets.clone() if self.sample else None  # the warm-up step advances the draw counters
         self._step_ops()
         torch.cuda.synchronize()
         self.lens_old.copy_(lo); self.lens_new.copy_(ln)
         if tk is not None:
             self.tokens.copy_(tk)
+        if off is not None:
+            self.offsets.copy_(off)
         g = torch.cuda.CUDAGraph()
         with torch.cuda.graph(g):
             self._step_ops()

@@ -651,6 +651,21 @@ def logprobs_merge(all_partials, n_top, out=None):
     return ids, tok_lp, top_ids, top_lp
 
 
+def sample(logits, temperature, top_k, top_p, seeds, offsets, out=None):
+    """A token drawn from each row of logits [rows, n] FT (b2_sample; any row stride): temperature, top_p fp32 [rows], top_k
+    int32 [rows], seeds, offsets int64 [rows] (read as uint64 bits), all on the device.  Advances offsets by 1 in place and
+    returns the ids, int64 [rows] (out, if given).  The contract, step by step: include/b200spark.h."""
+    rows, n = logits.shape
+    assert logits.stride(-1) == 1
+    out = torch.empty(rows, dtype=torch.int64, device=logits.device) if out is None else out
+    for t, dt, name in ((out, torch.int64, "out"), (temperature, torch.float32, "temperature"), (top_k, torch.int32, "top_k"),
+                        (top_p, torch.float32, "top_p"), (seeds, torch.int64, "seeds"), (offsets, torch.int64, "offsets")):
+        assert t.dtype == dt and t.is_contiguous() and tuple(t.shape) == (rows,), f"sample: {name} must be [{rows}] {dt} contiguous"
+    check(lib.b2_sample(_ptr(out), _ptr(logits), rows, n, logits.stride(0), _ptr(temperature), _ptr(top_k), _ptr(top_p),
+                        _ptr(seeds), _ptr(offsets), _ft(logits), _stream()), "b2_sample")
+    return out
+
+
 def lens_add(lens, delta):
     check(lib.b2_lens_add(_ptr(lens), lens.numel(), int(delta), _stream()), "b2_lens_add")
     return lens

@@ -30,6 +30,8 @@
  *                         QKLayerNormNoBeta (Qwen3, qwen_v30.py)  csrc/core/kernel/cuda/layernorm.cu:259-304
  *   b2_rotary_table, b2_span_cache_append_rope_table
  *                         Rotary with a [batch, head/2] inverse-frequency table  kernel/cuda/rotary.cu:24-80 (static tables)
+ *   b2_sample             gen_sample_gpu (top-k, top-p, temperature, Philox draw)
+ *                           csrc/core/operator/generate_opt/generate/generate_impl_gpu.hpp:116-191
  */
 #ifndef B200SPARK_H_
 #define B200SPARK_H_
@@ -420,6 +422,35 @@ int b2_logprobs_shard(void* partials, const int64_t* tok_ids /* or NULL */, cons
                       int64_t id_offset, int n_top, int ft, void* stream);
 int b2_logprobs_merge(int64_t* ids_out, float* tok_lp, int64_t* top_ids, float* top_lp, const void* all_partials, int nranks,
                       int rows, int n_top, void* stream);
+/* Sampling of the decode step (temperature, top-k, top-p; gen_sample_gpu, generate_impl_gpu.hpp:116-191), on the device,
+ * CUDA-graph replayable.  ids_out[r] = a token drawn from row r of logits [rows, ld] FT (ft = B2_DT_BF16 / B2_DT_F16, the
+ * first n columns).  temperature, top_p: fp32 [rows]; top_k: int32 [rows]; seeds, offsets: uint64 [rows]; all
+ * device-resident, so a captured graph picks up values the caller writes between replays.  offsets[r] += 1 for every row,
+ * every call.  Per row, with every logit widened to fp32 exactly:
+ *   1. Greedy rows take b2_argmax's id bit for bit: the row maximum m not finite (a NaN, a +inf, or every entry -inf),
+ *      temperature NaN or <= 0, or c = __fdiv_rn(LOG2E_F32, temperature) not finite (LOG2E_F32 = 0x3FB8AA3B).  The ids
+ *      always lie in [0, n).
+ *   2. Order: by value, highest first, the lower id first among equal values; -0 and +0 are equal.
+ *   3. Weights: W_i = 0 for x_i = -inf, else W_i = __float2ull_rn(ex2.approx.ftz(fl32(fl32(x_i - m) c)) 2^40), an integer
+ *      <= 2^40; the maximum has W = 2^40.  temperature = +inf gives c = 0: uniform over the finite entries.  A token below
+ *      about 2^-41 of the maximum's probability has weight 0 and is never drawn.
+ *   4. Top-k: k = top_k[r] (k <= 0 or k > n: n); the kept set is the first k elements in the order (ties at the boundary
+ *      split by id); S_k = the sum of their W (< 2^58).
+ *   5. Top-p: p24 = clamp(__float2uint_rn(top_p 2^24), 0, 2^24) (NaN or >= 1: 2^24); Pt = max(1, ceil(p24 S_k / 2^24)) in
+ *      exact 128-bit arithmetic; the nucleus is the shortest prefix of the kept set, in the order, whose W sum is at least
+ *      Pt (it always holds the maximum); S_p = its sum.
+ *   6. Draw: (r0, r1, r2, r3) = Philox4x32-10(counter = (lo32(off), hi32(off), 0, 0), key = (lo32(seed), hi32(seed))),
+ *      off = offsets[r] before the increment; u24 = r0 >> 8; U = floor(u24 S_p / 2^24) (0 <= U < S_p).  The drawn id is the
+ *      first element of the nucleus, in the order, at which the running W sum exceeds U (zero-weight elements are never
+ *      drawn).  The row index is not part of the counter: equal seeds, offsets and logits draw the same token at any batch
+ *      position and batch size.
+ * Everything after step 3 is integer arithmetic, so no summation order can change a result.  A row runs on one CTA, or on
+ * a cluster of 8 when n > 32768.
+ * n < 1, ld < n, rows < 0, a NULL pointer, ft other than bf16 / fp16: B2_ERR_PARAM; n > B2_SAMPLE_MAX_N: B2_ERR_LIMIT; all
+ * before any launch.  No workspace. */
+#define B2_SAMPLE_MAX_N 262144
+int b2_sample(int64_t* ids_out, const void* logits, int rows, int n, int64_t ld, const float* temperature,
+              const int32_t* top_k, const float* top_p, const uint64_t* seeds, uint64_t* offsets, int ft, void* stream);
 /* lens[b] += delta for b < batch (keeps sequence lengths device-resident under CUDA graphs) */
 int b2_lens_add(int32_t* lens, int batch, int delta, void* stream);
 /* Greedy verification of a multi-token step, on the device (CUDA-graph replayable).  tokens [batch][q_len] int64: column 0
