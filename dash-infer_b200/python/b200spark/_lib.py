@@ -21,6 +21,7 @@ SYMBOLS = [
     "b2_rmsnorm_ft", "b2_binary_ft", "b2_argmax_ft", "b2_qk_rmsnorm", "b2_span_cache_append_qknorm",
     "b2_rotary_table", "b2_span_cache_append_rope_table",
     "b2_logprobs", "b2_logprobs_partial_bytes", "b2_logprobs_shard", "b2_logprobs_merge", "b2_sample",
+    "b2_history_load", "b2_history_append", "b2_penalize",
     "b2_comm_create", "b2_comm_destroy", "b2_comm_buffer_bytes", "b2_comm_export", "b2_comm_connect", "b2_comm_connect_pointers",
     "b2_comm_local_buffer", "b2_comm_error", "b2_allreduce", "b2_allgather", "b2_gemm_wq_run_allreduce",
 ]
@@ -53,6 +54,17 @@ class QkNorm(C.Structure):
 
 class RopeTable(C.Structure):
     _fields_ = [("inv_freq", C.c_void_p), ("stride", C.c_int64), ("attn_factor", C.c_float), ("reserved", C.c_int32)]
+
+
+class TokenHistory(C.Structure):
+    _fields_ = [("tokens", C.c_void_p), ("len", C.c_void_p), ("prompt_len", C.c_void_p), ("table", C.c_void_p),
+                ("distinct", C.c_void_p), ("n_distinct", C.c_void_p), ("max_len", C.c_int32), ("vocab", C.c_int32)]
+
+
+class PenaltyParams(C.Structure):
+    _fields_ = [("repetition", C.c_void_p), ("presence", C.c_void_p), ("frequency", C.c_void_p),
+                ("no_repeat_ngram", C.c_void_p), ("min_length", C.c_void_p), ("eos_id", C.c_void_p), ("suppress", C.c_void_p),
+                ("reserved", C.c_void_p)]
 
 
 DT_F32, DT_F16, DT_I8, DT_BF16, DT_U8 = 1, 2, 3, 9, 10
@@ -134,6 +146,9 @@ def _load():
         "b2_logprobs_shard": (i32, [vp, vp, vp, i32, i32, i64, i64, i32, i32, vp]),
         "b2_logprobs_merge": (i32, [vp, vp, vp, vp, vp, i32, i32, i32, vp]),
         "b2_sample": (i32, [vp, vp, i32, i32, i64, vp, vp, vp, vp, vp, i32, vp]),
+        "b2_history_load": (i32, [C.POINTER(TokenHistory), i32, vp, i32, i32, vp]),
+        "b2_history_append": (i32, [C.POINTER(TokenHistory), vp, i32, vp]),
+        "b2_penalize": (i32, [vp, i32, i32, i64, i64, C.POINTER(TokenHistory), C.POINTER(PenaltyParams), i32, vp]),
         "b2_comm_create": (i32, [C.POINTER(vp), i32, i32, sz]),
         "b2_comm_destroy": (i32, [vp]),
         "b2_comm_buffer_bytes": (sz, [i32, sz]),

@@ -138,7 +138,8 @@ class _RefView:
 class DecodeStack:
     def __init__(self, cfg, batch, max_len, wbits=4, group=-1, kv="none", span=128, seed=1234, device="cuda",
                  keep_ref=False, layers=None, tp_rank=0, tp_size=1, tp_group=None, fuse_swiglu=True,
-                 collective=None, comm=None, dtype=torch.bfloat16, q_len=1, tree=False, logprobs=0, sample=False):
+                 collective=None, comm=None, dtype=torch.bfloat16, q_len=1, tree=False, logprobs=0, sample=False,
+                 penalties=False):
         """tp_size > 1: the reference's tensor-parallel layout (QKV/gate/up column split, o/down row split + all-reduce,
         vocab-split lm_head + B-element all-gather); every rank builds the SAME full synthetic weights from `seed` and
         keeps its shard, exactly like the reference splits an already-quantized checkpoint.
@@ -160,7 +161,12 @@ class DecodeStack:
         place, so a captured graph stays valid, and every step advances the offsets by 1.  With logprobs = N the step runs
         b2_sample, then b2_logprobs at the drawn ids (one launch more): tok_lp is the logprob of the sampled token under the
         model's distribution, before temperature and filtering (as the reference reports it), and top_ids / top_lp the N most
-        likely tokens of that distribution."""
+        likely tokens of that distribution.
+        penalties=True (q_len 1): the reference's logits processor runs on the lm_head's output (b2_penalize; each TP rank
+        its vocab shard), so the argmax, b2_sample and b2_logprobs all see the processed row; the step then appends next_ids
+        to a per-sequence token history on the device (one launch each).  set_history(b, ids, prompt_len) loads sequence
+        b's tokens, set_penalties() writes the per-sequence parameters in place (neutral until written).  self.history and
+        self.penalties are the views of the current batch; capture() leaves the history as it found it."""
         global _DT
         assert dtype in (torch.bfloat16, torch.float16) and (dtype == torch.bfloat16 or (tp_size == 1 and cfg.head == 128)), \
             "fp16: single GPU, head size 128 (the communicator and the head-64 kernels are bf16)"
@@ -172,7 +178,9 @@ class DecodeStack:
         assert 0 <= logprobs <= ops._lib.MAX_TOP_LOGPROBS, "logprobs: 0 .. 10 alternatives"
         assert not sample or (q_len == 1 and tp_size == 1), \
             "sample=True: single-token steps (q_len == 1) on one GPU (tp_size == 1); greedy verification stays greedy"
-        self.logprobs, self.sample = logprobs, sample
+        assert not penalties or q_len == 1, \
+            "penalties=True: single-token steps (q_len == 1); the history is not kept per draft position"
+        self.logprobs, self.sample, self.pen = logprobs, sample, penalties
         self.dtype = _DT = dtype
         self.q_len, self.tree = q_len, tree
         rows = batch * q_len  # activation rows of a step
@@ -244,6 +252,9 @@ class DecodeStack:
             self._top_p = torch.ones(batch, dtype=torch.float32, device=device)
             self._seeds = torch.zeros(batch, dtype=torch.int64, device=device)
             self._offsets = torch.zeros(batch, dtype=torch.int64, device=device)
+        if penalties:
+            self._history = ops.TokenHistory(batch, max_len, cfg.vocab, device)
+            self._penalties = ops.Penalties(batch, device)
         if q_len > 1:
             self._tokens = torch.zeros(batch, q_len, dtype=torch.int64, device=device)
             self._pred = torch.zeros(batch, q_len, dtype=torch.int64, device=device)
@@ -297,6 +308,8 @@ class DecodeStack:
         if self.sample:
             for k in ("temperature", "top_k", "top_p", "seeds", "offsets"):
                 setattr(self, k, getattr(self, "_" + k)[:b])
+        if self.pen:
+            self.history, self.penalties = self._history.view(b), self._penalties.view(b)
         if self.logprobs and self.tp > 1:
             rec = self._all_rec.numel() // (self.tp * self.Bmax)
             self.all_rec = self._all_rec[:self.tp * b * rec].view(self.tp, b * rec)
@@ -309,6 +322,18 @@ class DecodeStack:
             if v is not None:
                 t = getattr(self, k)
                 t.copy_(torch.as_tensor(v, dtype=t.dtype).expand(t.shape))
+
+    def set_penalties(self, repetition=None, presence=None, frequency=None, no_repeat_ngram=None, min_length=None, eos_id=None,
+                      suppress_repetition_in_generation=None):
+        """Write the logits-processor parameters of the current batch in place (a scalar or [B] values each; None keeps the
+        value).  Ranges as the reference's request checks: repetition in [0, 2], presence and frequency in [-2, 2]."""
+        assert self.pen, "set_penalties: the stack was built with penalties=False"
+        self.penalties.set(repetition, presence, frequency, no_repeat_ngram, min_length, eos_id, suppress_repetition_in_generation)
+
+    def set_history(self, b, ids, prompt_len=None):
+        """Load sequence b's tokens into its history (prompt first; prompt_len of them, all by default)."""
+        assert self.pen, "set_history: the stack was built with penalties=False"
+        self._history.load(b, ids, prompt_len)
 
     # ------------------------------------------------------------------ cache fill
     def set_context(self, ctx, seed=4321):
@@ -438,6 +463,8 @@ class DecodeStack:
         else:
             ops.rmsnorm(self.x, self.gf, cfg.eps, out=self.xn); n += 1
             self.lm_head(self.xn, ws, out=self.logits); n += 1
+        if self.pen:  # the logits processor, in place on this rank's vocab shard
+            ops.penalize(self.logits, self.history, self.penalties, self.tp_rank * self.vocab_l); n += 1
         if self.sample:  # the drawn ids; with logprobs, the log-probabilities at them (one launch more)
             ops.sample(self.logits, self.temperature, self.top_k, self.top_p, self.seeds, self.offsets, out=self.next_ids); n += 1
             if self.logprobs:
@@ -473,6 +500,8 @@ class DecodeStack:
         else:
             ops.lens_add(self.lens_old, 1); n += 1
             ops.lens_add(self.lens_new, 1); n += 1
+        if self.pen:  # the emitted token joins the history
+            self.history.append(self.next_ids); n += 1
         # rows per launch above 16 rows: 64 on the wgmma path (per-channel int4/int8, bf16 lm_head), 16 for sub-channel
         # weights (mma.sync path); below, one launch takes all rows
         hchunks = (R + 63) // 64 if R > 16 else 1
@@ -504,8 +533,11 @@ class DecodeStack:
         lo, ln = self.lens_old.clone(), self.lens_new.clone()
         tk = self.tokens.clone() if self.q_len > 1 else None  # the accept kernel rewrites column 0
         off = self.offsets.clone() if self.sample else None  # the warm-up step advances the draw counters
+        hist = self.history.snapshot() if self.pen else None  # ... and appends a token to the history
         self._step_ops()
         torch.cuda.synchronize()
+        if hist is not None:
+            self.history.restore(hist)
         self.lens_old.copy_(lo); self.lens_new.copy_(ln)
         if tk is not None:
             self.tokens.copy_(tk)

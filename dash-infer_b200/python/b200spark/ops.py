@@ -7,8 +7,8 @@ import ctypes as C
 import torch
 
 from . import _lib
-from ._lib import (ACT_NONE, BIN_ADD, BIN_MUL, DT_BF16, DT_I8, DT_U8, KV_I8, KV_NONE, KV_U4, GemmDesc, GemmFuse, QkNorm, RopeCfg,
-                   RopeTable, SpanCfg, check, lib)
+from ._lib import (ACT_NONE, BIN_ADD, BIN_MUL, DT_BF16, DT_I8, DT_U8, KV_I8, KV_NONE, KV_U4, GemmDesc, GemmFuse, PenaltyParams,
+                   QkNorm, RopeCfg, RopeTable, SpanCfg, check, lib)
 
 
 def _stream():
@@ -669,3 +669,117 @@ def sample(logits, temperature, top_k, top_p, seeds, offsets, out=None):
 def lens_add(lens, delta):
     check(lib.b2_lens_add(_ptr(lens), lens.numel(), int(delta), _stream()), "b2_lens_add")
     return lens
+
+
+class TokenHistory:
+    """The per-sequence token history of the logits processor (b2_token_history), on the device: `rows` slots of at most
+    max_len tokens each over a vocabulary of `vocab` ids.  tokens [rows, max_len], len / prompt_len / n_distinct [rows],
+    table [rows, vocab] (bit 30: in the prompt, bits 0..29: generated count) and distinct [rows, max_len], all int32.
+    view(b) shares the storage with the first b slots (DecodeStack.set_batch)."""
+
+    _FIELDS = ("tokens", "len", "prompt_len", "table", "distinct", "n_distinct")
+
+    def __init__(self, rows, max_len, vocab, device="cuda"):
+        assert rows >= 1 and 1 <= max_len < 2 ** 30 and vocab >= 1
+        self.rows, self.max_len, self.vocab = rows, max_len, vocab
+        z = lambda *shape: torch.zeros(*shape, dtype=torch.int32, device=device)
+        self.tokens, self.len, self.prompt_len = z(rows, max_len), z(rows), z(rows)
+        self.table, self.distinct, self.n_distinct = z(rows, vocab), z(rows, max_len), z(rows)
+        self.c = _lib.TokenHistory(*(t.data_ptr() for t in (self.tokens, self.len, self.prompt_len, self.table, self.distinct,
+                                                              self.n_distinct)), max_len, vocab)
+
+    def view(self, rows):
+        assert 1 <= rows
+        v = object.__new__(TokenHistory)
+        v.__dict__.update(self.__dict__)
+        v.rows = rows
+        for k in self._FIELDS:
+            setattr(v, k, getattr(self, k)[:rows])
+        return v
+
+    def load(self, slot, ids, prompt_len=None):
+        """Slot `slot` := ids (the prompt first; prompt_len of them, all by default), after clearing its previous tokens."""
+        ids = torch.as_tensor(ids, dtype=torch.int32).reshape(-1).to(self.tokens.device)
+        n = ids.numel()
+        prompt_len = n if prompt_len is None else int(prompt_len)
+        assert 0 <= slot < self.rows, f"history slot {slot} outside [0, {self.rows})"
+        assert n <= self.max_len and 0 <= prompt_len <= n, f"history: {n} tokens (max {self.max_len}), prompt {prompt_len}"
+        assert n == 0 or (int(ids.min()) >= 0 and int(ids.max()) < self.vocab), f"history: token ids outside [0, {self.vocab})"
+        check(lib.b2_history_load(C.byref(self.c), int(slot), _ptr(ids), n, prompt_len, _stream()), "b2_history_load")
+        return self
+
+    def reset(self, slot):
+        return self.load(slot, [], 0)
+
+    def append(self, ids):
+        """Append ids[r] (int64 [rows], on the device) to slot r, for the first ids.numel() slots."""
+        assert ids.dtype == torch.int64 and ids.is_contiguous() and ids.numel() <= self.rows
+        check(lib.b2_history_append(C.byref(self.c), _ptr(ids), ids.numel(), _stream()), "b2_history_append")
+        return self
+
+    def snapshot(self):
+        return [getattr(self, k).clone() for k in self._FIELDS]
+
+    def restore(self, snap):
+        for k, s in zip(self._FIELDS, snap):
+            getattr(self, k).copy_(s)
+
+
+class Penalties:
+    """Per-row parameters of b2_penalize, device arrays [rows]: repetition, presence, frequency (fp32), no_repeat_ngram,
+    min_length, eos_id, suppress (int32).  They start neutral (1, 0, 0, 0, 0, -1, 0), which changes nothing."""
+
+    FLOAT = ("repetition", "presence", "frequency")
+    INT = ("no_repeat_ngram", "min_length", "eos_id", "suppress")
+
+    def __init__(self, rows, device="cuda"):
+        self.rows = rows
+        self.repetition = torch.ones(rows, dtype=torch.float32, device=device)
+        self.presence = torch.zeros(rows, dtype=torch.float32, device=device)
+        self.frequency = torch.zeros(rows, dtype=torch.float32, device=device)
+        for k in self.INT:
+            setattr(self, k, torch.zeros(rows, dtype=torch.int32, device=device))
+        self.eos_id.fill_(-1)
+
+    def view(self, rows):
+        v = object.__new__(Penalties)
+        v.rows = rows
+        for k in self.FLOAT + self.INT:
+            setattr(v, k, getattr(self, k)[:rows])
+        return v
+
+    def set(self, repetition=None, presence=None, frequency=None, no_repeat_ngram=None, min_length=None, eos_id=None,
+            suppress_repetition_in_generation=None):
+        """Write parameters in place (a scalar or [rows] values each; None keeps the value).  The ranges are the reference's
+        request checks (as_engine.cpp): repetition in [0, 2], presence and frequency in [-2, 2]; n-gram size and min-length
+        >= 0."""
+        vals = dict(repetition=repetition, presence=presence, frequency=frequency, no_repeat_ngram=no_repeat_ngram,
+                    min_length=min_length, eos_id=eos_id, suppress=suppress_repetition_in_generation)
+        lim = dict(repetition=(0.0, 2.0), presence=(-2.0, 2.0), frequency=(-2.0, 2.0), no_repeat_ngram=(0, 2 ** 31 - 1),
+                   min_length=(0, 2 ** 31 - 1), eos_id=(-2 ** 31, 2 ** 31 - 1), suppress=(0, 1))
+        for k, v in vals.items():
+            if v is None:
+                continue
+            t = getattr(self, k)
+            h = torch.as_tensor(v, dtype=torch.float64).expand(t.shape)
+            lo, hi = lim[k]
+            if not bool(((h >= lo) & (h <= hi)).all()):
+                raise ValueError(f"penalties: {k} must lie in [{lo}, {hi}]")
+            if k in self.INT and not bool((h == h.round()).all()):
+                raise ValueError(f"penalties: {k} must be an integer")
+            t.copy_(h.to(t.dtype))
+        return self
+
+    def c(self):
+        return PenaltyParams(*(getattr(self, k).data_ptr() for k in self.FLOAT + self.INT), None)
+
+
+def penalize(logits, history, params, id_offset=0):
+    """The logits processor (b2_penalize), in place on logits [rows, n] FT (any row stride), which hold vocabulary ids
+    [id_offset, id_offset + n): row r reads history slot r and params row r.  Returns logits."""
+    rows, n = logits.shape
+    assert logits.stride(-1) == 1
+    assert rows <= history.rows and rows <= params.rows, "penalize: more rows than history slots or parameter rows"
+    check(lib.b2_penalize(_ptr(logits), rows, n, logits.stride(0), int(id_offset), C.byref(history.c), C.byref(params.c()),
+                          _ft(logits), _stream()), "b2_penalize")
+    return logits

@@ -451,6 +451,76 @@ int b2_logprobs_merge(int64_t* ids_out, float* tok_lp, int64_t* top_ids, float* 
 #define B2_SAMPLE_MAX_N 262144
 int b2_sample(int64_t* ids_out, const void* logits, int rows, int n, int64_t ld, const float* temperature,
               const int32_t* top_k, const float* top_p, const uint64_t* seeds, uint64_t* offsets, int ft, void* stream);
+/* Per-sequence token history on the device (the in_ids / cur_len / input_len of the reference's logits processor).  Every
+ * array has `rows` slots (row r of a step uses slot r); all pointers are device memory, zero-initialised before first use.
+ *   tokens     int32 [rows][max_len]  the sequence, prompt first; an id outside [0, vocab) is stored as -1
+ *   len        int32 [rows]           cur_len: the tokens held (prompt included)
+ *   prompt_len int32 [rows]           input_len: positions < prompt_len are the prompt
+ *   table      int32 [rows][vocab]    per id: bit 30 = occurs in the prompt, bits 0..29 = occurrences at positions
+ *                                     >= prompt_len (the generated count); 0 for an id that does not occur
+ *   distinct   int32 [rows][max_len]  the ids whose table entry is not 0, each once, in no particular order
+ *   n_distinct int32 [rows]
+ * max_len < 2^30.  The processor reads the table and the distinct list, so its work per row follows the distinct ids, not
+ * the vocabulary. */
+typedef struct b2_token_history {
+  int32_t* tokens;
+  int32_t* len;
+  int32_t* prompt_len;
+  int32_t* table;
+  int32_t* distinct;
+  int32_t* n_distinct;
+  int32_t max_len;
+  int32_t vocab;
+} b2_token_history;
+/* Load slot `slot` with ids[0 .. n_ids) (device int32, each in [0, vocab), n_ids <= max_len), the first prompt_len of them
+ * the prompt (0 <= prompt_len <= n_ids).  The table entries of the slot's previous ids are cleared first, through its
+ * distinct list (no vocab-wide clear).  n_ids = 0 empties the slot.  One CTA; the other slots are untouched. */
+int b2_history_load(const b2_token_history* hist, int slot, const int32_t* ids, int n_ids, int prompt_len, void* stream);
+/* Append ids[r] (int64, device) to slot r for r < rows, on the device (CUDA-graph replayable: each replay appends once).  A
+ * slot that holds max_len tokens is left as it is.  An id outside [0, vocab) is stored as -1 and counted nowhere. */
+int b2_history_append(const b2_token_history* hist, const int64_t* ids, int rows, void* stream);
+/* Per-row parameters of b2_penalize, device arrays [rows], read at every call (a captured step uses the values last
+ * written).  The neutral values repetition 1, presence 0, frequency 0, no_repeat_ngram 0, min_length 0 change nothing. */
+typedef struct b2_penalty_params {
+  const float* repetition;
+  const float* presence;
+  const float* frequency;
+  const int32_t* no_repeat_ngram;
+  const int32_t* min_length;
+  const int32_t* eos_id;    /* < 0: none */
+  const int32_t* suppress;  /* suppress_repetition_in_generation: != 0 counts only generated positions for repetition */
+  const void* reserved;     /* NULL */
+} b2_penalty_params;
+/* The logits processor of the reference's sampling step (LogitsProcessor, beam_search.cu), in place, CUDA-graph
+ * replayable.  logits FT [rows, ld] (ft = B2_DT_BF16 / B2_DT_F16) hold vocabulary ids [id_offset, id_offset + n) of the
+ * rows (a vocab-split lm_head passes its shard); columns n .. ld-1 are never written, and an id outside the shard is skipped.
+ * Row r reads slot r of hist: L = len[r], P = prompt_len[r], the table entry e_t of id t, c_t = its generated count.  FT(v)
+ * is round-to-nearest-even of fp32 v to FT.  For every id t with e_t != 0 (the ids occurring at positions < L), once,
+ * from its value x:
+ *   1. Repetition (when suppress[r] == 0, or c_t > 0): with R = FT(repetition[r]),  x < 0 ? x * R : x / R  in FT
+ *      arithmetic: the product is __hmul (correctly rounded); the quotient is CUDA's __hdiv of the FT type, the same
+ *      instructions the reference's fast-math build runs: bf16 div.approx.f32 of the widened values (operands scaled by
+ *      1/4 when |R| >= 2^126) rounded to bf16, fp16 the widened x times rcp.approx.ftz.f32(R) rounded to fp16 (one fma
+ *      correction step when that result is a nonzero value below 0x008F).  Both equal the correctly rounded FT quotient
+ *      except within about 2^-22 relative of a rounding midpoint.  0 and NaN take the quotient.  Skipped when R == 1.
+ *   2. Frequency and presence: x = x - FT(s) (__hsub, correctly rounded), s = fl32(c_t frequency[r]) + (c_t > 0 ?
+ *      presence[r] : 0), products and sums in fp32 with subnormals flushed (the reference's mul.ftz / add.ftz).  Skipped
+ *      when FT(s) is +0.  Repetition comes first, as in the reference; an id is penalised once however often it occurs.
+ * Then the bans, which write FT(-1e9f) (bf16 0xCE6E; fp16 -inf):
+ *   3. No-repeat n-gram, g = no_repeat_ngram[r] > 0: for every j <= L - g with tokens[j + i] == tokens[L - g + 1 + i] for
+ *      all i < g - 1, the id tokens[j + g - 1] (g == 1: every id of the history).  The comparison is of the stored
+ *      tokens, so positions that held ids outside [0, vocab) compare as -1, equal to one another (the reference compares
+ *      the raw ids); the front end never appends such an id.
+ *   4. Min-length: eos_id[r] when L < min_length[r] and eos_id[r] >= 0 (L counts the prompt, as in the reference).
+ * Differences from the reference, none visible to b2_argmax, b2_sample or b2_logprobs: the reference subtracts
+ * FT(0 * frequency) from every column of the row, so with frequency < 0 it turns -0 into +0 in columns outside the
+ * history (a non-finite frequency turns them into NaN); it writes canonical NaNs where this kernel leaves a NaN's bits
+ * as they are (steps 1 and 2 are skipped at neutral values, so neutral parameters leave the row bit-identical).
+ * Parameter ranges (the reference accepts repetition in [0, 2], presence and frequency in [-2, 2]) are the caller's to
+ * check; the arithmetic is as stated for any value.  One CTA per row.  rows < 0, n < 1, ld < n, id_offset < 0,
+ * id_offset + n > vocab, a NULL pointer or an ft other than bf16 / fp16: B2_ERR_PARAM, before any launch. */
+int b2_penalize(void* logits, int rows, int n, int64_t ld, int64_t id_offset, const b2_token_history* hist,
+                const b2_penalty_params* params, int ft, void* stream);
 /* lens[b] += delta for b < batch (keeps sequence lengths device-resident under CUDA graphs) */
 int b2_lens_add(int32_t* lens, int batch, int delta, void* stream);
 /* Greedy verification of a multi-token step, on the device (CUDA-graph replayable).  tokens [batch][q_len] int64: column 0
