@@ -318,12 +318,9 @@ __global__ void lens_add_kernel(int32_t* lens, int batch, int delta) {
 // (TREE = false) has the parent of c at c - 1, so its drafts tokens[b][1..] are accepted while each equals the prediction
 // before it, and it records no path.
 template <bool TREE>
-__global__ void spec_accept_kernel(int32_t* accepted, int32_t* path, int64_t* next_ids, int32_t* old_lens, int32_t* new_lens,
-                                   int64_t* tokens, const int64_t* pred, const int32_t* parents, int batch, int q_len) {
-  pdl_wait();
-  pdl_launch_dependents();
-  const int b = blockIdx.x * blockDim.x + threadIdx.x;
-  if (b >= batch) return;
+__device__ __forceinline__ int spec_accept_seq(int b, int32_t* accepted, int32_t* path, int64_t* next_ids, int32_t* old_lens,
+                                               int32_t* new_lens, int64_t* tokens, const int64_t* pred, const int32_t* parents,
+                                               int q_len) {
   const int64_t* tk = tokens + (size_t)b * q_len;
   const int64_t* pr = pred + (size_t)b * q_len;
   int n = 1, u = 0;
@@ -343,6 +340,30 @@ __global__ void spec_accept_kernel(int32_t* accepted, int32_t* path, int64_t* ne
   const int ol = old_lens[b] + n;
   old_lens[b] = ol;
   new_lens[b] = ol + q_len;
+  return n;
+}
+
+template <bool TREE>
+__global__ void spec_accept_kernel(int32_t* accepted, int32_t* path, int64_t* next_ids, int32_t* old_lens, int32_t* new_lens,
+                                   int64_t* tokens, const int64_t* pred, const int32_t* parents, int batch, int q_len) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= batch) return;
+  spec_accept_seq<TREE>(b, accepted, path, next_ids, old_lens, new_lens, tokens, pred, parents, q_len);
+}
+
+// sampled verification: the same walk over the step's draws (b2_sample_tokens), then the sequence's draw counter advances by
+// the tokens emitted, as that many single-token b2_sample steps would advance it
+template <bool TREE>
+__global__ void spec_accept_sampled_kernel(int32_t* accepted, int32_t* path, int64_t* next_ids, int32_t* old_lens,
+                                           int32_t* new_lens, int64_t* tokens, const int64_t* pred, const int32_t* parents,
+                                           uint64_t* offsets, int batch, int q_len) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= batch) return;
+  offsets[b] += spec_accept_seq<TREE>(b, accepted, path, next_ids, old_lens, new_lens, tokens, pred, parents, q_len);
 }
 
 // vocab-split lm_head: pick the global winner among the ranks' (max, argmax) pairs under argmax_beats' order; ties (equal
@@ -524,6 +545,19 @@ int b2_spec_accept(int32_t* accepted, int64_t* next_ids, int32_t* old_lens, int3
 int b2_spec_accept_tree(int32_t* accepted, int32_t* path, int64_t* next_ids, int32_t* old_lens, int32_t* new_lens, int64_t* tokens,
                         const int64_t* pred, const int32_t* parents, int batch, int q_len, void* stream) {
   return spec_accept(accepted, path, next_ids, old_lens, new_lens, tokens, pred, parents, true, batch, q_len, stream);
+}
+
+int b2_spec_accept_sampled(int32_t* accepted, int32_t* path, int64_t* next_ids, int32_t* old_lens, int32_t* new_lens,
+                           int64_t* tokens, const int64_t* pred, const int32_t* parents, uint64_t* offsets, int batch, int q_len,
+                           void* stream) {
+  if (!accepted || !old_lens || !new_lens || !tokens || !pred || !offsets || !path != !parents || batch < 0) return B2_ERR_PARAM;
+  if (q_len < 1 || q_len > kMaxQLen) return B2_ERR_LIMIT;
+  if (batch == 0) return B2_OK;
+  B2_LAUNCH_CHECK("spec_accept_sampled",
+                  launch(parents ? spec_accept_sampled_kernel<true> : spec_accept_sampled_kernel<false>, dim3((batch + 127) / 128),
+                         dim3(128), 0, (cudaStream_t)stream, true, accepted, path, next_ids, old_lens, new_lens, tokens, pred,
+                         parents, offsets, batch, q_len));
+  return B2_OK;
 }
 
 }  // extern "C"

@@ -186,10 +186,14 @@ __device__ __forceinline__ void smp_select(SmpShared& sh, const uint16_t* st, in
   __syncthreads();
 }
 
-template <bool H>
-__global__ void __launch_bounds__(kSmpThreads) sample_kernel(int64_t* ids_out, const __nv_bfloat16* __restrict__ logits, int n,
-                                                             int64_t ld, const float* temperature, const int32_t* top_k,
-                                                             const float* top_p, const uint64_t* seeds, uint64_t* offsets) {
+// The draw of one row, by all threads of every CTA of the row's cluster.  Row r of logits takes the parameters at index q
+// and the Philox counter off: q = r and off = offsets[r] (b2_sample, which then advances offsets[r]), or, for STEP (row r =
+// b q_len + t of a verify step, b2_sample_tokens), q = b and off = offsets[b] + depth(t), with the offsets only read.
+// STEP selects nothing but that mapping.
+template <bool H, bool STEP>
+__device__ __forceinline__ void smp_rows(int64_t* ids_out, const __nv_bfloat16* logits, int n, int64_t ld,
+                                         const float* temperature, const int32_t* top_k, const float* top_p,
+                                         const uint64_t* seeds, uint64_t* offsets, int q_len, const int32_t* parents) {
   extern __shared__ __align__(16) uint16_t st[];
   __shared__ SmpShared sh;
   pdl_wait();
@@ -199,10 +203,16 @@ __global__ void __launch_bounds__(kSmpThreads) sample_kernel(int64_t* ids_out, c
   const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
   const int start = cta * chunk, len = min(chunk, n - start);
   const uint16_t* row = reinterpret_cast<const uint16_t*>(logits) + (size_t)r * ld + start;
-  const float t = temperature[r];
-  const int32_t k_in = top_k[r];
-  const float p = top_p[r];
-  const u64 seed = seeds[r], off = offsets[r];  // read by every CTA before the first cluster barrier; CTA 0 writes off + 1 last
+  const int q = STEP ? r / q_len : r;
+  int depth = 0;
+  if (STEP) {
+    depth = r - q * q_len;
+    if (parents) tree_walk(parents + (size_t)q * q_len, r - q * q_len, depth);
+  }
+  const float t = temperature[q];
+  const int32_t k_in = top_k[q];
+  const float p = top_p[q];
+  const u64 seed = seeds[q], off = offsets[q] + (u64)depth;  // read by every CTA before the first cluster barrier
 
   for (int i = tid; i < 256; i += kSmpThreads) {
     sh.cnt1[i] = 0;
@@ -383,8 +393,25 @@ __global__ void __launch_bounds__(kSmpThreads) sample_kernel(int64_t* ids_out, c
       }
     }
   }
-  cluster_sync();  // no CTA leaves while another reads its shared memory; every CTA has read offsets[r]
-  if (cta == 0 && tid == 0) offsets[r] = off + 1;
+  cluster_sync();  // no CTA leaves while another reads its shared memory; every CTA has read offsets[q]
+  if (!STEP && cta == 0 && tid == 0) offsets[r] = off + 1;
+}
+
+template <bool H>
+__global__ void __launch_bounds__(kSmpThreads) sample_kernel(int64_t* ids_out, const __nv_bfloat16* __restrict__ logits, int n,
+                                                             int64_t ld, const float* temperature, const int32_t* top_k,
+                                                             const float* top_p, const uint64_t* seeds, uint64_t* offsets) {
+  smp_rows<H, false>(ids_out, logits, n, ld, temperature, top_k, top_p, seeds, offsets, 1, nullptr);
+}
+
+template <bool H>
+__global__ void __launch_bounds__(kSmpThreads) sample_tokens_kernel(int64_t* ids_out, const __nv_bfloat16* __restrict__ logits,
+                                                                    int n, int64_t ld, int q_len, const int32_t* parents,
+                                                                    const float* temperature, const int32_t* top_k,
+                                                                    const float* top_p, const uint64_t* seeds,
+                                                                    const uint64_t* offsets) {
+  // STEP never writes offsets
+  smp_rows<H, true>(ids_out, logits, n, ld, temperature, top_k, top_p, seeds, const_cast<uint64_t*>(offsets), q_len, parents);
 }
 
 }  // namespace b2
@@ -412,6 +439,32 @@ int b2_sample(int64_t* ids_out, const void* logits, int rows, int n, int64_t ld,
   });
   if (e != cudaSuccess) {
     set_last_error("sample", e);
+    return B2_ERR_CUDA;
+  }
+  return B2_OK;
+}
+
+int b2_sample_tokens(int64_t* ids_out, const void* logits, int batch, int q_len, const int32_t* parents, int n, int64_t ld,
+                     const float* temperature, const int32_t* top_k, const float* top_p, const uint64_t* seeds,
+                     const uint64_t* offsets, int ft, void* stream) {
+  if (!ids_out || !logits || !temperature || !top_k || !top_p || !seeds || !offsets || batch < 0 || n < 1 || ld < n)
+    return B2_ERR_PARAM;
+  if (ft != B2_DT_BF16 && ft != B2_DT_F16) return B2_ERR_PARAM;
+  if (q_len < 1 || q_len > kMaxQLen || n > B2_SAMPLE_MAX_N || (int64_t)batch * q_len * smp_ctas(n) > INT_MAX) return B2_ERR_LIMIT;
+  if (batch == 0) return B2_OK;
+  const int nc = smp_ctas(n);
+  const size_t smem = ((size_t)smp_chunk(n) * 2 + 15) & ~(size_t)15;
+  const cudaError_t e = with_flag(ft == B2_DT_F16, [&](auto h) {
+    constexpr bool H = decltype(h)::value;
+    static const cudaError_t attr = cudaFuncSetAttribute(sample_tokens_kernel<H>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                         kSmpSplitMin * 2);
+    if (attr != cudaSuccess) return attr;
+    return launch_cluster(sample_tokens_kernel<H>, dim3((unsigned)(batch * q_len * nc)), dim3(kSmpThreads), smem,
+                          (cudaStream_t)stream, true, (unsigned)nc, ids_out, (const __nv_bfloat16*)logits, n, ld, q_len, parents,
+                          temperature, top_k, top_p, seeds, offsets);
+  });
+  if (e != cudaSuccess) {
+    set_last_error("sample_tokens", e);
     return B2_ERR_CUDA;
   }
   return B2_OK;

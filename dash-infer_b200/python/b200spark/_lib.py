@@ -21,6 +21,7 @@ SYMBOLS = [
     "b2_rmsnorm_ft", "b2_binary_ft", "b2_argmax_ft", "b2_qk_rmsnorm", "b2_span_cache_append_qknorm",
     "b2_rotary_table", "b2_span_cache_append_rope_table",
     "b2_logprobs", "b2_logprobs_partial_bytes", "b2_logprobs_shard", "b2_logprobs_merge", "b2_sample",
+    "b2_sample_tokens", "b2_spec_accept_sampled",
     "b2_history_load", "b2_history_append", "b2_penalize",
     "b2_comm_create", "b2_comm_destroy", "b2_comm_buffer_bytes", "b2_comm_export", "b2_comm_connect", "b2_comm_connect_pointers",
     "b2_comm_local_buffer", "b2_comm_error", "b2_allreduce", "b2_allgather", "b2_gemm_wq_run_allreduce",
@@ -146,6 +147,8 @@ def _load():
         "b2_logprobs_shard": (i32, [vp, vp, vp, i32, i32, i64, i64, i32, i32, vp]),
         "b2_logprobs_merge": (i32, [vp, vp, vp, vp, vp, i32, i32, i32, vp]),
         "b2_sample": (i32, [vp, vp, i32, i32, i64, vp, vp, vp, vp, vp, i32, vp]),
+        "b2_sample_tokens": (i32, [vp, vp, i32, i32, vp, i32, i64, vp, vp, vp, vp, vp, i32, vp]),
+        "b2_spec_accept_sampled": (i32, [vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, vp]),
         "b2_history_load": (i32, [C.POINTER(TokenHistory), i32, vp, i32, i32, vp]),
         "b2_history_append": (i32, [C.POINTER(TokenHistory), vp, i32, vp]),
         "b2_penalize": (i32, [vp, i32, i32, i64, i64, C.POINTER(TokenHistory), C.POINTER(PenaltyParams), i32, vp]),

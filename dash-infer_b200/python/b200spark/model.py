@@ -139,7 +139,7 @@ class DecodeStack:
     def __init__(self, cfg, batch, max_len, wbits=4, group=-1, kv="none", span=128, seed=1234, device="cuda",
                  keep_ref=False, layers=None, tp_rank=0, tp_size=1, tp_group=None, fuse_swiglu=True,
                  collective=None, comm=None, dtype=torch.bfloat16, q_len=1, tree=False, logprobs=0, sample=False,
-                 penalties=False):
+                 penalties=False, sampled_verify=False):
         """tp_size > 1: the reference's tensor-parallel layout (QKV/gate/up column split, o/down row split + all-reduce,
         vocab-split lm_head + B-element all-gather); every rank builds the SAME full synthetic weights from `seed` and
         keeps its shard, exactly like the reference splits an already-quantized checkpoint.
@@ -166,7 +166,14 @@ class DecodeStack:
         its vocab shard), so the argmax, b2_sample and b2_logprobs all see the processed row; the step then appends next_ids
         to a per-sequence token history on the device (one launch each).  set_history(b, ids, prompt_len) loads sequence
         b's tokens, set_penalties() writes the per-sequence parameters in place (neutral until written).  self.history and
-        self.penalties are the views of the current batch; capture() leaves the history as it found it."""
+        self.penalties are the views of the current batch; capture() leaves the history as it found it.
+        sampled_verify=True (q_len = T > 1, chain or tree, one GPU): sampled speculative verification.  The step draws every
+        row with b2_sample_tokens in place of the argmax (row b*T + u at sequence b's counter offsets[b] + depth(u), with
+        sequence b's parameters, kept and written as for sample=True) and accepts along the draws with
+        b2_spec_accept_sampled, which also advances offsets[b] by accepted[b]; the launch count is the greedy verify step's.
+        step() returns what a verify step returns, the emitted tokens are pred[b, :accepted[b]] (pred[b, path[b, :accepted[b]]]
+        in a tree), and they are exactly the tokens single-token sampling would draw from the same rows and seeds.  With
+        logprobs = N, b2_logprobs runs at the drawn ids (one launch more): tok_lp at row b*T + u is the logprob of pred[b, u]."""
         global _DT
         assert dtype in (torch.bfloat16, torch.float16) and (dtype == torch.bfloat16 or (tp_size == 1 and cfg.head == 128)), \
             "fp16: single GPU, head size 128 (the communicator and the head-64 kernels are bf16)"
@@ -177,10 +184,13 @@ class DecodeStack:
         assert cfg.rope_scaling is None or cfg.head == 128, "rope scaling: head size 128"
         assert 0 <= logprobs <= ops._lib.MAX_TOP_LOGPROBS, "logprobs: 0 .. 10 alternatives"
         assert not sample or (q_len == 1 and tp_size == 1), \
-            "sample=True: single-token steps (q_len == 1) on one GPU (tp_size == 1); greedy verification stays greedy"
+            "sample=True: single-token steps (q_len == 1) on one GPU (tp_size == 1); sampled verify steps: sampled_verify=True"
+        assert not sampled_verify or (q_len > 1 and tp_size == 1 and not sample and not penalties), \
+            "sampled_verify=True: multi-token or tree steps (q_len > 1) on one GPU (tp_size == 1), without sample=True, and " \
+            "without penalties=True (the history is not kept per draft position)"
         assert not penalties or q_len == 1, \
             "penalties=True: single-token steps (q_len == 1); the history is not kept per draft position"
-        self.logprobs, self.sample, self.pen = logprobs, sample, penalties
+        self.logprobs, self.sample, self.pen, self.sv = logprobs, sample, penalties, sampled_verify
         self.dtype = _DT = dtype
         self.q_len, self.tree = q_len, tree
         rows = batch * q_len  # activation rows of a step
@@ -246,7 +256,7 @@ class DecodeStack:
         self._lens_new = torch.full((batch,), q_len, dtype=torch.int32, device=device)  # lens_old + q_len
         self._ids = torch.zeros(batch, dtype=torch.int64, device=device)
         self._next_ids = torch.zeros(batch, dtype=torch.int64, device=device)
-        if sample:
+        if sample or sampled_verify:
             self._temperature = torch.ones(batch, dtype=torch.float32, device=device)
             self._top_k = torch.zeros(batch, dtype=torch.int32, device=device)
             self._top_p = torch.ones(batch, dtype=torch.float32, device=device)
@@ -305,7 +315,7 @@ class DecodeStack:
             self.tokens, self.pred, self.accepted = self._tokens[:b], self._pred[:b], self._accepted[:b]
         if self.tree:
             self.parents, self.path = self._parents[:b], self._path[:b]
-        if self.sample:
+        if self.sample or self.sv:
             for k in ("temperature", "top_k", "top_p", "seeds", "offsets"):
                 setattr(self, k, getattr(self, "_" + k)[:b])
         if self.pen:
@@ -317,7 +327,7 @@ class DecodeStack:
 
     def set_sampling(self, temperature=None, top_k=None, top_p=None, seeds=None, offsets=None):
         """Write the sampling parameters of the current batch in place (a scalar or [B] values each; None keeps the value)."""
-        assert self.sample, "set_sampling: the stack was built with sample=False"
+        assert self.sample or self.sv, "set_sampling: the stack was built with sample=False and sampled_verify=False"
         for k, v in (("temperature", temperature), ("top_k", top_k), ("top_p", top_p), ("seeds", seeds), ("offsets", offsets)):
             if v is not None:
                 t = getattr(self, k)
@@ -465,7 +475,13 @@ class DecodeStack:
             self.lm_head(self.xn, ws, out=self.logits); n += 1
         if self.pen:  # the logits processor, in place on this rank's vocab shard
             ops.penalize(self.logits, self.history, self.penalties, self.tp_rank * self.vocab_l); n += 1
-        if self.sample:  # the drawn ids; with logprobs, the log-probabilities at them (one launch more)
+        if self.sv:  # every row's draw; with logprobs, the log-probabilities at them (one launch more)
+            ops.sample_tokens(self.logits, T, self.temperature, self.top_k, self.top_p, self.seeds, self.offsets,
+                              self.parents if self.tree else None, out=self.pred.view(-1)); n += 1
+            if self.logprobs:
+                ops.logprobs(self.logits, self.logprobs, tok_ids=self.pred.view(-1), out=(None, self.tok_lp, self.top_ids, self.top_lp))
+                n += 1
+        elif self.sample:  # the drawn ids; with logprobs, the log-probabilities at them (one launch more)
             ops.sample(self.logits, self.temperature, self.top_k, self.top_p, self.seeds, self.offsets, out=self.next_ids); n += 1
             if self.logprobs:
                 ops.logprobs(self.logits, self.logprobs, tok_ids=self.next_ids, out=(None, self.tok_lp, self.top_ids, self.top_lp))
@@ -492,9 +508,10 @@ class DecodeStack:
                 self.comm.allgather(self.loc_val, self.all_val); n += 1
                 self.comm.allgather(self.loc_ids, self.all_ids); n += 1
             ops.argmax_merge(self.all_val, self.all_ids, out=self.next_ids); n += 1  # lowest rank on ties == lowest vocab id
-        if T > 1:  # greedy verification: accepted counts, next token and lengths stay on the device
+        if T > 1:  # verification: accepted counts, next token, lengths (and the draw counters) stay on the device
             ops._spec_accept(self.accepted, self.next_ids, self.lens_old, self.lens_new, self.tokens, self.pred,
-                             self.path if self.tree else None, self.parents if self.tree else None); n += 1
+                             self.path if self.tree else None, self.parents if self.tree else None,
+                             self.offsets if self.sv else None); n += 1
             if self.tree:  # the accepted path's rows move to consecutive slots in every layer
                 ops.cache_compact([L["cache"] for L in self.layers], self.lens_old, self.accepted, self.path, T); n += 1
         else:
@@ -532,7 +549,7 @@ class DecodeStack:
         """Warm up once eagerly (plans, workspace growth), rewind the lengths, then capture one step."""
         lo, ln = self.lens_old.clone(), self.lens_new.clone()
         tk = self.tokens.clone() if self.q_len > 1 else None  # the accept kernel rewrites column 0
-        off = self.offsets.clone() if self.sample else None  # the warm-up step advances the draw counters
+        off = self.offsets.clone() if self.sample or self.sv else None  # the warm-up step advances the draw counters
         hist = self.history.snapshot() if self.pen else None  # ... and appends a token to the history
         self._step_ops()
         torch.cuda.synchronize()

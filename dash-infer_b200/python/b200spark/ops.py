@@ -395,19 +395,28 @@ def cache_append_tree(cache, qkv, old_lens, parents, q_len, q_out=None, rope=Non
     return _cache_append(cache, qkv, old_lens, q_out, rope, q_len, parents)
 
 
-def _spec_accept(accepted, next_ids, old_lens, new_lens, tokens, pred, path=None, parents=None):
+def _spec_accept(accepted, next_ids, old_lens, new_lens, tokens, pred, path=None, parents=None, offsets=None):
     """Greedy verification of a multi-token step (b2_spec_accept): tokens / pred int64 [B, T]; writes accepted (int32 [B]),
     next_ids (int64 [B] or None) and tokens[:, 0], advances old_lens by the accepted counts and sets new_lens = old_lens + T.
     With parents (int32 [B, T]) the step is a draft tree (b2_spec_accept_tree), which also writes path (int32 [B, T], the first
-    accepted[b] entries)."""
+    accepted[b] entries).  With offsets (int64 [B], the sequences' draw counters) pred holds sample_tokens' draws and the
+    sampled form runs (b2_spec_accept_sampled): the same walk, then offsets += accepted."""
     B, T = tokens.shape
     assert tokens.is_contiguous() and pred.is_contiguous() and pred.shape == tokens.shape
+    if parents is not None:
+        assert parents.dtype == torch.int32 and parents.is_contiguous() and parents.shape == tokens.shape
+        assert path.dtype == torch.int32 and path.is_contiguous() and path.shape == tokens.shape
+    if offsets is not None:
+        assert offsets.dtype == torch.int64 and offsets.is_contiguous() and tuple(offsets.shape) == (B,), \
+            f"spec_accept: offsets must be [{B}] int64 contiguous"
+        check(lib.b2_spec_accept_sampled(_ptr(accepted), _ptr(path), _ptr(next_ids), _ptr(old_lens), _ptr(new_lens),
+                                         _ptr(tokens), _ptr(pred), _ptr(parents), _ptr(offsets), B, T, _stream()),
+              "b2_spec_accept_sampled")
+        return accepted if parents is None else (accepted, path)
     if parents is None:
         check(lib.b2_spec_accept(_ptr(accepted), _ptr(next_ids), _ptr(old_lens), _ptr(new_lens), _ptr(tokens), _ptr(pred), B, T,
                                  _stream()), "b2_spec_accept")
         return accepted
-    assert parents.dtype == torch.int32 and parents.is_contiguous() and parents.shape == tokens.shape
-    assert path.dtype == torch.int32 and path.is_contiguous() and path.shape == tokens.shape
     check(lib.b2_spec_accept_tree(_ptr(accepted), _ptr(path), _ptr(next_ids), _ptr(old_lens), _ptr(new_lens), _ptr(tokens),
                                   _ptr(pred), _ptr(parents), B, T, _stream()), "b2_spec_accept_tree")
     return accepted, path
@@ -651,6 +660,13 @@ def logprobs_merge(all_partials, n_top, out=None):
     return ids, tok_lp, top_ids, top_lp
 
 
+def _sampling_args(rows, B, out, temperature, top_k, top_p, seeds, offsets, what):
+    for t, dt, name, n in ((out, torch.int64, "out", rows), (temperature, torch.float32, "temperature", B),
+                           (top_k, torch.int32, "top_k", B), (top_p, torch.float32, "top_p", B), (seeds, torch.int64, "seeds", B),
+                           (offsets, torch.int64, "offsets", B)):
+        assert t.dtype == dt and t.is_contiguous() and tuple(t.shape) == (n,), f"{what}: {name} must be [{n}] {dt} contiguous"
+
+
 def sample(logits, temperature, top_k, top_p, seeds, offsets, out=None):
     """A token drawn from each row of logits [rows, n] FT (b2_sample; any row stride): temperature, top_p fp32 [rows], top_k
     int32 [rows], seeds, offsets int64 [rows] (read as uint64 bits), all on the device.  Advances offsets by 1 in place and
@@ -658,11 +674,26 @@ def sample(logits, temperature, top_k, top_p, seeds, offsets, out=None):
     rows, n = logits.shape
     assert logits.stride(-1) == 1
     out = torch.empty(rows, dtype=torch.int64, device=logits.device) if out is None else out
-    for t, dt, name in ((out, torch.int64, "out"), (temperature, torch.float32, "temperature"), (top_k, torch.int32, "top_k"),
-                        (top_p, torch.float32, "top_p"), (seeds, torch.int64, "seeds"), (offsets, torch.int64, "offsets")):
-        assert t.dtype == dt and t.is_contiguous() and tuple(t.shape) == (rows,), f"sample: {name} must be [{rows}] {dt} contiguous"
+    _sampling_args(rows, rows, out, temperature, top_k, top_p, seeds, offsets, "sample")
     check(lib.b2_sample(_ptr(out), _ptr(logits), rows, n, logits.stride(0), _ptr(temperature), _ptr(top_k), _ptr(top_p),
                         _ptr(seeds), _ptr(offsets), _ft(logits), _stream()), "b2_sample")
+    return out
+
+
+def sample_tokens(logits, q_len, temperature, top_k, top_p, seeds, offsets, parents=None, out=None):
+    """The draws of a verify step (b2_sample_tokens): logits [B * q_len, n] FT (any row stride), row b*q_len + t = draft node
+    t of sequence b, drawn with sequence b's parameters (temperature, top_k, top_p, seeds, offsets: [B], as for sample()) at
+    counter offsets[b] + depth(t) (t for a chain; parents int32 [B, q_len] for a draft tree).  The offsets are only read.
+    Returns the ids, int64 [B * q_len] (out, if given)."""
+    rows, n = logits.shape
+    assert logits.stride(-1) == 1 and q_len >= 1 and rows % q_len == 0, "sample_tokens: logits rows = B * q_len"
+    B = rows // q_len
+    out = torch.empty(rows, dtype=torch.int64, device=logits.device) if out is None else out
+    _sampling_args(rows, B, out, temperature, top_k, top_p, seeds, offsets, "sample_tokens")
+    assert parents is None or (parents.dtype == torch.int32 and parents.is_contiguous() and tuple(parents.shape) == (B, q_len)), \
+        f"sample_tokens: parents must be [{B}, {q_len}] int32 contiguous"
+    check(lib.b2_sample_tokens(_ptr(out), _ptr(logits), B, q_len, _ptr(parents), n, logits.stride(0), _ptr(temperature),
+                               _ptr(top_k), _ptr(top_p), _ptr(seeds), _ptr(offsets), _ft(logits), _stream()), "b2_sample_tokens")
     return out
 
 

@@ -451,6 +451,17 @@ int b2_logprobs_merge(int64_t* ids_out, float* tok_lp, int64_t* top_ids, float* 
 #define B2_SAMPLE_MAX_N 262144
 int b2_sample(int64_t* ids_out, const void* logits, int rows, int n, int64_t ld, const float* temperature,
               const int32_t* top_k, const float* top_p, const uint64_t* seeds, uint64_t* offsets, int ft, void* stream);
+/* The step form of b2_sample, for sampled verification of a multi-token or tree step.  logits [batch q_len, ld] FT; row
+ * r = b q_len + t is draft node t of sequence b (tree format: b2_span_cache_append_tree; parents NULL: a chain).  Row r is
+ * drawn by b2_sample's steps 1-6 with sequence b's parameters temperature[b], top_k[b], top_p[b], seeds[b] (all [batch])
+ * and the counter off = offsets[b] + depth(t), depth(t) the parent steps from node t to the root (t for a chain): ids_out[r]
+ * equals b2_sample's id for that row at offsets[b] = off, bit for bit.  The offsets are read, not written; q_len = 1 gives
+ * b2_sample's ids without advancing them.  Same per-row decomposition as b2_sample (one CTA, or a cluster of 8 above 32768
+ * columns).  A NULL required pointer, n < 1, ld < n, batch < 0, ft other than bf16 / fp16: B2_ERR_PARAM; q_len outside
+ * [1, 16] or n > B2_SAMPLE_MAX_N: B2_ERR_LIMIT; all before any launch.  batch = 0 launches nothing. */
+int b2_sample_tokens(int64_t* ids_out, const void* logits, int batch, int q_len, const int32_t* parents /* NULL: chain */,
+                     int n, int64_t ld, const float* temperature, const int32_t* top_k, const float* top_p,
+                     const uint64_t* seeds, const uint64_t* offsets, int ft, void* stream);
 /* Per-sequence token history on the device (the in_ids / cur_len / input_len of the reference's logits processor).  Every
  * array has `rows` slots (row r of a step uses slot r); all pointers are device memory, zero-initialised before first use.
  *   tokens     int32 [rows][max_len]  the sequence, prompt first; an id outside [0, vocab) is stored as -1
@@ -538,6 +549,20 @@ int b2_spec_accept(int32_t* accepted, int64_t* next_ids, int32_t* old_lens, int3
  * are pred[b][path[b][i]], i < n.  A chain gives b2_spec_accept's results. */
 int b2_spec_accept_tree(int32_t* accepted, int32_t* path, int64_t* next_ids, int32_t* old_lens, int32_t* new_lens,
                         int64_t* tokens, const int64_t* pred, const int32_t* parents, int batch, int q_len, void* stream);
+/* Sampled verification of a chain (parents and path NULL) or a draft tree.  pred [batch][q_len] = b2_sample_tokens' draws
+ * of the step's rows.  The walk, the outputs and the lengths are b2_spec_accept's (chain) or b2_spec_accept_tree's (tree)
+ * over these draws; then offsets[b] += accepted[b].  The step emits pred[b][0 .. n_b-1] (pred[b][path[b][i]] in a tree).
+ * Exactness: a node at depth d of the accepted path is drawn at counter offsets[b] + d after the accepted prefix and the d
+ * tokens drawn before it, which is the context and the counter of single-token step d.  So when every row's logits equal
+ * those of the single-token steps, the emitted tokens are exactly the next n_b tokens b2_sample would draw from the same
+ * seed, and the offsets end where those n_b steps leave them.  The drafts decide only how many tokens a step emits, never
+ * which, so the output distribution is single-token sampling's for any drafter; a draft token of weight 0 is never
+ * accepted.  With every temperature <= 0 the draws are argmax ids, and every output but the offsets equals greedy
+ * verification's.  A NULL required pointer, path NULL while parents is not (or the reverse), batch < 0: B2_ERR_PARAM;
+ * q_len outside [1, 16]: B2_ERR_LIMIT; before any launch.  batch = 0 launches nothing. */
+int b2_spec_accept_sampled(int32_t* accepted, int32_t* path /* NULL iff parents is NULL */, int64_t* next_ids /* or NULL */,
+                           int32_t* old_lens, int32_t* new_lens, int64_t* tokens, const int64_t* pred,
+                           const int32_t* parents /* NULL: chain */, uint64_t* offsets, int batch, int q_len, void* stream);
 /* Move the accepted path's K/V rows to consecutive slots, in every layer with one launch.  k_tables / v_tables: device
  * arrays of n_layers span-table pointers (each table [batch][max_spans_per_seq], as for the other span entry points).  With
  * base = old_lens[b] - accepted[b] (the lengths as b2_spec_accept_tree left them), slot base + path[b][i] is copied to slot

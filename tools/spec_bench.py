@@ -22,10 +22,21 @@ Usage (the DESIGN.md §5 table): python tools/spec_bench.py --steps 30 --warmup 
 Replaying the same tree step stays valid after compaction: the step rewrites all T slots past the restored length before
 anything reads them, and compaction only writes inside those slots.
 Usage (the DESIGN.md §5 tree table): python tools/spec_bench.py --tree --steps 30 --warmup 5
+
+--sample: sampled verification (DecodeStack(sampled_verify=True)) against greedy verification on the same stack, for T in
+{4, 8, 16}, batch 1 and 8, chains and trees, at t = 0.7, k = 50, p = 0.9:
+  * ms per CUDA-graph-replayed step of each, alternated over --rounds rounds: medians and the spread (min, max);
+  * µs per launch of b2_sample_tokens and of b2_argmax on [B*T, 152064] bf16 rows (a graph of 20 launches);
+  * accepted tokens/s of the sampled step for two draft sets: "own", the continuation a single-token sampled stack
+    (sample=True, same weights, caches, seeds and offsets) draws, on a chain, or on a tree's last branch behind a first
+    branch of random drafts; "random", random drafts (and random parents).  "own" is not accepted whole: verify rows pass
+    the GEMMs at M = B*T, so their logits differ from the single-token step's by rounding, and a draw can change.
+Usage (the DESIGN.md §5 sampled-verification table): python tools/spec_bench.py --sample --steps 30 --warmup 5
 """
 import argparse
 import json
 import os
+import statistics
 import subprocess
 import sys
 
@@ -160,16 +171,116 @@ def tree_main(args, name, power):
                       "tree": True, "results": res}))
 
 
+def sample_main(args, name, power):
+    from b200spark import ops
+    cfg = model.QWEN2_7B
+    t, k, p = 0.7, 50, 0.9
+    gen = torch.Generator(device="cuda").manual_seed(8)
+    seeds, offs = torch.arange(8, dtype=torch.int64, device="cuda") * 7919 + 1, torch.full((8,), 1000, dtype=torch.int64,
+                                                                                          device="cuda")
+    one = model.DecodeStack(cfg, 8, args.ctx + 64, wbits=4, group=-1, kv="none", span=128, sample=True)
+    one.set_context(args.ctx)
+    one.set_sampling(temperature=t, top_k=k, top_p=p, seeds=seeds, offsets=offs)
+    first = torch.randint(0, cfg.vocab, (8,), generator=gen, device="cuda")
+
+    def continuation(B, n):
+        """the single-token sampled stack's next n tokens after `first`, from the context and offsets of the verify step"""
+        one.set_batch(B)
+        one.lens_old.fill_(args.ctx); one.lens_new.fill_(args.ctx + 1)
+        one.offsets.copy_(offs[:B]); one.ids.copy_(first[:B])
+        out = []
+        for _ in range(n):
+            out.append(one.step().clone())
+            one.ids.copy_(out[-1])
+        return torch.stack(out, 1)
+
+    res = []
+    for T in (4, 8, 16):
+        st = model.DecodeStack(cfg, 8, args.ctx + 64, wbits=4, group=-1, kv="none", span=128, q_len=T, tree=True,
+                               sampled_verify=True)
+        st.set_context(args.ctx)
+        h = T // 2
+        own_tree = [0] + [0 if u in (1, h) else u - 1 for u in range(1, T)]  # nodes 1 .. h-1 and h .. T-1: two branches
+        for B in (8, 1):
+            st.set_batch(B)
+            st.set_sampling(temperature=t, top_k=k, top_p=p, seeds=seeds[:B], offsets=offs[:B])
+            lo, ln, off0 = st.lens_old.clone(), st.lens_new.clone(), st.offsets.clone()
+            cont = continuation(B, T)
+            lg = (torch.randn(B * T, cfg.vocab, generator=gen, device="cuda") * 3).to(torch.bfloat16)
+            ids = torch.empty(B * T, dtype=torch.int64, device="cuda")
+            cpu_gen = torch.Generator().manual_seed(7 + T + B)
+            par_rnd = torch.tensor([[0] + [int(torch.randint(0, u, (1,), generator=cpu_gen).item()) for u in range(1, T)]
+                                    for _ in range(B)], dtype=torch.int32, device="cuda")
+            launches = {"argmax": lambda: ops.argmax(lg, out=ids),
+                        "sample_tokens": lambda: ops.sample_tokens(lg, T, st.temperature, st.top_k, st.top_p, st.seeds, st.offsets,
+                                                                   parents=par_rnd, out=ids)}
+            for form in ("chain", "tree"):
+                st.tree = form == "tree"
+                rnd = torch.cat([first[:B, None], torch.randint(0, cfg.vocab, (B, T - 1), generator=gen, device="cuda")], 1)
+                own = rnd.clone()
+                if st.tree:
+                    own[:, h:] = cont[:, :T - h]
+                else:
+                    own[:, 1:] = cont[:, :T - 1]
+                row = {"batch": B, "q_len": T, "form": form}
+                graphs = {}
+                for mode in ("greedy", "sampled"):
+                    st.sv = mode == "sampled"
+                    if st.tree:
+                        st.parents.copy_(torch.tensor([own_tree] * B, dtype=torch.int32))
+                    st.tokens.copy_(own)
+                    graphs[mode] = st.capture()
+                for drafts, (tokens, par) in {"own": (own, own_tree), "random": (rnd, None)}.items():
+                    if st.tree:
+                        st.parents.copy_(par_rnd if par is None else torch.tensor([par] * B, dtype=torch.int32))
+
+                    def step():
+                        st.graph.replay()
+                        st.lens_old.copy_(lo); st.lens_new.copy_(ln)
+                        st.tokens.copy_(tokens); st.offsets.copy_(off0)
+
+                    ms = {"greedy": [], "sampled": []}
+                    for _ in range(args.rounds):  # alternated
+                        for mode in ms:
+                            st.graph = graphs[mode]
+                            ms[mode].append(time_ms(step, args.steps, args.warmup))
+                    st.graph = graphs["sampled"]
+                    step()
+                    acc = int(st.accepted.sum().item())
+                    for mode, v in ms.items():
+                        row["ms_%s_%s" % (mode, drafts)] = round(statistics.median(v), 4)
+                        row["ms_%s_%s_spread" % (mode, drafts)] = [round(min(v), 4), round(max(v), 4)]
+                    row["cost_pct_" + drafts] = round(100 * (statistics.median(ms["sampled"]) / statistics.median(ms["greedy"]) - 1), 2)
+                    row["accepted_" + drafts] = acc
+                    row["tok_s_" + drafts] = round(acc / statistics.median(ms["sampled"]) * 1e3, 1)
+                res.append(row)
+                print(json.dumps(row), file=sys.stderr, flush=True)
+            us = {}
+            for name_, f in launches.items():
+                g = graph_of(lambda: [f() for _ in range(20)])
+                us[name_] = round(1e3 * time_ms(g.replay, 10, 3) / 20, 2)
+            res[-1]["launch_us"] = res[-2]["launch_us"] = us
+            st.sv, st.graph = True, None
+        del st
+        torch.cuda.empty_cache()
+    print(json.dumps({"gpu": name, "power_limit": power, "model": "Qwen2-7B int4 per-channel, bf16 KV", "ctx": args.ctx,
+                      "sample": {"temperature": t, "top_k": k, "top_p": p}, "rounds": args.rounds, "results": res}))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=30)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--ctx", type=int, default=2048)
     ap.add_argument("--tree", action="store_true", help="draft trees against chains (T = 4, 8, 16)")
+    ap.add_argument("--sample", action="store_true", help="sampled against greedy verification (T = 4, 8, 16)")
+    ap.add_argument("--rounds", type=int, default=5, help="--sample: alternations of the greedy / sampled measurements")
     args = ap.parse_args()
     name, power = gpu_info()
     if args.tree:
         return tree_main(args, name, power)
+    if args.sample:
+        return sample_main(args, name, power)
     res = []
     gen = torch.Generator(device="cuda").manual_seed(5)
     for T in (1, 2, 4, 8):
