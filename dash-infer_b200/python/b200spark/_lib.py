@@ -22,6 +22,7 @@ SYMBOLS = [
     "b2_rotary_table", "b2_span_cache_append_rope_table",
     "b2_logprobs", "b2_logprobs_partial_bytes", "b2_logprobs_shard", "b2_logprobs_merge", "b2_sample",
     "b2_sample_tokens", "b2_spec_accept_sampled",
+    "b2_sample_shard_record_bytes", "b2_sample_shard_state_bytes", "b2_sample_shard", "b2_sample_shard_merge",
     "b2_history_load", "b2_history_append", "b2_penalize",
     "b2_comm_create", "b2_comm_destroy", "b2_comm_buffer_bytes", "b2_comm_export", "b2_comm_connect", "b2_comm_connect_pointers",
     "b2_comm_local_buffer", "b2_comm_error", "b2_allreduce", "b2_allgather", "b2_gemm_wq_run_allreduce",
@@ -77,6 +78,7 @@ KV_FP8 = 3  # extension (not a span::QuantMode value): fp8-e4m3 KV cache, head 1
 COMM_HANDLE_BYTES = 64
 MAX_TOP_LOGPROBS = 10  # B2_MAX_TOP_LOGPROBS
 SAMPLE_MAX_N = 262144  # B2_SAMPLE_MAX_N
+SAMPLE_SHARD_PHASES = 6  # B2_SAMPLE_SHARD_PHASES
 
 
 class B2Error(RuntimeError):
@@ -149,6 +151,10 @@ def _load():
         "b2_sample": (i32, [vp, vp, i32, i32, i64, vp, vp, vp, vp, vp, i32, vp]),
         "b2_sample_tokens": (i32, [vp, vp, i32, i32, vp, i32, i64, vp, vp, vp, vp, vp, i32, vp]),
         "b2_spec_accept_sampled": (i32, [vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, vp]),
+        "b2_sample_shard_record_bytes": (sz, [i32]),
+        "b2_sample_shard_state_bytes": (sz, []),
+        "b2_sample_shard": (i32, [i32, vp, vp, vp, i32, vp, i32, i32, i64, i64, i64, vp, vp, vp, vp, vp, i32, vp]),
+        "b2_sample_shard_merge": (i32, [vp, vp, vp, i32, i32, vp, vp]),
         "b2_history_load": (i32, [C.POINTER(TokenHistory), i32, vp, i32, i32, vp]),
         "b2_history_append": (i32, [C.POINTER(TokenHistory), vp, i32, vp]),
         "b2_penalize": (i32, [vp, i32, i32, i64, i64, C.POINTER(TokenHistory), C.POINTER(PenaltyParams), i32, vp]),

@@ -142,7 +142,9 @@ class DecodeStack:
                  penalties=False, sampled_verify=False):
         """tp_size > 1: the reference's tensor-parallel layout (QKV/gate/up column split, o/down row split + all-reduce,
         vocab-split lm_head + B-element all-gather); every rank builds the SAME full synthetic weights from `seed` and
-        keeps its shard, exactly like the reference splits an already-quantized checkpoint.
+        keeps its shard, exactly like the reference splits an already-quantized checkpoint.  A rank reaches its peers through
+        an initialised torch.distributed process group, or through a connected `comm` (collective "b2" / "fused"); a stack
+        with neither is refused before any weight is built.
         q_len = T > 1: multi-token verify steps (speculative decoding).  Every step runs T rows per sequence: self.tokens
         [B, T] holds the last emitted token (column 0, written by the step itself) and T-1 drafts (filled by the caller);
         step() returns (pred [B, T], accepted [B]) and advances the lengths by the accepted counts on the device.
@@ -155,13 +157,20 @@ class DecodeStack:
         [B*T] fp32 (the logprob of each row's own argmax), self.top_ids [B*T, N] int64 and self.top_lp [B*T, N] fp32 (the N
         most likely tokens, argmax order).  Every row of a multi-token or tree step gets them; the logprob of an emitted token
         is tok_lp at its row: row b*T + u for the token pred[b, u] (u = path[b, j] in a tree).  N = 0 runs today's step.
-        sample=True (q_len 1, one GPU): the step draws next_ids with b2_sample in place of the argmax, with the same launch
+        sample=True (q_len 1): the step draws next_ids with b2_sample in place of the argmax, with the same launch
         count.  The per-sequence parameters live on the device, [B] each: self.temperature (fp32, default 1.0), self.top_k
         (int32, 0 = no limit), self.top_p (fp32, 1.0), self.seeds and self.offsets (int64, 0); set_sampling() writes them in
         place, so a captured graph stays valid, and every step advances the offsets by 1.  With logprobs = N the step runs
         b2_sample, then b2_logprobs at the drawn ids (one launch more): tok_lp is the logprob of the sampled token under the
         model's distribution, before temperature and filtering (as the reference reports it), and top_ids / top_lp the N most
         likely tokens of that distribution.
+        sample=True with tp_size > 1: every rank draws b2_sample's id of the whole row from its vocab shard, bit for bit
+        (b2_sample_shard: six phases, each followed by an all-gather of small per-row records, then b2_sample_shard_merge)
+        in place of argmax_shard, its two all-gathers and the merge.  The caller writes the same parameters on every rank.
+        That is 9 launches more than the greedy TP step with collective "b2" or "fused" (7 kernels and 6 all-gathers in place
+        of 4 launches) and 5 more with "nccl" (whose all-gathers are not counted).  With logprobs = N, b2_logprobs_shard at
+        the drawn ids, the all-gather of its records and b2_logprobs_merge follow, as in the greedy TP step: 13 launches
+        more than that step with "b2" / "fused", 7 with "nccl".
         penalties=True (q_len 1): the reference's logits processor runs on the lm_head's output (b2_penalize; each TP rank
         its vocab shard), so the argmax, b2_sample and b2_logprobs all see the processed row; the step then appends next_ids
         to a per-sequence token history on the device (one launch each).  set_history(b, ids, prompt_len) loads sequence
@@ -183,13 +192,22 @@ class DecodeStack:
         assert not cfg.qk_norm or cfg.head == 128, "per-head Q/K norm: head size 128"
         assert cfg.rope_scaling is None or cfg.head == 128, "rope scaling: head size 128"
         assert 0 <= logprobs <= ops._lib.MAX_TOP_LOGPROBS, "logprobs: 0 .. 10 alternatives"
-        assert not sample or (q_len == 1 and tp_size == 1), \
-            "sample=True: single-token steps (q_len == 1) on one GPU (tp_size == 1); sampled verify steps: sampled_verify=True"
+        assert not sample or q_len == 1, "sample=True: single-token steps (q_len == 1); sampled verify steps: sampled_verify=True"
         assert not sampled_verify or (q_len > 1 and tp_size == 1 and not sample and not penalties), \
             "sampled_verify=True: multi-token or tree steps (q_len > 1) on one GPU (tp_size == 1), without sample=True, and " \
             "without penalties=True (the history is not kept per draft position)"
         assert not penalties or q_len == 1, \
             "penalties=True: single-token steps (q_len == 1); the history is not kept per draft position"
+        import os
+
+        import torch.distributed as dist
+        collective = collective or os.environ.get("B2_TP_COLLECTIVE", "b2")
+        # a rank reaches its peers through a torch.distributed process group (the "nccl" collectives, and the handle
+        # exchange that connects the communicator), or through a communicator the caller connected; refuse before any
+        # weight is built rather than fail in the first exchange
+        assert tp_size == 1 or (dist.is_available() and dist.is_initialized()) or (comm is not None and collective != "nccl"), \
+            "tp_size > 1: initialise a torch.distributed process group (or pass a connected comm with collective 'b2' / " \
+            "'fused') first; a stack without peers runs with tp_size == 1"
         self.logprobs, self.sample, self.pen, self.sv = logprobs, sample, penalties, sampled_verify
         self.dtype = _DT = dtype
         self.q_len, self.tree = q_len, tree
@@ -199,8 +217,7 @@ class DecodeStack:
         # tensor-parallel exchange: "fused" = all-reduce inside the row-parallel GEMV's epilogue (b2_gemm_wq_run_allreduce;
         # batches <= 16, else it degrades to "b2"), "b2" = GEMM + b2_allreduce (one-shot over NVLink peer memory, residual
         # fused), "nccl" = torch.distributed all_reduce + copy (the baseline the reference's AllReduceOp amounts to)
-        import os
-        self.collective = collective or os.environ.get("B2_TP_COLLECTIVE", "b2")
+        self.collective = collective
         self.comm = comm
         self.fuse_swiglu = fuse_swiglu
         self.group_size, self.wbits = group, wbits
@@ -286,8 +303,11 @@ class DecodeStack:
             if logprobs:  # one record per row and rank (b2_logprobs_shard), all-gathered as bytes
                 self._bufs["loc_rec"] = torch.empty(batch, rec, dtype=torch.uint8, device=device)
                 self._all_rec = torch.empty(tp * batch * rec, dtype=torch.uint8, device=device)
-            if self.collective != "nccl" and self.comm is None:
-                self.comm = ops.Comm(tp_rank, tp, max(batch * H * 2, 4096, batch * rec)).connect_group(tp_group)
+            if sample:  # this rank's state and records of the vocab-split draw (b2_sample_shard), for the construction batch
+                self._stp = ops.sample_tp_buffers(batch, tp, device)
+            if self.collective != "nccl" and self.comm is None:  # the largest exchange: activations, or a phase-1 record
+                rec_max = max(rec, ops.sample_shard_record_bytes(1) if sample else 0)
+                self.comm = ops.Comm(tp_rank, tp, max(batch * H * 2, 4096, batch * rec_max)).connect_group(tp_group)
             self._bufs["part"] = torch.empty(batch, H, **bf)             # row-split partial sums (all-reduced)
             if not logprobs:  # the argmax path's per-rank (max, argmax) pairs
                 self.loc_ids = torch.empty(batch, dtype=torch.int64, device=device)
@@ -323,6 +343,10 @@ class DecodeStack:
         if self.logprobs and self.tp > 1:
             rec = self._all_rec.numel() // (self.tp * self.Bmax)
             self.all_rec = self._all_rec[:self.tp * b * rec].view(self.tp, b * rec)
+        if self.sample and self.tp > 1:
+            f = self._stp
+            self.stp = {"state": f["state"][:b], "rec": [r[:b] for r in f["rec"]],
+                        "all": [a.view(-1)[:a.numel() // self.Bmax * b].view(self.tp, -1) for a in f["all"]]}
         self.graph = None
 
     def set_sampling(self, temperature=None, top_k=None, top_p=None, seeds=None, offsets=None):
@@ -481,6 +505,16 @@ class DecodeStack:
             if self.logprobs:
                 ops.logprobs(self.logits, self.logprobs, tok_ids=self.pred.view(-1), out=(None, self.tok_lp, self.top_ids, self.top_lp))
                 n += 1
+        elif self.sample and self.tp > 1:  # every rank draws the whole row's id from its shard by exchanging records
+            ops.sample_tp(self.logits, self.tp_rank * self.vocab_l, cfg.vocab, self.temperature, self.top_k, self.top_p,
+                          self.seeds, self.offsets, self._gather, self.tp, out=self.next_ids, bufs=self.stp)
+            n += ops._lib.SAMPLE_SHARD_PHASES + 1 + ops._lib.SAMPLE_SHARD_PHASES * (self.collective != "nccl")
+            if self.logprobs:  # the log-probabilities at the drawn ids: the greedy TP step's records, all-gather and merge
+                ops.logprobs_shard(self.logits, self.logprobs, self.tp_rank * self.vocab_l, tok_ids=self.next_ids,
+                                   out=self.loc_rec); n += 1
+                self._gather_records()
+                n += self.collective != "nccl"
+                ops.logprobs_merge(self.all_rec, self.logprobs, out=(None, self.tok_lp, self.top_ids, self.top_lp)); n += 1
         elif self.sample:  # the drawn ids; with logprobs, the log-probabilities at them (one launch more)
             ops.sample(self.logits, self.temperature, self.top_k, self.top_p, self.seeds, self.offsets, out=self.next_ids); n += 1
             if self.logprobs:
@@ -528,11 +562,15 @@ class DecodeStack:
 
     def _gather_records(self):
         """all-gather the per-rank logprob records (opaque bytes) of the vocab-split lm_head"""
+        self._gather(self.loc_rec, self.all_rec)
+
+    def _gather(self, rec, all_rec):
+        """all-gather this rank's records (opaque bytes, [rows, bytes]) into all_rec [tp, rows * bytes], in rank order"""
         if self.collective == "nccl":
             import torch.distributed as dist
-            dist.all_gather_into_tensor(self.all_rec, self.loc_rec.view(-1), group=self.tp_group)
+            dist.all_gather_into_tensor(all_rec.view(-1), rec.view(-1), group=self.tp_group)
         else:
-            self.comm.allgather(self.loc_rec, self.all_rec)
+            self.comm.allgather(rec, all_rec)
 
     def step(self):
         """q_len 1: returns next_ids [B].  q_len > 1: one verify step, returns (pred [B, T], accepted [B]); the step's

@@ -664,6 +664,8 @@ def _sampling_args(rows, B, out, temperature, top_k, top_p, seeds, offsets, what
     for t, dt, name, n in ((out, torch.int64, "out", rows), (temperature, torch.float32, "temperature", B),
                            (top_k, torch.int32, "top_k", B), (top_p, torch.float32, "top_p", B), (seeds, torch.int64, "seeds", B),
                            (offsets, torch.int64, "offsets", B)):
+        if t is None:  # no output (sample_shard)
+            continue
         assert t.dtype == dt and t.is_contiguous() and tuple(t.shape) == (n,), f"{what}: {name} must be [{n}] {dt} contiguous"
 
 
@@ -695,6 +697,85 @@ def sample_tokens(logits, q_len, temperature, top_k, top_p, seeds, offsets, pare
     check(lib.b2_sample_tokens(_ptr(out), _ptr(logits), B, q_len, _ptr(parents), n, logits.stride(0), _ptr(temperature),
                                _ptr(top_k), _ptr(top_p), _ptr(seeds), _ptr(offsets), _ft(logits), _stream()), "b2_sample_tokens")
     return out
+
+
+def sample_shard_record_bytes(phase):
+    return lib.b2_sample_shard_record_bytes(int(phase))
+
+
+def sample_shard_state_bytes():
+    return lib.b2_sample_shard_state_bytes()
+
+
+def sample_shard(phase, logits, id_offset, n_total, temperature, top_k, top_p, seeds, offsets, state, all_records=None,
+                 out=None, nranks=None):
+    """One phase of sampling under tensor parallelism (b2_sample_shard) on this rank's shard: logits [rows, n] FT hold
+    columns id_offset .. id_offset + n - 1 of rows of n_total columns; the sampling parameters are sample()'s, the same on
+    every rank; state uint8 [rows, sample_shard_state_bytes()] is this rank's own.  all_records: the previous phase's
+    records of every rank as all-gathered, uint8 [nranks, rows * bytes] (None for phase 0).  Returns this phase's records,
+    uint8 [rows, sample_shard_record_bytes(phase)] (out, if given)."""
+    rows, n = logits.shape
+    assert logits.stride(-1) == 1
+    assert 0 <= phase < _lib.SAMPLE_SHARD_PHASES and (all_records is None) == (phase == 0)
+    _sampling_args(rows, rows, None, temperature, top_k, top_p, seeds, offsets, "sample_shard")
+    assert state.dtype == torch.uint8 and state.is_contiguous() and state.numel() == rows * sample_shard_state_bytes()
+    if all_records is not None:
+        nranks = all_records.shape[0]
+        rb = sample_shard_record_bytes(phase - 1)
+        assert all_records.dtype == torch.uint8 and all_records.is_contiguous() and all_records.numel() == nranks * rows * rb, \
+            f"sample_shard: all_records must be [nranks, {rows} * {rb}] uint8 contiguous (phase {phase - 1}'s records)"
+    rb = sample_shard_record_bytes(phase)
+    out = torch.empty(rows, rb, dtype=torch.uint8, device=logits.device) if out is None else out
+    assert out.dtype == torch.uint8 and out.is_contiguous() and out.numel() == rows * rb
+    check(lib.b2_sample_shard(int(phase), _ptr(out), _ptr(state), _ptr(all_records), int(nranks or 1), _ptr(logits), rows, n,
+                              logits.stride(0), int(id_offset), int(n_total), _ptr(temperature), _ptr(top_k), _ptr(top_p),
+                              _ptr(seeds), _ptr(offsets), _ft(logits), _stream()), "b2_sample_shard")
+    return out
+
+
+def sample_shard_merge(all_records, state, offsets, out=None):
+    """The end of sampling under tensor parallelism (b2_sample_shard_merge): all_records uint8 [nranks, rows * 8], the last
+    phase's records as all-gathered; state and offsets this rank's.  Advances offsets by 1 in place and returns the ids,
+    int64 [rows] (out, if given): b2_sample's ids of the whole rows, the same on every rank."""
+    nranks, rows = all_records.shape[0], offsets.numel()
+    assert all_records.dtype == torch.uint8 and all_records.is_contiguous()
+    assert all_records.numel() == nranks * rows * sample_shard_record_bytes(_lib.SAMPLE_SHARD_PHASES - 1)
+    assert state.dtype == torch.uint8 and state.numel() == rows * sample_shard_state_bytes()
+    assert offsets.dtype == torch.int64 and offsets.is_contiguous()
+    out = torch.empty(rows, dtype=torch.int64, device=offsets.device) if out is None else out
+    assert out.dtype == torch.int64 and out.is_contiguous() and out.numel() == rows
+    check(lib.b2_sample_shard_merge(_ptr(out), _ptr(all_records), _ptr(state), nranks, rows, _ptr(offsets), _stream()),
+          "b2_sample_shard_merge")
+    return out
+
+
+def sample_tp_buffers(rows, nranks, device="cuda"):
+    """The buffers of sample_tp() for `rows` rows and `nranks` ranks: this rank's state, each phase's own records and
+    their all-gathered form ([nranks, rows * bytes], the layout an all-gather writes)."""
+    P = _lib.SAMPLE_SHARD_PHASES
+    u8 = dict(dtype=torch.uint8, device=device)
+    return {"state": torch.empty(rows, sample_shard_state_bytes(), **u8),
+            "rec": [torch.empty(rows, sample_shard_record_bytes(p), **u8) for p in range(P)],
+            "all": [torch.empty(nranks, rows * sample_shard_record_bytes(p), **u8) for p in range(P)]}
+
+
+def sample_tp(logits_shard, id_offset, n_total, temperature, top_k, top_p, seeds, offsets, exchange, nranks, out=None,
+              bufs=None):
+    """sample() of the whole rows under tensor parallelism, on one rank: every phase of b2_sample_shard, each followed by
+    exchange(record, all_records) (the all-gather of this rank's records into all_records [nranks, rows * bytes] in rank
+    order: Comm.allgather, torch.distributed.all_gather_into_tensor, ...), then the merge.  Every rank calls it with its
+    own shard and the same parameters; every rank returns the same ids (out, if given), b2_sample's ids of the
+    concatenated rows, and advances its offsets by 1.  The launch sequence is static, so a CUDA graph can capture it.
+    bufs: sample_tp_buffers(rows, nranks), kept by a caller that captures graphs."""
+    rows = logits_shard.shape[0]
+    bufs = sample_tp_buffers(rows, nranks, logits_shard.device) if bufs is None else bufs
+    prev = None
+    for p in range(_lib.SAMPLE_SHARD_PHASES):
+        sample_shard(p, logits_shard, id_offset, n_total, temperature, top_k, top_p, seeds, offsets, bufs["state"], prev,
+                     out=bufs["rec"][p], nranks=nranks)
+        exchange(bufs["rec"][p], bufs["all"][p])
+        prev = bufs["all"][p]
+    return sample_shard_merge(prev, bufs["state"], offsets, out=out)
 
 
 def lens_add(lens, delta):

@@ -462,6 +462,44 @@ int b2_sample(int64_t* ids_out, const void* logits, int rows, int n, int64_t ld,
 int b2_sample_tokens(int64_t* ids_out, const void* logits, int batch, int q_len, const int32_t* parents /* NULL: chain */,
                      int n, int64_t ld, const float* temperature, const int32_t* top_k, const float* top_p,
                      const uint64_t* seeds, const uint64_t* offsets, int ft, void* stream);
+/* b2_sample under tensor parallelism: the rows' columns are split over the ranks of a vocab-split lm_head, and every rank
+ * draws b2_sample's id of the whole row by exchanging small per-row records instead of the logits.  Rank q of P
+ * (1 <= P <= 8) holds columns [id_offset_q, id_offset_q + n_q) of a row of n_total columns (n_q >= 1): the ranges are
+ * contiguous, ascend with the rank and together cover [0, n_total); they may be unequal.  Every rank passes the same
+ * temperature, top_k, top_p, seeds and offsets ([rows] each, its own device copies); top_k is read against n_total
+ * (k <= 0 or k > n_total: n_total).
+ * Result: ids_out[r] on every rank equals b2_sample's id of the concatenated row at the same offset, bit for bit (all of
+ * its steps 1-6, greedy rows included, whose id is b2_argmax's of the whole row), and every rank's offsets[r] advances by
+ * exactly 1.
+ * Protocol, per row: phases p = 0 .. B2_SAMPLE_SHARD_PHASES - 1 in order, each followed by an all-gather of its records
+ * (record_out [rows][b2_sample_shard_record_bytes(p)] on each rank -> all_records [nranks][rows][bytes] in rank order,
+ * opaque bytes: b2_allgather or an NCCL all-gather moves them unchanged), then b2_sample_shard_merge.  Phase p >= 1 reads
+ * the all-gathered records of phase p - 1 (all_records; NULL for phase 0).  state [rows][b2_sample_shard_state_bytes()]
+ * is this rank's own memory, written and read by the phases in turn and never exchanged: every rank derives the same
+ * values from the same records.
+ *   0  reads the shard: its argmax under b2_argmax's order (value, global id)                        record 8 B
+ *   1  the row's m, c, greedy predicate and argmax; the shard's level-1 histogram (high byte of the key: counts and
+ *      weight sums at the row's m and c)                                                            record 3072 B
+ *   2  the row's level 1; with k < n_total the k-th element's high byte; the shard's level-2 counts in it   1024 B
+ *   3  S_k; the top-p target Pt and its high byte; the shard's level-2 counts in it                        1024 B
+ *   4  S_p; the draw's U (offsets[r] read here) and its high byte; the shard's level-2 counts in it        1024 B
+ *   5  the drawn key K and its rank j among K's elements; the rank holding the j-th writes its id, the others -1   8 B
+ *   merge: ids_out[r] = the holder's id (the argmax for a greedy row); offsets[r] += 1.
+ * A greedy row, or one without a top-k or top-p limit, passes through the phases with an empty record, so the launch
+ * sequence is static (a CUDA graph captures it).  The records depend only on the row, the parameters and the split.
+ * Errors, all before any launch: a NULL pointer (all_records may be NULL for phase 0 only), nranks outside [1, 8],
+ * rows < 0, n < 1, ld < n, id_offset < 0, id_offset + n > n_total, ft other than bf16 / fp16, or a phase out of range:
+ * B2_ERR_PARAM; n_total > B2_SAMPLE_MAX_N: B2_ERR_LIMIT.  rows = 0 launches nothing.  One 1024-thread CTA per row and
+ * phase; the merge reads state and offsets of its own rank. */
+#define B2_SAMPLE_SHARD_PHASES 6
+size_t b2_sample_shard_record_bytes(int phase); /* bytes per row; 0 for a phase out of range */
+size_t b2_sample_shard_state_bytes(void);       /* bytes per row of the rank-local state */
+int b2_sample_shard(int phase, void* record_out, void* state, const void* all_records /* NULL for phase 0 */, int nranks,
+                    const void* logits, int rows, int n, int64_t ld, int64_t id_offset, int64_t n_total,
+                    const float* temperature, const int32_t* top_k, const float* top_p, const uint64_t* seeds,
+                    const uint64_t* offsets, int ft, void* stream);
+int b2_sample_shard_merge(int64_t* ids_out, const void* all_records, const void* state, int nranks, int rows,
+                          uint64_t* offsets, void* stream);
 /* Per-sequence token history on the device (the in_ids / cur_len / input_len of the reference's logits processor).  Every
  * array has `rows` slots (row r of a step uses slot r); all pointers are device memory, zero-initialised before first use.
  *   tokens     int32 [rows][max_len]  the sequence, prompt first; an id outside [0, vocab) is stored as -1
