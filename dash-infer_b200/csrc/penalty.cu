@@ -1,5 +1,6 @@
 // b200spark — the logits processor of the sampling step (b2_penalize: repetition, presence and frequency penalties,
-// no-repeat n-grams, min-length) over a per-sequence token history kept on the device (b2_history_load / _append).
+// no-repeat n-grams, min-length) over a per-sequence token history kept on the device (b2_history_load / _append /
+// _append_tokens).
 // Reference counterpart: LogitsProcessor, beam_search.cu:329-539, called from GenerateOp::RunSample.  The contract is in
 // include/b200spark.h.
 //
@@ -75,14 +76,13 @@ __global__ void __launch_bounds__(kLoadThreads) history_load_kernel(b2_token_his
   }
 }
 
-__global__ void history_append_kernel(b2_token_history h, const int64_t* ids, int rows) {
-  pdl_wait();
-  pdl_launch_dependents();
-  const int r = blockIdx.x * blockDim.x + threadIdx.x;
-  if (r >= rows) return;
+// Append id *id to slot r: the token, its table entry, the distinct list (an id whose entry leaves 0 goes to its end) and
+// len.  A full slot is left as it is.  Every append of the history goes through here.  The id is passed by address and
+// read after the full-slot check, as history_append_kernel always read it; that keeps its machine code what it was.
+__device__ __forceinline__ void history_push(const b2_token_history& h, int r, const int64_t* id) {
   const int L = h.len[r];
   if (L >= h.max_len) return;
-  const int64_t t = ids[r];
+  const int64_t t = *id;
   const bool ok = t >= 0 && t < h.vocab;
   h.tokens[(size_t)r * h.max_len + L] = ok ? (int32_t)t : -1;
   if (ok) {
@@ -96,6 +96,33 @@ __global__ void history_append_kernel(b2_token_history h, const int64_t* ids, in
     *e = old + 1;
   }
   h.len[r] = L + 1;
+}
+
+__global__ void history_append_kernel(b2_token_history h, const int64_t* ids, int rows) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= rows) return;
+  history_push(h, r, ids + r);
+}
+
+// The emitted tokens of a verify step, in order, one thread per sequence (appends to one slot are sequential).
+__global__ void history_append_tokens_kernel(b2_token_history h, const int64_t* pred, const int32_t* accepted,
+                                             const int32_t* path, int batch, int q_len) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= batch) return;
+  const int64_t* row = pred + (size_t)r * q_len;
+  const int n = min(max(accepted[r], 0), q_len);
+  for (int i = 0; i < n; ++i) {
+    int u = i;
+    if (path != nullptr) {
+      u = path[(size_t)r * q_len + i];
+      u = (unsigned)u < (unsigned)q_len ? u : 0;
+    }
+    history_push(h, r, row + u);
+  }
 }
 
 template <bool H>
@@ -182,6 +209,16 @@ int b2_history_append(const b2_token_history* hist, const int64_t* ids, int rows
   if (rows == 0) return B2_OK;
   B2_CUDA_TRY(launch(history_append_kernel, dim3((rows + 127) / 128), dim3(128), 0, (cudaStream_t)stream, true, *hist,
                      ids, rows));
+  return B2_OK;
+}
+
+int b2_history_append_tokens(const b2_token_history* hist, const int64_t* pred, const int32_t* accepted, const int32_t* path,
+                             int batch, int q_len, void* stream) {
+  if (!history_ok(hist) || !pred || !accepted || batch < 0) return B2_ERR_PARAM;
+  if (q_len < 1 || q_len > kMaxQLen) return B2_ERR_LIMIT;
+  if (batch == 0) return B2_OK;
+  B2_CUDA_TRY(launch(history_append_tokens_kernel, dim3((batch + 127) / 128), dim3(128), 0, (cudaStream_t)stream, true,
+                     *hist, pred, accepted, path, batch, q_len));
   return B2_OK;
 }
 

@@ -139,7 +139,7 @@ class DecodeStack:
     def __init__(self, cfg, batch, max_len, wbits=4, group=-1, kv="none", span=128, seed=1234, device="cuda",
                  keep_ref=False, layers=None, tp_rank=0, tp_size=1, tp_group=None, fuse_swiglu=True,
                  collective=None, comm=None, dtype=torch.bfloat16, q_len=1, tree=False, logprobs=0, sample=False,
-                 penalties=False, sampled_verify=False):
+                 penalties=False, sampled_verify=False, ngram=None):
         """tp_size > 1: the reference's tensor-parallel layout (QKV/gate/up column split, o/down row split + all-reduce,
         vocab-split lm_head + B-element all-gather); every rank builds the SAME full synthetic weights from `seed` and
         keeps its shard, exactly like the reference splits an already-quantized checkpoint.  A rank reaches its peers through
@@ -182,7 +182,14 @@ class DecodeStack:
         b2_spec_accept_sampled, which also advances offsets[b] by accepted[b]; the launch count is the greedy verify step's.
         step() returns what a verify step returns, the emitted tokens are pred[b, :accepted[b]] (pred[b, path[b, :accepted[b]]]
         in a tree), and they are exactly the tokens single-token sampling would draw from the same rows and seeds.  With
-        logprobs = N, b2_logprobs runs at the drawn ids (one launch more): tok_lp at row b*T + u is the logprob of pred[b, u]."""
+        logprobs = N, b2_logprobs runs at the drawn ids (one launch more): tok_lp at row b*T + u is the logprob of pred[b, u].
+        ngram=(n_min, n_max, width) (q_len = T > 1, chain or tree, greedy or sampled_verify): the step drafts its own tokens
+        on the device.  Before the embedding, b2_ngram_draft fills self.tokens[:, 1:] (and self.parents in a tree) from a
+        per-sequence token history by n-gram (prompt-lookup) matching; width > 1 candidates make a draft tree and need
+        tree=True.  After accept (and compaction) b2_history_append_tokens appends the step's emitted tokens to the history.
+        Two launches more; the verify body is unchanged.  set_history(b, ids, prompt_len) loads sequence b's history and
+        sets self.tokens[b, 0] = ids[-1], the last emitted token; self.n_draft [B] int32 holds the drafts each step filled.
+        capture() leaves the history as it found it."""
         global _DT
         assert dtype in (torch.bfloat16, torch.float16) and (dtype == torch.bfloat16 or (tp_size == 1 and cfg.head == 128)), \
             "fp16: single GPU, head size 128 (the communicator and the head-64 kernels are bf16)"
@@ -198,6 +205,13 @@ class DecodeStack:
             "without penalties=True (the history is not kept per draft position)"
         assert not penalties or q_len == 1, \
             "penalties=True: single-token steps (q_len == 1); the history is not kept per draft position"
+        if ngram is not None:
+            assert q_len > 1, "ngram: drafting needs multi-token verify steps (q_len > 1)"
+            n_min, n_max, width = ngram
+            assert 1 <= n_min <= n_max <= 16, "ngram=(n_min, n_max, width): 1 <= n_min <= n_max <= 16"
+            assert 1 <= width <= q_len - 1 and (width == 1 or tree), \
+                "ngram=(n_min, n_max, width): 1 <= width <= q_len - 1, and width > 1 drafts a tree (tree=True)"
+            ngram = (int(n_min), int(n_max), int(width))
         import os
 
         import torch.distributed as dist
@@ -208,7 +222,7 @@ class DecodeStack:
         assert tp_size == 1 or (dist.is_available() and dist.is_initialized()) or (comm is not None and collective != "nccl"), \
             "tp_size > 1: initialise a torch.distributed process group (or pass a connected comm with collective 'b2' / " \
             "'fused') first; a stack without peers runs with tp_size == 1"
-        self.logprobs, self.sample, self.pen, self.sv = logprobs, sample, penalties, sampled_verify
+        self.logprobs, self.sample, self.pen, self.sv, self.ngram = logprobs, sample, penalties, sampled_verify, ngram
         self.dtype = _DT = dtype
         self.q_len, self.tree = q_len, tree
         rows = batch * q_len  # activation rows of a step
@@ -279,9 +293,12 @@ class DecodeStack:
             self._top_p = torch.ones(batch, dtype=torch.float32, device=device)
             self._seeds = torch.zeros(batch, dtype=torch.int64, device=device)
             self._offsets = torch.zeros(batch, dtype=torch.int64, device=device)
-        if penalties:
+        if penalties or ngram:
             self._history = ops.TokenHistory(batch, max_len, cfg.vocab, device)
+        if penalties:
             self._penalties = ops.Penalties(batch, device)
+        if ngram:
+            self._n_draft = torch.zeros(batch, dtype=torch.int32, device=device)
         if q_len > 1:
             self._tokens = torch.zeros(batch, q_len, dtype=torch.int64, device=device)
             self._pred = torch.zeros(batch, q_len, dtype=torch.int64, device=device)
@@ -340,6 +357,8 @@ class DecodeStack:
                 setattr(self, k, getattr(self, "_" + k)[:b])
         if self.pen:
             self.history, self.penalties = self._history.view(b), self._penalties.view(b)
+        if self.ngram:
+            self.history, self.n_draft = self._history.view(b), self._n_draft[:b]
         if self.logprobs and self.tp > 1:
             rec = self._all_rec.numel() // (self.tp * self.Bmax)
             self.all_rec = self._all_rec[:self.tp * b * rec].view(self.tp, b * rec)
@@ -365,9 +384,13 @@ class DecodeStack:
         self.penalties.set(repetition, presence, frequency, no_repeat_ngram, min_length, eos_id, suppress_repetition_in_generation)
 
     def set_history(self, b, ids, prompt_len=None):
-        """Load sequence b's tokens into its history (prompt first; prompt_len of them, all by default)."""
-        assert self.pen, "set_history: the stack was built with penalties=False"
+        """Load sequence b's tokens into its history (prompt first; prompt_len of them, all by default).  With ngram the last
+        of them is also the last emitted token of the next step: tokens[b, 0] = ids[-1]."""
+        assert self.pen or self.ngram, "set_history: the stack was built with penalties=False and without ngram"
         self._history.load(b, ids, prompt_len)
+        ids = torch.as_tensor(ids).reshape(-1)
+        if self.ngram and ids.numel():
+            self._tokens[b, 0] = int(ids[-1])
 
     # ------------------------------------------------------------------ cache fill
     def set_context(self, ctx, seed=4321):
@@ -459,6 +482,9 @@ class DecodeStack:
         # the step form of append + attention: single token, chain of T tokens, or draft tree
         form = {} if T == 1 else {"q_len": T, "parents": self.parents if self.tree else None}
         n = 0
+        if self.ngram:  # this step's drafts, from the history the previous step extended
+            ops.ngram_draft(self.history, self.tokens, self.parents if self.tree else None, *self.ngram, n_draft=self.n_draft)
+            n += 1
         ops.embedding(self.embed, self.ids if T == 1 else self.tokens.view(-1), out=self.x); n += 1
         for li, L in enumerate(self.layers):
             if norm == "self":
@@ -553,6 +579,8 @@ class DecodeStack:
             ops.lens_add(self.lens_new, 1); n += 1
         if self.pen:  # the emitted token joins the history
             self.history.append(self.next_ids); n += 1
+        if self.ngram:  # the step's emitted tokens join the history
+            self.history.append_tokens(self.pred, self.accepted, self.path if self.tree else None); n += 1
         # rows per launch above 16 rows: 64 on the wgmma path (per-channel int4/int8, bf16 lm_head), 16 for sub-channel
         # weights (mma.sync path); below, one launch takes all rows
         hchunks = (R + 63) // 64 if R > 16 else 1
@@ -588,7 +616,7 @@ class DecodeStack:
         lo, ln = self.lens_old.clone(), self.lens_new.clone()
         tk = self.tokens.clone() if self.q_len > 1 else None  # the accept kernel rewrites column 0
         off = self.offsets.clone() if self.sample or self.sv else None  # the warm-up step advances the draw counters
-        hist = self.history.snapshot() if self.pen else None  # ... and appends a token to the history
+        hist = self.history.snapshot() if self.pen or self.ngram else None  # ... and appends tokens to the history
         self._step_ops()
         torch.cuda.synchronize()
         if hist is not None:

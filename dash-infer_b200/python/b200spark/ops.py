@@ -829,12 +829,38 @@ class TokenHistory:
         check(lib.b2_history_append(C.byref(self.c), _ptr(ids), ids.numel(), _stream()), "b2_history_append")
         return self
 
+    def append_tokens(self, pred, accepted, path=None):
+        """Append the emitted tokens of a verify step to slot b, for the first pred.shape[0] slots (b2_history_append_tokens):
+        pred[b, path[b, i]] (chain, path None: pred[b, i]) for i < accepted[b].  pred int64 [B, T], accepted int32 [B], path
+        int32 [B, T], on the device."""
+        B, T = pred.shape
+        assert pred.dtype == torch.int64 and pred.is_contiguous() and B <= self.rows
+        assert accepted.dtype == torch.int32 and accepted.is_contiguous() and tuple(accepted.shape) == (B,)
+        assert path is None or (path.dtype == torch.int32 and path.is_contiguous() and path.shape == pred.shape)
+        check(lib.b2_history_append_tokens(C.byref(self.c), _ptr(pred), _ptr(accepted), _ptr(path), B, T, _stream()),
+              "b2_history_append_tokens")
+        return self
+
     def snapshot(self):
         return [getattr(self, k).clone() for k in self._FIELDS]
 
     def restore(self, snap):
         for k, s in zip(self._FIELDS, snap):
             getattr(self, k).copy_(s)
+
+
+def ngram_draft(history, tokens, parents, n_min, n_max, width, n_draft=None):
+    """N-gram (prompt-lookup) drafts of a verify step from the token history (b2_ngram_draft), written in place: tokens int64
+    [B, T] (column 0, the last emitted token, is read; columns 1.. get the drafts), parents int32 [B, T] for a draft tree
+    (None: a chain, width 1), n_draft int32 [B] (optional) = the drafts filled per sequence.  Slot b of history is
+    sequence b.  The contract (matching, periodic continuation, trie numbering, padding): include/b200spark.h."""
+    B, T = tokens.shape
+    assert tokens.dtype == torch.int64 and tokens.is_contiguous() and B <= history.rows
+    assert parents is None or (parents.dtype == torch.int32 and parents.is_contiguous() and parents.shape == tokens.shape)
+    assert n_draft is None or (n_draft.dtype == torch.int32 and n_draft.is_contiguous() and tuple(n_draft.shape) == (B,))
+    check(lib.b2_ngram_draft(_ptr(tokens), _ptr(parents), _ptr(n_draft), C.byref(history.c), B, T, int(n_min), int(n_max),
+                             int(width), _stream()), "b2_ngram_draft")
+    return tokens
 
 
 class Penalties:

@@ -528,6 +528,42 @@ int b2_history_load(const b2_token_history* hist, int slot, const int32_t* ids, 
 /* Append ids[r] (int64, device) to slot r for r < rows, on the device (CUDA-graph replayable: each replay appends once).  A
  * slot that holds max_len tokens is left as it is.  An id outside [0, vocab) is stored as -1 and counted nowhere. */
 int b2_history_append(const b2_token_history* hist, const int64_t* ids, int rows, void* stream);
+/* Append the emitted tokens of a verify step (b2_spec_accept / _tree / _sampled) to slot b for b < batch, in order:
+ * pred[b][path[b][i]] (chain, path NULL: pred[b][i]) for i < accepted[b].  pred int64 [batch][q_len], accepted int32
+ * [batch], path int32 [batch][q_len], all device memory.  Every array of the history ends as accepted[b] successive
+ * b2_history_append calls leave it, the order of the distinct list included; a slot stops at max_len like there.
+ * accepted[b] is clamped to [0, q_len] and a path entry outside [0, q_len) is read as 0, so no input reads out of bounds.
+ * One thread per sequence, CUDA-graph replayable (each replay appends once).  A NULL required pointer, batch < 0 or a
+ * history b2_history_append refuses: B2_ERR_PARAM; q_len outside [1, 16]: B2_ERR_LIMIT; before any launch.  batch = 0
+ * launches nothing. */
+int b2_history_append_tokens(const b2_token_history* hist, const int64_t* pred, const int32_t* accepted,
+                             const int32_t* path /* NULL: chain */, int batch, int q_len, void* stream);
+/* N-gram (prompt-lookup) drafting of a verify step from the token history, on the device (CUDA-graph replayable): the
+ * drafts continue the most recent earlier occurrences of the sequence's last tokens.  For sequence b, S = hist.tokens[b][0
+ * .. L), L = hist.len[b]; S[L-1] is the last emitted token, which the caller keeps equal to tokens[b][0] (DecodeStack does
+ * so by construction).  tokens int64 [batch][q_len]: column 0 is read, never written.
+ *   m(e), for an end position e in [0, L-2]: the number of leading i < n_max with e - i >= 0 and S[e-i] == S[L-1-i]
+ *        (-1 entries compare like any id, as in b2_penalize's n-gram step).  n* = max_e m(e); n* < n_min: no match.
+ *   Candidates: the `width` largest e with m(e) >= n*, most recent first.  Candidate e has period p = L-1-e and
+ *        continuation c_k = S[e+1 + (k mod p)], k < q_len-1: the tokens that followed the match and, past the end of the
+ *        history, the same period again, so a loop keeps being predicted.  A match therefore always fills all q_len-1
+ *        drafts (prompt lookup that truncates at the end of the history drafts fewer): a verify step runs q_len rows
+ *        whether they hold drafts or not.
+ *   Chain (parents NULL, width == 1): tokens[b][1+k] = c_k of the candidate.
+ *   Tree (parents int32 [batch][q_len], tree format: b2_span_cache_append_tree): the trie of the candidates'
+ *        continuations, a node per distinct prefix, node 0 the root (the empty prefix).  Nodes are numbered breadth first;
+ *        within a level by parent index, then by the rank of the first candidate that has the prefix.  The first q_len
+ *        nodes are kept: tokens[b][t] = the last token of node t's prefix, parents[b][t] = its parent (always < t),
+ *        parents[b][0] = 0.  Identical continuations merge, so an exact loop drafts a chain and distinct continuations
+ *        branch; a candidate whose continuation equals a more recent one's still takes one of the `width` slots.
+ *   Padding: drafts or nodes that no candidate fills (all of them without a match) get token tokens[b][0] and parent 0; a
+ *        draft that would be -1 is written as tokens[b][0] too.  n_draft[b] (int32 [batch], may be NULL) = the drafts a
+ *        candidate fills: q_len-1 for a matched chain, the kept nodes minus the root for a tree, 0 without a match.
+ * Integer arithmetic only: the results are exact.  One CTA per sequence.  A NULL required pointer, batch < 0, n_min < 1,
+ * n_min > n_max, width < 1, width > q_len-1 or a chain with width != 1: B2_ERR_PARAM; q_len outside [2, 16] or n_max >
+ * 16: B2_ERR_LIMIT; before any launch.  batch = 0 launches nothing. */
+int b2_ngram_draft(int64_t* tokens, int32_t* parents /* NULL: chain */, int32_t* n_draft /* or NULL */,
+                   const b2_token_history* hist, int batch, int q_len, int n_min, int n_max, int width, void* stream);
 /* Per-row parameters of b2_penalize, device arrays [rows], read at every call (a captured step uses the values last
  * written).  The neutral values repetition 1, presence 0, frequency 0, no_repeat_ngram 0, min_length 0 change nothing. */
 typedef struct b2_penalty_params {

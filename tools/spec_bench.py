@@ -32,6 +32,18 @@ Usage (the DESIGN.md §5 tree table): python tools/spec_bench.py --tree --steps 
     branch of random drafts; "random", random drafts (and random parents).  "own" is not accepted whole: verify rows pass
     the GEMMs at M = B*T, so their logits differ from the single-token step's by rounding, and a draw can change.
 Usage (the DESIGN.md §5 sampled-verification table): python tools/spec_bench.py --sample --steps 30 --warmup 5
+
+--ngram: the on-device n-gram drafter (DecodeStack(ngram=(1, 4, width))):
+  * µs per launch of b2_ngram_draft (a graph of 20) at T = 8, B = 1 / 8 / 64, history L = 2K / 32K / 128K, width 1 (chain)
+    and 4 (tree), over random histories (the full scan) and periodic ones (the candidate walk stops early); and of
+    b2_history_append_tokens (8 tokens per sequence);
+  * ms per CUDA-graph-replayed verify step with the drafter against the same step with host-written drafts (the drafter's
+    own, so both verify the same tokens), alternated over --rounds rounds: medians and the spread; T = 4 / 8 / 16, B = 1
+    and 8, chain and tree;
+  * generation at T = 8: --steps graph replays back to back with nothing restored, from prompts that repeat a random
+    61-token segment and from random prompts: accepted tokens per step and tokens/s, against the q_len = 1 step on the
+    same weights.  The weights are synthetic, so the acceptance says nothing about a real model's.
+Usage (the DESIGN.md §5 drafter table): python tools/spec_bench.py --ngram --steps 30 --warmup 5
 """
 import argparse
 import json
@@ -267,6 +279,144 @@ def sample_main(args, name, power):
                       "sample": {"temperature": t, "top_k": k, "top_p": p}, "rounds": args.rounds, "results": res}))
 
 
+def _fill_history(h, B, L, kind, gen):
+    """slots 0 .. B-1 of h := L tokens: "random" ids (the drafter scans everything) or a repeated random segment of 37
+    tokens ("periodic": the longest matches are the most recent, so the candidate walk stops in its first chunk)"""
+    if kind == "random":
+        tok = torch.randint(0, 152064, (B, L), generator=gen, device="cuda", dtype=torch.int32)
+    else:
+        seg = torch.randint(0, 152064, (B, 37), generator=gen, device="cuda", dtype=torch.int32)
+        tok = seg.repeat(1, L // 37 + 1)[:, :L]
+    h.tokens[:B, :L] = tok
+    h.len[:B] = L
+
+
+def ngram_main(args, name, power):
+    from b200spark import ops
+    cfg = model.QWEN2_7B
+    gen = torch.Generator(device="cuda").manual_seed(9)
+    res = {"kernel": [], "step": [], "generate": []}
+    # 1. the two launches alone: a graph of 20, µs per launch
+    T = 8
+    hist = ops.TokenHistory(64, 131072 + 4096, cfg.vocab)
+    for kind in ("random", "periodic"):
+        for L in (2048, 32768, 131072):
+            for B in (1, 8, 64):
+                _fill_history(hist, B, L, kind, gen)
+                h = hist.view(B)
+                tokens = torch.zeros(B, T, dtype=torch.int64, device="cuda")
+                tokens[:, 0] = h.tokens[:, L - 1]
+                parents = torch.zeros(B, T, dtype=torch.int32, device="cuda")
+                row = {"kind": kind, "L": L, "batch": B, "q_len": T}
+                for width in (1, 4):
+                    par = parents if width > 1 else None
+                    g = graph_of(lambda: [ops.ngram_draft(h, tokens, par, 1, 4, width) for _ in range(20)])
+                    row["draft_us_w%d" % width] = round(1e3 * time_ms(g.replay, 10, 3) / 20, 2)
+                if kind == "random" and L == 2048:  # T accepted tokens per sequence and launch
+                    acc = torch.full((B,), T, dtype=torch.int32, device="cuda")
+                    pred = torch.randint(0, cfg.vocab, (B, T), generator=gen, device="cuda")
+                    g = graph_of(lambda: [h.append_tokens(pred, acc) for _ in range(20)])
+                    row["append_us"] = round(1e3 * time_ms(g.replay, 10, 3) / 20, 2)
+                res["kernel"].append(row)
+                print(json.dumps(row), file=sys.stderr, flush=True)
+    del hist
+    # 2. the verify step with the drafter against the same step with host-written drafts (the drafter's own, so both
+    # verify the same tokens), alternated; 3. generation: steps replayed back to back, nothing restored
+    seg = torch.randint(0, cfg.vocab, (8, 61), generator=gen, device="cuda").cpu()
+    prompts = {"repeat": seg.repeat(1, args.ctx // 61 + 1)[:, :args.ctx],
+               "random": torch.randint(0, cfg.vocab, (8, args.ctx), generator=gen, device="cuda").cpu()}
+    n_gen = args.steps
+    one = None
+    for T in (4, 8, 16):
+        st = model.DecodeStack(cfg, 8, args.ctx + 16 * n_gen + 64, wbits=4, group=-1, kv="none", span=128, q_len=T, tree=True,
+                               ngram=(1, 4, 1))
+        st.set_context(args.ctx)
+        for B in (8, 1):
+            st.set_batch(B)
+            for b in range(B):
+                st.set_history(b, prompts["repeat"][b])
+            lo, ln, hl = st.lens_old.clone(), st.lens_new.clone(), st.history.len.clone()
+            tk0 = st.tokens.clone()
+            for form, ngram in (("chain", (1, 4, 1)), ("tree", (1, 4, min(4, T - 1)))):
+                st.tree, st.ngram = form == "tree", ngram
+                graphs = {"ngram": st.capture()}
+                st.step()  # the drafter's drafts become the host drafts
+                torch.cuda.synchronize()
+                drafted = (st.tokens.clone(), st.parents.clone())
+                st.lens_old.copy_(lo); st.lens_new.copy_(ln); st.history.len.copy_(hl); st.tokens.copy_(tk0)
+                st.ngram = None
+                st.tokens[:, 1:] = drafted[0][:, 1:]
+                st.parents.copy_(drafted[1])
+                graphs["host"] = st.capture()
+                st.ngram = ngram
+                tokens = {"ngram": tk0.clone(), "host": st.tokens.clone()}
+                ms = {"ngram": [], "host": []}
+                for _ in range(args.rounds):
+                    for mode in ms:
+                        st.graph = graphs[mode]
+
+                        def step():
+                            st.graph.replay()
+                            st.lens_old.copy_(lo); st.lens_new.copy_(ln); st.history.len.copy_(hl)
+                            st.tokens.copy_(tokens[mode])
+                            st.parents.copy_(drafted[1])
+
+                        ms[mode].append(time_ms(step, args.steps, args.warmup))
+                row = {"batch": B, "q_len": T, "form": form, "width": ngram[2], "accepted": int(st.accepted.sum())}
+                for mode, v in ms.items():
+                    row["ms_" + mode] = round(statistics.median(v), 4)
+                    row["ms_%s_spread" % mode] = [round(min(v), 4), round(max(v), 4)]
+                row["cost_pct"] = round(100 * (statistics.median(ms["ngram"]) / statistics.median(ms["host"]) - 1), 2)
+                res["step"].append(row)
+                print(json.dumps(row), file=sys.stderr, flush=True)
+                if T != 8:
+                    continue
+                st.graph = graphs["ngram"]
+                for pk, pr in prompts.items():  # generation from each prompt kind
+                    for b in range(B):
+                        st.set_history(b, pr[b])
+                    st.lens_old.copy_(lo); st.lens_new.copy_(ln)
+                    h0 = st.history.len.clone()
+                    torch.cuda.synchronize()
+                    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                    e0.record()
+                    for _ in range(n_gen):
+                        st.graph.replay()
+                    e1.record()
+                    torch.cuda.synchronize()
+                    ms_ = e0.elapsed_time(e1)
+                    toks = int((st.history.len - h0).sum())
+                    g_row = {"batch": B, "q_len": T, "form": form, "width": ngram[2], "prompt": pk, "steps": n_gen,
+                             "accepted_per_step": round(toks / (n_gen * B), 3), "tok_s": round(toks / ms_ * 1e3, 1),
+                             "ms_per_step": round(ms_ / n_gen, 4)}
+                    res["generate"].append(g_row)
+                    print(json.dumps(g_row), file=sys.stderr, flush=True)
+                st.lens_old.copy_(lo); st.lens_new.copy_(ln)
+                for b in range(B):
+                    st.set_history(b, prompts["repeat"][b])
+                st.tokens.copy_(tk0)
+        del st
+        torch.cuda.empty_cache()
+    # the single-token step on the same weights: tokens/s = B / step time
+    one = model.DecodeStack(cfg, 8, args.ctx + 64, wbits=4, group=-1, kv="none", span=128)
+    one.set_context(args.ctx)
+    q1 = {}
+    for B in (8, 1):
+        one.set_batch(B)
+        lo, ln = one.lens_old.clone(), one.lens_new.clone()
+        one.capture()
+
+        def step1():
+            one.step()
+            one.lens_old.copy_(lo); one.lens_new.copy_(ln)
+
+        ms = time_ms(step1, args.steps, args.warmup)
+        q1[str(B)] = {"ms_per_step": round(ms, 4), "tok_s": round(B / ms * 1e3, 1)}
+    print(json.dumps({"gpu": name, "power_limit": power, "model": "Qwen2-7B int4 per-channel, bf16 KV", "ctx": args.ctx,
+                      "ngram": {"n_min": 1, "n_max": 4}, "rounds": args.rounds, "q_len_1": q1, **res,
+                      "note": "synthetic weights: the acceptance says nothing about a real model's"}))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=30)
@@ -274,13 +424,16 @@ def main():
     ap.add_argument("--ctx", type=int, default=2048)
     ap.add_argument("--tree", action="store_true", help="draft trees against chains (T = 4, 8, 16)")
     ap.add_argument("--sample", action="store_true", help="sampled against greedy verification (T = 4, 8, 16)")
-    ap.add_argument("--rounds", type=int, default=5, help="--sample: alternations of the greedy / sampled measurements")
+    ap.add_argument("--ngram", action="store_true", help="the on-device n-gram drafter: kernel times, step cost, generation")
+    ap.add_argument("--rounds", type=int, default=5, help="--sample, --ngram: alternations of the two steps measured")
     args = ap.parse_args()
     name, power = gpu_info()
     if args.tree:
         return tree_main(args, name, power)
     if args.sample:
         return sample_main(args, name, power)
+    if args.ngram:
+        return ngram_main(args, name, power)
     res = []
     gen = torch.Generator(device="cuda").manual_seed(5)
     for T in (1, 2, 4, 8):
