@@ -1,6 +1,6 @@
 // b200spark — the logits processor of the sampling step (b2_penalize: repetition, presence and frequency penalties,
-// no-repeat n-grams, min-length) over a per-sequence token history kept on the device (b2_history_load / _append /
-// _append_tokens).
+// no-repeat n-grams, min-length) and of a verify step's rows (b2_penalize_tokens) over a per-sequence token history kept
+// on the device (b2_history_load / _append / _append_tokens).
 // Reference counterpart: LogitsProcessor, beam_search.cu:329-539, called from GenerateOp::RunSample.  The contract is in
 // include/b200spark.h.
 //
@@ -125,6 +125,21 @@ __global__ void history_append_tokens_kernel(b2_token_history h, const int64_t* 
   }
 }
 
+// Steps 1 and 2 of the contract for one id of generated count cnt, from its value v: penalize_kernel's loop body, which
+// keeps its own copy (calling this from it changes its register allocation).
+template <bool H>
+__device__ __forceinline__ typename PenFt<H>::T pen_value(typename PenFt<H>::T v, int cnt, typename PenFt<H>::T R, bool rep,
+                                                          bool sup, float freq, float pres) {
+  using F = PenFt<H>;
+  using T = typename F::T;
+  if (rep && (!sup || cnt > 0)) v = __hlt(v, F::from_f(0.f)) ? __hmul(v, R) : __hdiv(v, R);
+  float s = mul_ftz(__int2float_rn(cnt), freq);
+  if (cnt > 0) s = add_ftz(s, pres);
+  const T pen = F::from_f(s);
+  if (*reinterpret_cast<const unsigned short*>(&pen) != 0) v = __hsub(v, pen);
+  return v;
+}
+
 template <bool H>
 __global__ void __launch_bounds__(kPenThreads) penalize_kernel(__nv_bfloat16* logits, int n, int64_t ld, int64_t id_offset,
                                                                b2_token_history h, b2_penalty_params p) {
@@ -184,6 +199,95 @@ __global__ void __launch_bounds__(kPenThreads) penalize_kernel(__nv_bfloat16* lo
   }
 }
 
+// Row r = b * q_len + t of a verify step: penalize_kernel's row over the virtual history V = slot b followed by the
+// drafts on the path from the root to node t (the set bits of anc(t) above bit 0, ascending), appended as
+// history_push would append them.  The slot is only read; the path's d tokens sit in shared memory, and a path token
+// counts as one more generated occurrence of its id.  Distinct ids of V: the slot's list, then the path ids whose table
+// entry is 0 at their first path position; the two sets are disjoint, so each column is still written once before the
+// barrier.
+template <bool H>
+__global__ void __launch_bounds__(kPenThreads) penalize_tokens_kernel(__nv_bfloat16* logits, int n, int64_t ld, int64_t id_offset,
+                                                                      b2_token_history h, b2_penalty_params p,
+                                                                      const int64_t* tokens, const int32_t* parents, int q_len) {
+  using F = PenFt<H>;
+  using T = typename F::T;
+  __shared__ int32_t s_path[kMaxQLen - 1];
+  __shared__ int s_d;
+  pdl_wait();
+  pdl_launch_dependents();
+  const int r = blockIdx.x;
+  const int b = r / q_len, node = r - b * q_len;
+  T* x = reinterpret_cast<T*>(logits + (size_t)r * ld);
+  const int L = h.len[b];
+  const int nd = h.n_distinct[b];
+  const int32_t* tab = h.table + (size_t)b * h.vocab;
+  const int32_t* dl = h.distinct + (size_t)b * h.max_len;
+  const int32_t* tok = h.tokens + (size_t)b * h.max_len;
+  if (threadIdx.x == 0) {
+    int depth;
+    unsigned anc = parents != nullptr ? tree_walk(parents + (size_t)b * q_len, node, depth) : (2u << node) - 1u;
+    const int room = max(h.max_len - L, 0);
+    int d = 0;
+    for (anc &= ~1u; anc != 0 && d < room; anc &= anc - 1u) {
+      const int64_t v = tokens[(size_t)b * q_len + (__ffs(anc) - 1)];
+      s_path[d++] = v >= 0 && v < h.vocab ? (int32_t)v : -1;
+    }
+    s_d = d;
+  }
+  __syncthreads();
+  const int d = s_d, Lv = L + d;
+  const T R = F::from_f(p.repetition[b]);
+  const bool rep = !__heq(R, F::from_f(1.f));
+  const bool sup = p.suppress[b] != 0;
+  const float freq = p.frequency[b], pres = p.presence[b];
+  const int g = p.no_repeat_ngram[b];
+  auto col = [&](int32_t t) { return (uint64_t)((int64_t)t - id_offset) < (uint64_t)n ? (int)((int64_t)t - id_offset) : -1; };
+  auto on_path = [&](int32_t t, int end) {
+    int k = 0;
+    for (int j = 0; j < end; ++j) k += s_path[j] == t;
+    return k;
+  };
+  auto token = [&](int q) { return q < L ? tok[q] : s_path[q - L]; };
+
+  for (int i = threadIdx.x; i < nd; i += blockDim.x) {
+    const int32_t t = dl[i];
+    const int c = col(t);
+    if (c < 0) continue;
+    x[c] = pen_value<H>(x[c], (tab[t] & kCountMask) + on_path(t, d), R, rep, sup, freq, pres);
+  }
+  if (threadIdx.x < d) {
+    const int32_t t = s_path[threadIdx.x];
+    const int c = col(t);
+    if (c >= 0 && tab[t] == 0 && on_path(t, threadIdx.x) == 0) x[c] = pen_value<H>(x[c], on_path(t, d), R, rep, sup, freq, pres);
+  }
+  __syncthreads();  // every penalty write lands before a ban may overwrite it
+  const T ban = F::from_f(-1e9f);
+  if (g == 1) {  // every id of V
+    for (int i = threadIdx.x; i < nd; i += blockDim.x) {
+      const int c = col(dl[i]);
+      if (c >= 0) x[c] = ban;
+    }
+    if (threadIdx.x < d) {
+      const int c = col(s_path[threadIdx.x]);
+      if (c >= 0) x[c] = ban;
+    }
+  } else if (g > 1) {
+    const int tail = Lv - g + 1;  // the last g - 1 tokens of V start here
+    for (int j = threadIdx.x; j <= Lv - g; j += blockDim.x) {
+      int i = 0;
+      while (i < g - 1 && token(j + i) == token(tail + i)) ++i;
+      if (i == g - 1) {
+        const int c = col(token(j + g - 1));
+        if (c >= 0) x[c] = ban;
+      }
+    }
+  }
+  if (threadIdx.x == 0 && Lv < p.min_length[b] && p.eos_id[b] >= 0) {
+    const int c = col(p.eos_id[b]);
+    if (c >= 0) x[c] = ban;
+  }
+}
+
 static bool history_ok(const b2_token_history* h) {
   return h && h->tokens && h->len && h->prompt_len && h->table && h->distinct && h->n_distinct && h->max_len > 0 &&
          h->max_len < kInPrompt && h->vocab > 0;
@@ -237,6 +341,27 @@ int b2_penalize(void* logits, int rows, int n, int64_t ld, int64_t id_offset, co
   });
   if (e != cudaSuccess) {
     set_last_error("penalize", e);
+    return B2_ERR_CUDA;
+  }
+  return B2_OK;
+}
+
+int b2_penalize_tokens(void* logits, int batch, int q_len, const int32_t* parents, const int64_t* tokens, int n, int64_t ld,
+                       int64_t id_offset, const b2_token_history* hist, const b2_penalty_params* params, int ft, void* stream) {
+  if (!logits || !tokens || !history_ok(hist) || !params || !params->repetition || !params->presence || !params->frequency ||
+      !params->no_repeat_ngram || !params->min_length || !params->eos_id || !params->suppress)
+    return B2_ERR_PARAM;
+  if (batch < 0 || n < 1 || ld < n || id_offset < 0 || id_offset + n > hist->vocab) return B2_ERR_PARAM;
+  if (ft != B2_DT_BF16 && ft != B2_DT_F16) return B2_ERR_PARAM;
+  if (q_len < 1 || q_len > kMaxQLen || (int64_t)batch * q_len > INT32_MAX) return B2_ERR_LIMIT;
+  if (batch == 0) return B2_OK;
+  const cudaError_t e = with_flag(ft == B2_DT_F16, [&](auto h) {
+    constexpr bool H = decltype(h)::value;
+    return launch(penalize_tokens_kernel<H>, dim3((unsigned)(batch * q_len)), dim3(kPenThreads), 0, (cudaStream_t)stream, true,
+                  (__nv_bfloat16*)logits, n, ld, id_offset, *hist, *params, tokens, parents, q_len);
+  });
+  if (e != cudaSuccess) {
+    set_last_error("penalize_tokens", e);
     return B2_ERR_CUDA;
   }
   return B2_OK;

@@ -24,6 +24,7 @@ SYMBOLS = [
     "b2_sample_tokens", "b2_spec_accept_sampled",
     "b2_sample_shard_record_bytes", "b2_sample_shard_state_bytes", "b2_sample_shard", "b2_sample_shard_merge",
     "b2_history_load", "b2_history_append", "b2_penalize", "b2_history_append_tokens", "b2_ngram_draft",
+    "b2_penalize_tokens",
     "b2_comm_create", "b2_comm_destroy", "b2_comm_buffer_bytes", "b2_comm_export", "b2_comm_connect", "b2_comm_connect_pointers",
     "b2_comm_local_buffer", "b2_comm_error", "b2_allreduce", "b2_allgather", "b2_gemm_wq_run_allreduce",
 ]
@@ -160,6 +161,8 @@ def _load():
         "b2_history_append_tokens": (i32, [C.POINTER(TokenHistory), vp, vp, vp, i32, i32, vp]),
         "b2_ngram_draft": (i32, [vp, vp, vp, C.POINTER(TokenHistory), i32, i32, i32, i32, i32, vp]),
         "b2_penalize": (i32, [vp, i32, i32, i64, i64, C.POINTER(TokenHistory), C.POINTER(PenaltyParams), i32, vp]),
+        "b2_penalize_tokens": (i32, [vp, i32, i32, vp, vp, i32, i64, i64, C.POINTER(TokenHistory), C.POINTER(PenaltyParams),
+                                     i32, vp]),
         "b2_comm_create": (i32, [C.POINTER(vp), i32, i32, sz]),
         "b2_comm_destroy": (i32, [vp]),
         "b2_comm_buffer_bytes": (sz, [i32, sz]),

@@ -921,3 +921,21 @@ def penalize(logits, history, params, id_offset=0):
     check(lib.b2_penalize(_ptr(logits), rows, n, logits.stride(0), int(id_offset), C.byref(history.c), C.byref(params.c()),
                           _ft(logits), _stream()), "b2_penalize")
     return logits
+
+
+def penalize_tokens(logits, history, params, tokens, parents=None, id_offset=0):
+    """The logits processor of a verify step (b2_penalize_tokens), in place on logits [B * T, n] FT (any row stride), which
+    hold vocabulary ids [id_offset, id_offset + n): row b*T + t = draft node t of sequence b, processed as b2_penalize
+    would process it with history slot b followed by the drafts on the path from the root to t (tokens int64 [B, T], the
+    step's token array; parents int32 [B, T] for a draft tree, None for a chain).  Params row b is sequence b's; the
+    history is only read.  Returns logits."""
+    rows, n = logits.shape
+    B, T = tokens.shape
+    assert logits.stride(-1) == 1 and rows == B * T, f"penalize_tokens: logits rows must be B * T = {B * T}"
+    assert tokens.dtype == torch.int64 and tokens.is_contiguous()
+    assert parents is None or (parents.dtype == torch.int32 and parents.is_contiguous() and parents.shape == tokens.shape), \
+        f"penalize_tokens: parents must be [{B}, {T}] int32 contiguous"
+    assert B <= history.rows and B <= params.rows, "penalize_tokens: more sequences than history slots or parameter rows"
+    check(lib.b2_penalize_tokens(_ptr(logits), B, T, _ptr(parents), _ptr(tokens), n, logits.stride(0), int(id_offset),
+                                 C.byref(history.c), C.byref(params.c()), _ft(logits), _stream()), "b2_penalize_tokens")
+    return logits

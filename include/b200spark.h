@@ -606,6 +606,26 @@ typedef struct b2_penalty_params {
  * id_offset + n > vocab, a NULL pointer or an ft other than bf16 / fp16: B2_ERR_PARAM, before any launch. */
 int b2_penalize(void* logits, int rows, int n, int64_t ld, int64_t id_offset, const b2_token_history* hist,
                 const b2_penalty_params* params, int ft, void* stream);
+/* The logits processor of a verify step (b2_spec_accept / _tree / _sampled), in place, CUDA-graph replayable.  logits FT
+ * [batch * q_len, ld]: row r = b * q_len + t is draft node t of sequence b (tree format: b2_span_cache_append_tree;
+ * parents NULL: a chain).  tokens int64 [batch][q_len] is the array the append and accept kernels read; column 0 is never
+ * read.  History slot b and parameter row b are sequence b's (params [batch], as in b2_sample_tokens).
+ *   V(b, t): slot b (length L, prompt length P) followed by tokens[b][a_1 .. a_d], where a_1 < ... < a_d = t are the
+ *   non-root nodes on the path from the root to t (d = depth(t); a chain has a_i = i; a parent outside [0, t) is read as
+ *   the root), appended as b2_history_append appends: an id outside [0, vocab) is stored as -1 and counted nowhere, the
+ *   appends stop at max_len (L' = min(L + d, max_len)), and the prompt length stays P, so every path token counts as
+ *   generated.
+ * Row (b, t) is exactly, bit for bit, b2_penalize's result for that row with slot b holding V(b, t): repetition (with
+ * suppress), presence and frequency over the counts of V, the no-repeat n-gram over V (its tail may lie in the path) and
+ * min-length against L'.  So a verify row is processed as the single-token step with the same context would be, and a
+ * penalised speculative loop emits exactly the tokens of single-token penalised decoding.  q_len = 1 is b2_penalize on
+ * batch rows.  The history is only read; columns n .. ld-1 and ids outside the shard are never written (id_offset as in
+ * b2_penalize); neutral parameters leave the rows bit-identical.  One CTA per row.  A NULL required pointer, batch < 0,
+ * n < 1, ld < n, id_offset < 0, id_offset + n > vocab or an ft other than bf16 / fp16: B2_ERR_PARAM; q_len outside
+ * [1, 16] (or batch * q_len >= 2^31): B2_ERR_LIMIT; before any launch.  batch = 0 launches nothing. */
+int b2_penalize_tokens(void* logits, int batch, int q_len, const int32_t* parents /* NULL: chain */, const int64_t* tokens,
+                       int n, int64_t ld, int64_t id_offset, const b2_token_history* hist, const b2_penalty_params* params,
+                       int ft, void* stream);
 /* lens[b] += delta for b < batch (keeps sequence lengths device-resident under CUDA graphs) */
 int b2_lens_add(int32_t* lens, int batch, int delta, void* stream);
 /* Greedy verification of a multi-token step, on the device (CUDA-graph replayable).  tokens [batch][q_len] int64: column 0
