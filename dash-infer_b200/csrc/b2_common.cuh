@@ -106,6 +106,10 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
 // ---- thread-block clusters: barrier + distributed shared memory reads
 __device__ __forceinline__ void cluster_arrive() { asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory"); }
 __device__ __forceinline__ void cluster_wait() { asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory"); }
+__device__ __forceinline__ void cluster_sync() {
+  cluster_arrive();
+  cluster_wait();
+}
 __device__ __forceinline__ uint32_t dsmem_addr(uint32_t local_smem_addr, uint32_t cta_rank) {
   uint32_t r;
   asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_smem_addr), "r"(cta_rank));
@@ -119,6 +123,17 @@ __device__ __forceinline__ float4 ld_dsmem_f4(uint32_t addr) {
 __device__ __forceinline__ float ld_dsmem_f(uint32_t addr) {
   float v;
   asm volatile("ld.shared::cluster.f32 %0, [%1];" : "=f"(v) : "r"(addr) : "memory");
+  return v;
+}
+// the word at p (this CTA's shared memory) in CTA cta of the cluster
+__device__ __forceinline__ uint32_t ld_dsmem_u32(const void* p, uint32_t cta) {
+  uint32_t v;
+  asm volatile("ld.shared::cluster.u32 %0, [%1];" : "=r"(v) : "r"(dsmem_addr(smem_u32(p), cta)) : "memory");
+  return v;
+}
+__device__ __forceinline__ unsigned long long ld_dsmem_u64(const void* p, uint32_t cta) {
+  unsigned long long v;
+  asm volatile("ld.shared::cluster.u64 %0, [%1];" : "=l"(v) : "r"(dsmem_addr(smem_u32(p), cta)) : "memory");
   return v;
 }
 
@@ -368,6 +383,15 @@ __device__ __forceinline__ bool argmax_beats(float v, int i, float best, int bi)
   const bool vn = v != v, bn = best != best;
   if (vn != bn) return vn;
   return (!vn && v > best) || ((vn || v == best) && i < bi);
+}
+// the warp's best (v, i) under argmax_beats, in every lane
+__device__ __forceinline__ void warp_argmax(float& v, int& i) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float ov = __shfl_xor_sync(0xffffffffu, v, o);
+    const int oi = __shfl_xor_sync(0xffffffffu, i, o);
+    if (argmax_beats(ov, oi, v, i)) { v = ov; i = oi; }
+  }
 }
 
 template <int ACT>

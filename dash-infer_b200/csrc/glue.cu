@@ -281,23 +281,13 @@ __global__ void __launch_bounds__(1024) argmax_kernel(int64_t* __restrict__ ids_
     const float v = Ft<H>::to_f(row[i]);
     if (argmax_beats(v, i, best, bi)) { best = v; bi = i; }
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const float ov = __shfl_xor_sync(0xffffffffu, best, o);
-    const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-    if (argmax_beats(ov, oi, best, bi)) { best = ov; bi = oi; }
-  }
+  warp_argmax(best, bi);
   if ((threadIdx.x & 31) == 0) { sv[threadIdx.x >> 5] = best; si[threadIdx.x >> 5] = bi; }
   __syncthreads();
   if (threadIdx.x < 32) {
     best = sv[threadIdx.x];
     bi = si[threadIdx.x];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const float ov = __shfl_xor_sync(0xffffffffu, best, o);
-      const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-      if (argmax_beats(ov, oi, best, bi)) { best = ov; bi = oi; }
-    }
+    warp_argmax(best, bi);
     if (threadIdx.x == 0) {
       ids_out[b] = bi + id_offset;
       if (vals_out) vals_out[b] = best;

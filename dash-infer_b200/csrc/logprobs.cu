@@ -52,23 +52,11 @@ __device__ __forceinline__ void lp_insert(float (&v)[K], int (&id)[K], float x, 
   }
 }
 
-__device__ __forceinline__ void lp_warp_best(float& v, int& i) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const float ov = __shfl_xor_sync(0xffffffffu, v, o);
-    const int oi = __shfl_xor_sync(0xffffffffu, i, o);
-    if (argmax_beats(ov, oi, v, i)) { v = ov; i = oi; }
-  }
-}
-
 // Rows longer than kLpSplitMin run on a cluster of kLpCtas CTAs, CTA c taking the elements c * 1024 + t + 1024 kLpCtas j
 // (a function of n alone, so a row gives the same bits at every batch size).
 constexpr int kLpCtas = 8;
 constexpr int kLpSplitMin = 32768;
 __host__ __device__ constexpr int lp_ctas(int n) { return n > kLpSplitMin ? kLpCtas : 1; }
-
-__device__ __forceinline__ float ld_dsmem_at(const void* p, uint32_t cta) { return ld_dsmem_f(dsmem_addr(smem_u32(p), cta)); }
-__device__ __forceinline__ int ld_dsmem_int_at(const void* p, uint32_t cta) { return __float_as_int(ld_dsmem_at(p, cta)); }
 
 // The per-row reduction shared by the whole-row and the shard kernels: the `nc` CTAs of a cluster (nc = lp_ctas(n)) fill the
 // record `rec` (shared memory of the cluster's CTA 0) of row r.
@@ -115,7 +103,7 @@ __device__ __forceinline__ void lp_row(LpHead* rec, const __nv_bfloat16* __restr
     const float x = F::to_f(row[i]);
     if (argmax_beats(x, i, bv, bi)) { bv = x; bi = i; }
   }
-  lp_warp_best(bv, bi);
+  warp_argmax(bv, bi);
   if (lane == 0) { sv[w] = bv; si[w] = bi; }
   __syncthreads();
   if (w == 0) {
@@ -129,12 +117,11 @@ __device__ __forceinline__ void lp_row(LpHead* rec, const __nv_bfloat16* __restr
     if (rank == 0) { cb_v = cv; cb_i = ci; }
     if (rank == kk - 1 && ci != INT_MAX) { tv = cv; ti = ci; }
   }
-  cluster_arrive();  // the CTAs' bests are visible cluster-wide after the wait (it also orders the block)
-  cluster_wait();
+  cluster_sync();  // the CTAs' bests are visible cluster-wide after it (it also orders the block)
   if (w == 0) {
-    float mv = lane < nc ? ld_dsmem_at(&cb_v, lane) : -INFINITY;
-    int mi = lane < nc ? ld_dsmem_int_at(&cb_i, lane) : INT_MAX;
-    lp_warp_best(mv, mi);
+    float mv = lane < nc ? __uint_as_float(ld_dsmem_u32(&cb_v, lane)) : -INFINITY;
+    int mi = lane < nc ? (int)ld_dsmem_u32(&cb_i, lane) : INT_MAX;
+    warp_argmax(mv, mi);
     if (lane == 0) m_sh = mv;
   }
   __syncthreads();
@@ -173,7 +160,7 @@ __device__ __forceinline__ void lp_row(LpHead* rec, const __nv_bfloat16* __restr
     for (int k = 0; k < kk; ++k) {  // the warp's list: kk rounds of "pop the best head" over its lanes
       float hv = v[0];
       int hi = id[0];
-      lp_warp_best(hv, hi);
+      warp_argmax(hv, hi);
       if (lane == 0) { wl_v[w][k] = hv; wl_i[w][k] = hi; }
       if (hi != INT_MAX && id[0] == hi) {
 #pragma unroll
@@ -195,20 +182,19 @@ __device__ __forceinline__ void lp_row(LpHead* rec, const __nv_bfloat16* __restr
         float hv = p < kk ? wl_v[lane][p] : -INFINITY;
         int hi = p < kk ? wl_i[lane][p] : INT_MAX;
         const int mine = hi;
-        lp_warp_best(hv, hi);
+        warp_argmax(hv, hi);
         if (lane == 0) { cl_v[k] = hv; cl_i[k] = hi; }
         if (hi != INT_MAX && mine == hi) ++p;
       }
     }
   }
-  cluster_arrive();  // every CTA's list and partial sum are ready
-  cluster_wait();
+  cluster_sync();  // every CTA's list and partial sum are ready
   if (c == 0) {  // the row's list from the nc CTA lists, the sum in CTA order
     if (tid < nc * kk) {
-      ml_v[tid] = ld_dsmem_at(&cl_v[tid % kk], tid / kk);
-      ml_i[tid] = ld_dsmem_int_at(&cl_i[tid % kk], tid / kk);
+      ml_v[tid] = __uint_as_float(ld_dsmem_u32(&cl_v[tid % kk], tid / kk));
+      ml_i[tid] = (int)ld_dsmem_u32(&cl_i[tid % kk], tid / kk);
     }
-    if (tid < nc) ml_s[tid] = ld_dsmem_at(&cs, tid);
+    if (tid < nc) ml_s[tid] = __uint_as_float(ld_dsmem_u32(&cs, tid));
     if (tid < kk) { vals[tid] = -INFINITY; ids[tid] = INT_MAX; }
     __syncthreads();
     if (tid < nc * kk) {
@@ -232,8 +218,7 @@ __device__ __forceinline__ void lp_row(LpHead* rec, const __nv_bfloat16* __restr
       }
     }
   }
-  cluster_arrive();  // no CTA leaves while CTA 0 reads its shared memory
-  cluster_wait();
+  cluster_sync();  // no CTA leaves while CTA 0 reads its shared memory
 }
 
 // Finish row r from the records of nranks shards (rank q's at recs + q * rank_stride), one thread:
