@@ -187,6 +187,17 @@ if os.environ.get("B2_PDL", "1") == "0":
     lib.b2_set_pdl(0)
 
 
-def check(status, what=""):
+# Library calls checked so far, plus the launches beyond the first that a call reports (a GEMM's row chunks).  Every
+# launching entry point goes through check(), so the difference across a piece of host code is the kernels it launched
+# (DecodeStack.launches_per_step) provided that code makes no checked call that launches nothing: create / destroy,
+# prepare, connect, b2_comm_error (Comm.check_error), b2_history_load, b2_span_context_copy and the like are also counted
+# and must stay out of DecodeStack._step_ops.  tests/test_stack_launches_gpu.py compares the count with the kernel nodes of
+# a captured step.
+calls = 0
+
+
+def check(status, what="", launches=1):
+    global calls
+    calls += launches
     if status != 0:
         raise B2Error(f"{what}: {lib.b2_status_string(status).decode()} ({lib.b2_last_error().decode()})")

@@ -10,11 +10,13 @@ Graph per layer (reference order, with the fusions the C ABI offers):
   -> GemmA16Wx(o_proj) (+residual) -> RMSNorm -> GemmA16Wx(gate, SiLU) -> GemmA16Wx(up) -> MUL
   -> GemmA16Wx(down) (+residual);  final RMSNorm -> Gemm(lm_head, bf16) -> argmax.
 """
+import os
 from dataclasses import dataclass
 
 import torch
+import torch.distributed as dist
 
-from . import ops, quantize as PQ, tp as TP
+from . import _lib, ops, quantize as PQ, tp as TP
 from ._lib import ACT_NONE, ACT_SILU, BIN_MUL, KV_FP8, KV_I8, KV_NONE, KV_U4
 
 
@@ -64,6 +66,19 @@ def synth_weight(K, N, gen, device, std=0.02):
     return (torch.randn(K, N, generator=gen, device=device, dtype=torch.float32) * std).to(_DT)
 
 
+def _quantize(w, wbits, group, keep_ref):
+    """IQ quantizer of a synthetic [K, N] weight: (q, scales, zeros, ref); wbits 16 keeps the weight dense (no scales or
+    zeros).  ref: the dense fp32 (q - z) * s of the FULL matrix for the CPU oracle (keep_ref), else None."""
+    if wbits == 4:
+        q, s, z = PQ.quantize_a16w4(w, group)
+    elif wbits == 8:
+        q, s, z = PQ.quantize_a16w8(w, group)
+    else:
+        q, s, z = w, None, None
+    ref = (PQ.dequantize(q, s, z, group, wbits, w.shape[1]) if wbits != 16 else w.float()).cpu() if keep_ref else None
+    return q, s, z, ref
+
+
 class QuantLinear:
     """One projection: synthetic bf16 weight -> IQ quantizer -> (TP shard) -> GemmWQ handle (keeps nothing but the handle).
     shard: None | ("cols", ranges) | ("rows", rank, tp)."""
@@ -71,15 +86,8 @@ class QuantLinear:
     def __init__(self, K, N, wbits, group, gen, device, max_m, bias=False, keep_ref=False, shard=None):
         w = synth_weight(K, N, gen, device)
         b = (torch.randn(N, generator=gen, device=device) * 0.02).to(_DT) if bias else None
-        if wbits == 4:
-            q, s, z = PQ.quantize_a16w4(w, group)
-        elif wbits == 8:
-            q, s, z = PQ.quantize_a16w8(w, group)
-        else:
-            q, s, z = w, None, None
-        self.ref = None
-        if keep_ref:  # dense fp32 (q - z) * s of the FULL matrix for the CPU oracle
-            self.ref = (PQ.dequantize(q, s, z, group, wbits, N) if wbits != 16 else w.float()).cpu()
+        q, s, z, self.ref = _quantize(w, wbits, group, keep_ref)
+        if keep_ref:
             self.ref_bias = b.float().cpu() if b is not None else None
         if shard is not None:
             if shard[0] == "cols":
@@ -106,15 +114,9 @@ class SwiGLULinear:
         qs = []
         self.ref = []
         for _ in range(2):
-            w = synth_weight(K, N, gen, device)
-            if wbits == 4:
-                q, s, z = PQ.quantize_a16w4(w, group)
-            elif wbits == 8:
-                q, s, z = PQ.quantize_a16w8(w, group)
-            else:
-                q, s, z = w, None, None
+            q, s, z, ref = _quantize(synth_weight(K, N, gen, device), wbits, group, keep_ref)
             if keep_ref:
-                self.ref.append((PQ.dequantize(q, s, z, group, wbits, N) if wbits != 16 else w.float()).cpu())
+                self.ref.append(ref)
             if shard is not None:
                 q, s, z, _ = TP.shard_cols(q, s, z, None, wbits, shard[1])
             qs.append((q, s, z))
@@ -212,9 +214,6 @@ class DecodeStack:
             assert 1 <= width <= q_len - 1 and (width == 1 or tree), \
                 "ngram=(n_min, n_max, width): 1 <= width <= q_len - 1, and width > 1 drafts a tree (tree=True)"
             ngram = (int(n_min), int(n_max), int(width))
-        import os
-
-        import torch.distributed as dist
         collective = collective or os.environ.get("B2_TP_COLLECTIVE", "b2")
         # a rank reaches its peers through a torch.distributed process group (the "nccl" collectives, and the handle
         # exchange that connects the communicator), or through a communicator the caller connected; refuse before any
@@ -281,91 +280,100 @@ class DecodeStack:
         # rope scaling: one fp32 frequency table on the device, shared by every layer and sequence (every TP rank builds the
         # same one); without it the append computes base^(-2f / head) itself, as before
         self.rope = (cfg.rope_base, hd) if cfg.rope_scaling is None else ops.rope_table(cfg.rope_scaling, cfg.rope_base, hd, device)
-        # device-resident step state, allocated for the construction batch; set_batch() re-views it for a smaller batch
-        self.Bmax = batch
-        self._lens_old = torch.zeros(batch, dtype=torch.int32, device=device)
-        self._lens_new = torch.full((batch,), q_len, dtype=torch.int32, device=device)  # lens_old + q_len
-        self._ids = torch.zeros(batch, dtype=torch.int64, device=device)
-        self._next_ids = torch.zeros(batch, dtype=torch.int64, device=device)
-        if sample or sampled_verify:
-            self._temperature = torch.ones(batch, dtype=torch.float32, device=device)
-            self._top_k = torch.zeros(batch, dtype=torch.int32, device=device)
-            self._top_p = torch.ones(batch, dtype=torch.float32, device=device)
-            self._seeds = torch.zeros(batch, dtype=torch.int64, device=device)
-            self._offsets = torch.zeros(batch, dtype=torch.int64, device=device)
-        if penalties or ngram:
-            self._history = ops.TokenHistory(batch, max_len, cfg.vocab, device)
-        if penalties:
-            self._penalties = ops.Penalties(batch, device)
-        if ngram:
-            self._n_draft = torch.zeros(batch, dtype=torch.int32, device=device)
-        if q_len > 1:
-            self._tokens = torch.zeros(batch, q_len, dtype=torch.int64, device=device)
-            self._pred = torch.zeros(batch, q_len, dtype=torch.int64, device=device)
-            self._accepted = torch.zeros(batch, dtype=torch.int32, device=device)
-        if tree:  # a chain until the caller writes its trees
-            self._parents = (torch.arange(q_len, dtype=torch.int32, device=device) - 1).clamp_(min=0).repeat(batch, 1)
-            self._path = torch.zeros(batch, q_len, dtype=torch.int32, device=device)
-        bf = dict(dtype=_DT, device=device)
-        self._bufs = dict(x=torch.empty(rows, H, **bf), xn=torch.empty(rows, H, **bf),
-                          qkv=torch.empty(rows, (nHl + 2 * nGl) * hd, **bf), q=torch.empty(rows, nHl * hd, **bf),
-                          ao=torch.empty(rows, nHl * hd, **bf), gate=torch.empty(rows, self.I_l, **bf),
-                          up=torch.empty(rows, self.I_l, **bf), logits=torch.empty(rows, self.vocab_l, **bf))
-        if logprobs:
-            self._bufs.update(tok_lp=torch.empty(rows, dtype=torch.float32, device=device),
-                              top_ids=torch.empty(rows, logprobs, dtype=torch.int64, device=device),
-                              top_lp=torch.empty(rows, logprobs, dtype=torch.float32, device=device))
-        if tp > 1:
-            rec = ops.logprobs_partial_bytes(logprobs) if logprobs else 0
-            if logprobs:  # one record per row and rank (b2_logprobs_shard), all-gathered as bytes
-                self._bufs["loc_rec"] = torch.empty(batch, rec, dtype=torch.uint8, device=device)
-                self._all_rec = torch.empty(tp * batch * rec, dtype=torch.uint8, device=device)
-            if sample:  # this rank's state and records of the vocab-split draw (b2_sample_shard), for the construction batch
-                self._stp = ops.sample_tp_buffers(batch, tp, device)
-            if self.collective != "nccl" and self.comm is None:  # the largest exchange: activations, or a phase-1 record
-                rec_max = max(rec, ops.sample_shard_record_bytes(1) if sample else 0)
-                self.comm = ops.Comm(tp_rank, tp, max(batch * H * 2, 4096, batch * rec_max)).connect_group(tp_group)
-            self._bufs["part"] = torch.empty(batch, H, **bf)             # row-split partial sums (all-reduced)
-            if not logprobs:  # the argmax path's per-rank (max, argmax) pairs
-                self.loc_ids = torch.empty(batch, dtype=torch.int64, device=device)
-                self.loc_val = torch.empty(batch, dtype=torch.float32, device=device)
-                self.all_ids = torch.empty(tp, batch, dtype=torch.int64, device=device)
-                self.all_val = torch.empty(tp, batch, dtype=torch.float32, device=device)
+        rec = ops.logprobs_partial_bytes(logprobs) if logprobs else 0  # bytes of one row's logprob record (TP > 1)
+        if tp > 1 and self.collective != "nccl" and self.comm is None:  # the largest exchange: activations, or a record
+            rec_max = max(rec, ops.sample_shard_record_bytes(1) if sample else 0)
+            self.comm = ops.Comm(tp_rank, tp, max(batch * H * 2, 4096, batch * rec_max)).connect_group(tp_group)
+        # The step state, declared once: every array a step reads or writes per sequence or per activation row.  Columns:
+        # the layout for b sequences, dtype, initial value (None: uninitialised), whether this stack needs it, and whether a
+        # step carries it to the next (capture() rewinds those after its warm-up step).  Layouts: per_seq(*s) is [b, *s];
+        # per_row(*s) is [b * T, *s], a row per token; gathered(n, k) is [n, b * k], the layout an all-gather writes (n ranks)
+        # and the per-tile row statistics take (n tiles).  Without a dtype, the layout makes an object for b sequences
+        # that views a prefix of them itself (.view(b)).  self._<name> holds the construction batch's array and
+        # self.<name> the current batch's view (set_batch); both are None when the stack does not need it.
+        T, i32, i64, f32, u8 = q_len, torch.int32, torch.int64, torch.float32, torch.uint8
+        per_seq = lambda *s: lambda b: (b, *s)
+        per_row = lambda *s: lambda b: (b * T, *s)
+        gathered = lambda n, k=1: lambda b: (n, b * k)
+        drawn, greedy_tp, lp_tp = sample or sampled_verify, tp > 1 and not logprobs, tp > 1 and logprobs > 0
+        handoff = self._norm_placement(rows) == "handoff"
+        chain = (torch.arange(T) - 1).clamp_(min=0)  # the parents of a chain: a tree stack's drafts until the caller writes trees
+        state = (
+            ("lens_old", per_seq(), i32, 0, True, True),
+            ("lens_new", per_seq(), i32, T, True, True),  # lens_old + q_len
+            ("ids", per_seq(), i64, 0, True, False),
+            ("next_ids", per_seq(), i64, 0, True, False),
+            ("tokens", per_seq(T), i64, 0, T > 1, True),
+            ("pred", per_seq(T), i64, 0, T > 1, False),
+            ("accepted", per_seq(), i32, 0, T > 1, False),
+            ("parents", per_seq(T), i32, chain, tree, False),
+            ("path", per_seq(T), i32, 0, tree, False),
+            ("temperature", per_seq(), f32, 1.0, drawn, False),
+            ("top_k", per_seq(), i32, 0, drawn, False),
+            ("top_p", per_seq(), f32, 1.0, drawn, False),
+            ("seeds", per_seq(), i64, 0, drawn, False),
+            ("offsets", per_seq(), i64, 0, drawn, True),
+            ("history", lambda b: ops.TokenHistory(b, max_len, cfg.vocab, device), None, None, penalties or ngram is not None,
+             True),
+            ("penalties", lambda b: ops.Penalties(b, device), None, None, penalties, False),
+            ("n_draft", per_seq(), i32, 0, ngram is not None, False),
+            ("x", per_row(H), _DT, None, True, False),
+            ("xn", per_row(H), _DT, None, True, False),
+            ("qkv", per_row((nHl + 2 * nGl) * hd), _DT, None, True, False),
+            ("q", per_row(nHl * hd), _DT, None, True, False),
+            ("ao", per_row(nHl * hd), _DT, None, True, False),
+            ("gate", per_row(self.I_l), _DT, None, True, False),
+            ("up", per_row(self.I_l), _DT, None, True, False),
+            ("logits", per_row(self.vocab_l), _DT, None, True, False),
+            ("tok_lp", per_row(), f32, None, logprobs > 0, False),
+            ("top_ids", per_row(logprobs), i64, None, logprobs > 0, False),
+            ("top_lp", per_row(logprobs), f32, None, logprobs > 0, False),
+            # per-tile row statistics of o_proj / down_proj ([tiles][R] per step) for the next norm
+            ("ssq_o", gathered(self.layers[0]["o"].op.sumsq_parts(), T), f32, 0, handoff, False),
+            ("ssq_d", gathered(self.layers[0]["down"].op.sumsq_parts(), T), f32, 0, handoff, False),
+            ("part", per_row(H), _DT, None, tp > 1, False),  # row-split partial sums (all-reduced)
+            # the vocab-split argmax: per-rank (max, argmax) pairs and their all-gathers
+            ("loc_ids", per_seq(), i64, None, greedy_tp, False),
+            ("loc_val", per_seq(), f32, None, greedy_tp, False),
+            ("all_ids", gathered(tp), i64, None, greedy_tp, False),
+            ("all_val", gathered(tp), f32, None, greedy_tp, False),
+            # vocab-split logprobs: one record per row and rank (b2_logprobs_shard), all-gathered as bytes
+            ("loc_rec", per_seq(rec), u8, None, lp_tp, False),
+            ("all_rec", gathered(tp, rec), u8, None, lp_tp, False),
+            # this rank's state and records of the vocab-split draw (b2_sample_shard)
+            ("stp", lambda b: ops.sample_tp_buffers(b, tp, device), None, None, sample and tp > 1, False),
+        )
+        self.Bmax, self._layouts, self._carried = batch, {}, []
+        for name, layout, dt, init, needed, carried in state:
+            full = None
+            if needed:
+                if dt is None:
+                    full = layout(batch)
+                else:
+                    full = torch.empty(layout(batch), dtype=dt, device=device)
+                    if init is not None:
+                        full.copy_(torch.as_tensor(init))
+                self._layouts[name] = layout
+                if carried:
+                    self._carried.append(name)
+            setattr(self, "_" + name, full)
+            setattr(self, name, full)
         self.graph = None
         self.set_batch(batch)
-        if self._norm_placement(rows) == "handoff":  # per-tile row statistics of o_proj / down_proj, [tiles][R] per step
-            self._ssq_o = torch.zeros(self.layers[0]["o"].op.sumsq_parts() * rows, dtype=torch.float32, device=device)
-            self._ssq_d = torch.zeros(self.layers[0]["down"].op.sumsq_parts() * rows, dtype=torch.float32, device=device)
         self.launches_per_step = 0
 
     def set_batch(self, b):
-        """Run the next steps with the first `b` sequences only (b <= construction batch): every step buffer, the length
-        vectors and the span tables are re-viewed (row-major, so the first b rows are contiguous); a captured graph is
-        dropped.  bench.py measures batch 64, 8 and 1 on ONE set of weights and caches this way."""
+        """Run the next steps with the first `b` sequences only (b <= construction batch): every array of the step state is
+        re-viewed (its first b sequences are a prefix of its storage); a captured graph is dropped.  bench.py measures batch
+        64, 8 and 1 on ONE set of weights and caches this way."""
         assert 1 <= b <= self.Bmax
         self.B = b
-        for k, v in self._bufs.items():
-            setattr(self, k, v[:b * self.q_len])
-        self.lens_old, self.lens_new = self._lens_old[:b], self._lens_new[:b]
-        self.ids, self.next_ids = self._ids[:b], self._next_ids[:b]
-        if self.q_len > 1:
-            self.tokens, self.pred, self.accepted = self._tokens[:b], self._pred[:b], self._accepted[:b]
-        if self.tree:
-            self.parents, self.path = self._parents[:b], self._path[:b]
-        if self.sample or self.sv:
-            for k in ("temperature", "top_k", "top_p", "seeds", "offsets"):
-                setattr(self, k, getattr(self, "_" + k)[:b])
-        if self.pen:
-            self.history, self.penalties = self._history.view(b), self._penalties.view(b)
-        if self.ngram:
-            self.history, self.n_draft = self._history.view(b), self._n_draft[:b]
-        if self.logprobs and self.tp > 1:
-            rec = self._all_rec.numel() // (self.tp * self.Bmax)
-            self.all_rec = self._all_rec[:self.tp * b * rec].view(self.tp, b * rec)
-        if self.sample and self.tp > 1:
-            f = self._stp
-            self.stp = {"state": f["state"][:b], "rec": [r[:b] for r in f["rec"]],
-                        "all": [a.view(-1)[:a.numel() // self.Bmax * b].view(self.tp, -1) for a in f["all"]]}
+        for name, layout in self._layouts.items():
+            full = getattr(self, "_" + name)
+            if isinstance(full, torch.Tensor):
+                setattr(self, name, full.view(-1)[:full.numel() // self.Bmax * b].view(layout(b)))
+            else:
+                setattr(self, name, full.view(b))
         self.graph = None
 
     def set_sampling(self, temperature=None, top_k=None, top_p=None, seeds=None, offsets=None):
@@ -406,7 +414,7 @@ class DecodeStack:
             for t in range(ctx):
                 rows = torch.randn(self.Bmax, width, generator=gen, device=self.device).to(self.dtype)
                 for L in self.layers:
-                    ops.cache_append(L["cache"], rows, pos, q_out=self._bufs["q"])
+                    ops.cache_append(L["cache"], rows, pos, q_out=self._q)
                 pos += 1
         for b in range(self.Bmax if self.head == 128 else 0):
             rows = torch.randn(ctx, kw + vw, generator=gen, device=self.device).to(self.dtype)
@@ -418,24 +426,19 @@ class DecodeStack:
         torch.cuda.synchronize()
 
     # ------------------------------------------------------------------ one decode step (eager or captured)
-    def _row_parallel(self, lin, inp, n):
+    def _row_parallel(self, lin, inp):
         """o_proj / down_proj.  TP=1: residual fused in the GEMM epilogue.  TP>1: per-rank partial sums exchanged over NVLink
         (reference: AllReduceOp after o_proj and down_proj, allreduce_op.cpp:73-115 — here stream-ordered, no host sync);
         the residual is added once, after the sum, on every rank."""
         if self.tp == 1:
             lin(inp, self.ws, out=self.x, residual=self.x)
-            return n + 1
-        if self.collective == "nccl":
-            import torch.distributed as dist
+        elif self.collective == "nccl":
             lin(inp, self.ws, out=self.part, residual=self.x if self.tp_rank == 0 else None)
             dist.all_reduce(self.part, group=self.tp_group)
             self.x.copy_(self.part)
-            return n + 1
-        if self.collective == "fused" and lin.op.run_allreduce(inp, self.ws, self.comm, out=self.x, residual=self.x):
-            return n + 1
-        lin(inp, self.ws, out=self.part)
-        self.comm.allreduce(self.part, out=self.x, residual=self.x)
-        return n + 2
+        elif self.collective != "fused" or not lin.op.run_allreduce(inp, self.ws, self.comm, out=self.x, residual=self.x):
+            lin(inp, self.ws, out=self.part)  # "b2", and "fused" where the fused form does not cover the call
+            self.comm.allreduce(self.part, out=self.x, residual=self.x)
 
     @property
     def collective_impl(self):
@@ -445,12 +448,18 @@ class DecodeStack:
     def _allreduce(self, t, out=None):
         """the exchange alone (collective_probe)"""
         if self.collective == "nccl":
-            import torch.distributed as dist
             dist.all_reduce(t, group=self.tp_group)
             if out is not None:
                 out.copy_(t)
         else:
             self.comm.allreduce(t, out=out if out is not None else t)
+
+    def _gather(self, rec, all_rec):
+        """all-gather this rank's records (opaque bytes, [rows, bytes]) into all_rec [tp, rows * bytes], in rank order"""
+        if self.collective == "nccl":
+            dist.all_gather_into_tensor(all_rec.view(-1), rec.view(-1), group=self.tp_group)
+        else:
+            self.comm.allgather(rec, all_rec)
 
     def _norm_placement(self, R):
         """Where a step of R activation rows runs its RMSNorms.
@@ -474,131 +483,100 @@ class DecodeStack:
         cfg, ws = self.cfg, self.ws
         H = cfg.hidden
         T = self.q_len
-        R = self.B * T  # activation rows
-        norm = self._norm_placement(R)
-        if norm == "handoff":
-            ssq_o = self._ssq_o[:self._ssq_o.numel() // self.Bmax * self.B].view(-1, R)
-            ssq_d = self._ssq_d[:self._ssq_d.numel() // self.Bmax * self.B].view(-1, R)
+        norm = self._norm_placement(self.B * T)
+        # The flags choose the step's form, not which arrays were allocated: a stack built with tree, sampled_verify, ngram
+        # or penalties may have the flag switched off and capture the other form (tools/spec_bench.py, penalty_bench.py).
+        parents, path = (self.parents, self.path) if self.tree else (None, None)
         # the step form of append + attention: single token, chain of T tokens, or draft tree
-        form = {} if T == 1 else {"q_len": T, "parents": self.parents if self.tree else None}
-        n = 0
+        form = {} if T == 1 else {"q_len": T, "parents": parents}
         if self.ngram:  # this step's drafts, from the history the previous step extended
-            ops.ngram_draft(self.history, self.tokens, self.parents if self.tree else None, *self.ngram, n_draft=self.n_draft)
-            n += 1
-        ops.embedding(self.embed, self.ids if T == 1 else self.tokens.view(-1), out=self.x); n += 1
+            ops.ngram_draft(self.history, self.tokens, parents, *self.ngram, n_draft=self.n_draft)
+        ops.embedding(self.embed, self.ids if T == 1 else self.tokens.view(-1), out=self.x)
         for li, L in enumerate(self.layers):
             if norm == "self":
-                L["qkv"](self.x, ws, out=self.qkv, norm_in=(None, L["g1"], H, cfg.eps)); n += 1
+                L["qkv"](self.x, ws, out=self.qkv, norm_in=(None, L["g1"], H, cfg.eps))
             elif norm == "handoff" and li > 0:  # xn = bf16(x * g1) and the row statistics were written by the previous layer's down_proj
-                L["qkv"](self.xn, ws, out=self.qkv, norm_in=(ssq_d, None, H, cfg.eps)); n += 1
+                L["qkv"](self.xn, ws, out=self.qkv, norm_in=(self.ssq_d, None, H, cfg.eps))
             else:
-                ops.rmsnorm(self.x, L["g1"], cfg.eps, out=self.xn); n += 1
-                L["qkv"](self.xn, ws, out=self.qkv); n += 1
+                ops.rmsnorm(self.x, L["g1"], cfg.eps, out=self.xn)
+                L["qkv"](self.xn, ws, out=self.qkv)
             ops._cache_append(L["cache"], self.qkv, self.lens_old, q_out=self.q, rope=self.rope,
-                              qk_norm=(L["qn"], L["kn"], cfg.eps) if cfg.qk_norm else None, **form); n += 1
-            self.attn._run(self.q, L["cache"], self.lens_new, self.max_len, ws, out=self.ao, **form); n += 1
+                              qk_norm=(L["qn"], L["kn"], cfg.eps) if cfg.qk_norm else None, **form)
+            self.attn._run(self.q, L["cache"], self.lens_new, self.max_len, ws, out=self.ao, **form)
             if norm == "self":
-                n = self._row_parallel(L["o"], self.ao, n)
+                self._row_parallel(L["o"], self.ao)
                 mlp_in, nin = self.x, (None, L["g2"], H, cfg.eps)
             elif norm == "handoff":
-                L["o"](self.ao, ws, out=self.x, residual=self.x, sumsq_out=ssq_o, xg_out=(self.xn, L["g2"])); n += 1
-                mlp_in, nin = self.xn, (ssq_o, None, H, cfg.eps)
+                L["o"](self.ao, ws, out=self.x, residual=self.x, sumsq_out=self.ssq_o, xg_out=(self.xn, L["g2"]))
+                mlp_in, nin = self.xn, (self.ssq_o, None, H, cfg.eps)
             else:
-                n = self._row_parallel(L["o"], self.ao, n)
-                ops.rmsnorm(self.x, L["g2"], cfg.eps, out=self.xn); n += 1
+                self._row_parallel(L["o"], self.ao)
+                ops.rmsnorm(self.x, L["g2"], cfg.eps, out=self.xn)
                 mlp_in, nin = self.xn, None
             if self.fuse_swiglu:
-                L["gateup"](mlp_in, ws, out=self.gate, norm_in=nin); n += 1
+                L["gateup"](mlp_in, ws, out=self.gate, norm_in=nin)
             else:
-                L["gate"](mlp_in, ws, out=self.gate, act=ACT_SILU, norm_in=nin); n += 1
-                L["up"](mlp_in, ws, out=self.up, norm_in=nin); n += 1
-                ops.binary(self.gate, self.up, BIN_MUL, out=self.gate); n += 1
+                L["gate"](mlp_in, ws, out=self.gate, act=ACT_SILU, norm_in=nin)
+                L["up"](mlp_in, ws, out=self.up, norm_in=nin)
+                ops.binary(self.gate, self.up, BIN_MUL, out=self.gate)
             if norm == "handoff":
                 g_next = self.layers[li + 1]["g1"] if li + 1 < len(self.layers) else self.gf
-                L["down"](self.gate, ws, out=self.x, residual=self.x, sumsq_out=ssq_d, xg_out=(self.xn, g_next)); n += 1
+                L["down"](self.gate, ws, out=self.x, residual=self.x, sumsq_out=self.ssq_d, xg_out=(self.xn, g_next))
             else:
-                n = self._row_parallel(L["down"], self.gate, n)
+                self._row_parallel(L["down"], self.gate)
         if norm == "handoff":
-            self.lm_head(self.xn, ws, out=self.logits, norm_in=(ssq_d, None, H, cfg.eps)); n += 1
+            self.lm_head(self.xn, ws, out=self.logits, norm_in=(self.ssq_d, None, H, cfg.eps))
         else:
-            ops.rmsnorm(self.x, self.gf, cfg.eps, out=self.xn); n += 1
-            self.lm_head(self.xn, ws, out=self.logits); n += 1
+            ops.rmsnorm(self.x, self.gf, cfg.eps, out=self.xn)
+            self.lm_head(self.xn, ws, out=self.logits)
+        # the token choice: one id per row, drawn or the argmax, with the log-probabilities if asked for
+        ids = self.next_ids if T == 1 else self.pred.view(-1)
+        drawn = self.sample or self.sv
         if self.pen:  # the logits processor, in place on this rank's vocab shard
-            ops.penalize(self.logits, self.history, self.penalties, self.tp_rank * self.vocab_l); n += 1
-        if self.sv:  # every row's draw; with logprobs, the log-probabilities at them (one launch more)
-            ops.sample_tokens(self.logits, T, self.temperature, self.top_k, self.top_p, self.seeds, self.offsets,
-                              self.parents if self.tree else None, out=self.pred.view(-1)); n += 1
-            if self.logprobs:
-                ops.logprobs(self.logits, self.logprobs, tok_ids=self.pred.view(-1), out=(None, self.tok_lp, self.top_ids, self.top_lp))
-                n += 1
+            ops.penalize(self.logits, self.history, self.penalties, self.tp_rank * self.vocab_l)
+        if self.sv:  # row b*T + u at sequence b's counter offsets[b] + depth(u)
+            ops.sample_tokens(self.logits, T, self.temperature, self.top_k, self.top_p, self.seeds, self.offsets, parents,
+                              out=ids)
         elif self.sample and self.tp > 1:  # every rank draws the whole row's id from its shard by exchanging records
             ops.sample_tp(self.logits, self.tp_rank * self.vocab_l, cfg.vocab, self.temperature, self.top_k, self.top_p,
-                          self.seeds, self.offsets, self._gather, self.tp, out=self.next_ids, bufs=self.stp)
-            n += ops._lib.SAMPLE_SHARD_PHASES + 1 + ops._lib.SAMPLE_SHARD_PHASES * (self.collective != "nccl")
-            if self.logprobs:  # the log-probabilities at the drawn ids: the greedy TP step's records, all-gather and merge
-                ops.logprobs_shard(self.logits, self.logprobs, self.tp_rank * self.vocab_l, tok_ids=self.next_ids,
-                                   out=self.loc_rec); n += 1
-                self._gather_records()
-                n += self.collective != "nccl"
-                ops.logprobs_merge(self.all_rec, self.logprobs, out=(None, self.tok_lp, self.top_ids, self.top_lp)); n += 1
-        elif self.sample:  # the drawn ids; with logprobs, the log-probabilities at them (one launch more)
-            ops.sample(self.logits, self.temperature, self.top_k, self.top_p, self.seeds, self.offsets, out=self.next_ids); n += 1
-            if self.logprobs:
-                ops.logprobs(self.logits, self.logprobs, tok_ids=self.next_ids, out=(None, self.tok_lp, self.top_ids, self.top_lp))
-                n += 1
-        elif self.logprobs and self.tp == 1:  # the argmax ids and the log-probabilities in one launch
-            ids = self.pred.view(-1) if T > 1 else self.next_ids
-            ops.logprobs(self.logits, self.logprobs, out=(ids, self.tok_lp, self.top_ids, self.top_lp)); n += 1
-        elif self.logprobs:  # vocab-split: per-rank records, one all-gather of them, the merge
-            ops.logprobs_shard(self.logits, self.logprobs, self.tp_rank * self.vocab_l, out=self.loc_rec); n += 1
-            self._gather_records()
-            n += self.collective != "nccl"
-            ops.logprobs_merge(self.all_rec, self.logprobs, out=(self.next_ids, self.tok_lp, self.top_ids, self.top_lp)); n += 1
-        elif T > 1:
-            ops.argmax(self.logits, out=self.pred.view(-1)); n += 1
-        elif self.tp == 1:
-            ops.argmax(self.logits, out=self.next_ids); n += 1
-        else:  # vocab-split lm_head: local (max, argmax) + B-element all-gather instead of all-reducing 152064 logits
-            ops.argmax_shard(self.logits, self.tp_rank * self.vocab_l, self.loc_ids, self.loc_val); n += 1
-            if self.collective == "nccl":
-                import torch.distributed as dist
-                dist.all_gather_into_tensor(self.all_val, self.loc_val, group=self.tp_group)
-                dist.all_gather_into_tensor(self.all_ids, self.loc_ids, group=self.tp_group)
-            else:
-                self.comm.allgather(self.loc_val, self.all_val); n += 1
-                self.comm.allgather(self.loc_ids, self.all_ids); n += 1
-            ops.argmax_merge(self.all_val, self.all_ids, out=self.next_ids); n += 1  # lowest rank on ties == lowest vocab id
+                          self.seeds, self.offsets, self._gather, self.tp, out=ids, bufs=self.stp)
+        elif self.sample:
+            ops.sample(self.logits, self.temperature, self.top_k, self.top_p, self.seeds, self.offsets, out=ids)
+        if self.logprobs:  # at the drawn ids; greedy, the same launch writes the argmax ids
+            lp = (self.tok_lp, self.top_ids, self.top_lp)
+            tok_ids, out = (ids, (None, *lp)) if drawn else (None, (ids, *lp))
+            if self.tp == 1:
+                ops.logprobs(self.logits, self.logprobs, tok_ids=tok_ids, out=out)
+            else:  # vocab-split: per-rank records, one all-gather of them, the merge
+                ops.logprobs_shard(self.logits, self.logprobs, self.tp_rank * self.vocab_l, tok_ids=tok_ids, out=self.loc_rec)
+                self._gather(self.loc_rec, self.all_rec)
+                ops.logprobs_merge(self.all_rec, self.logprobs, out=out)
+        elif not drawn and self.tp == 1:
+            ops.argmax(self.logits, out=ids)
+        elif not drawn:  # vocab-split lm_head: local (max, argmax) + B-element all-gathers instead of all-reducing the logits
+            ops.argmax_shard(self.logits, self.tp_rank * self.vocab_l, self.loc_ids, self.loc_val)
+            self._gather(self.loc_val, self.all_val)
+            self._gather(self.loc_ids, self.all_ids)
+            ops.argmax_merge(self.all_val, self.all_ids, out=ids)  # lowest rank on ties == lowest vocab id
         if T > 1:  # verification: accepted counts, next token, lengths (and the draw counters) stay on the device
-            ops._spec_accept(self.accepted, self.next_ids, self.lens_old, self.lens_new, self.tokens, self.pred,
-                             self.path if self.tree else None, self.parents if self.tree else None,
-                             self.offsets if self.sv else None); n += 1
+            ops._spec_accept(self.accepted, self.next_ids, self.lens_old, self.lens_new, self.tokens, self.pred, path, parents,
+                             self.offsets if self.sv else None)
             if self.tree:  # the accepted path's rows move to consecutive slots in every layer
-                ops.cache_compact([L["cache"] for L in self.layers], self.lens_old, self.accepted, self.path, T); n += 1
+                ops.cache_compact([L["cache"] for L in self.layers], self.lens_old, self.accepted, path, T)
         else:
-            ops.lens_add(self.lens_old, 1); n += 1
-            ops.lens_add(self.lens_new, 1); n += 1
-        if self.pen:  # the emitted token joins the history
-            self.history.append(self.next_ids); n += 1
-        if self.ngram:  # the step's emitted tokens join the history
-            self.history.append_tokens(self.pred, self.accepted, self.path if self.tree else None); n += 1
-        # rows per launch above 16 rows: 64 on the wgmma path (per-channel int4/int8, bf16 lm_head), 16 for sub-channel
-        # weights (mma.sync path); below, one launch takes all rows
-        hchunks = (R + 63) // 64 if R > 16 else 1
-        qchunks = ((R + 15) // 16 if (self.group_size != -1 and self.wbits != 4) else hchunks) if R > 16 else 1
-        n += (qchunks - 1) * (4 if self.fuse_swiglu else 5) * len(self.layers) + (hchunks - 1)
-        self.launches_per_step = n
+            ops.lens_add(self.lens_old, 1)
+            ops.lens_add(self.lens_new, 1)
+        if self.pen or self.ngram:  # the step's emitted tokens join the history
+            if T == 1:
+                self.history.append(self.next_ids)
+            else:
+                self.history.append_tokens(self.pred, self.accepted, path)
 
-    def _gather_records(self):
-        """all-gather the per-rank logprob records (opaque bytes) of the vocab-split lm_head"""
-        self._gather(self.loc_rec, self.all_rec)
-
-    def _gather(self, rec, all_rec):
-        """all-gather this rank's records (opaque bytes, [rows, bytes]) into all_rec [tp, rows * bytes], in rank order"""
-        if self.collective == "nccl":
-            import torch.distributed as dist
-            dist.all_gather_into_tensor(all_rec.view(-1), rec.view(-1), group=self.tp_group)
-        else:
-            self.comm.allgather(rec, all_rec)
+    def _eager_step(self):
+        """one step run eagerly; launches_per_step := the kernels it launched"""
+        n = _lib.calls
+        self._step_ops()
+        self.launches_per_step = _lib.calls - n
 
     def step(self):
         """q_len 1: returns next_ids [B].  q_len > 1: one verify step, returns (pred [B, T], accepted [B]); the step's
@@ -606,32 +584,25 @@ class DecodeStack:
         if self.graph is not None:
             self.graph.replay()
         else:
-            self._step_ops()
+            self._eager_step()
         if self.tree:
             return self.pred, self.accepted, self.path
         return self.next_ids if self.q_len == 1 else (self.pred, self.accepted)
 
     def capture(self):
-        """Warm up once eagerly (plans, workspace growth), rewind the lengths, then capture one step."""
-        lo, ln = self.lens_old.clone(), self.lens_new.clone()
-        tk = self.tokens.clone() if self.q_len > 1 else None  # the accept kernel rewrites column 0
-        off = self.offsets.clone() if self.sample or self.sv else None  # the warm-up step advances the draw counters
-        hist = self.history.snapshot() if self.pen or self.ngram else None  # ... and appends tokens to the history
-        self._step_ops()
+        """Warm up once eagerly (plans, workspace growth), rewind the state the step carries, then capture one step."""
+        carried = [getattr(self, k) for k in self._carried]
+        saved = [v.snapshot() if isinstance(v, ops.TokenHistory) else v.clone() for v in carried]
+        self._eager_step()
         torch.cuda.synchronize()
-        if hist is not None:
-            self.history.restore(hist)
-        self.lens_old.copy_(lo); self.lens_new.copy_(ln)
-        if tk is not None:
-            self.tokens.copy_(tk)
-        if off is not None:
-            self.offsets.copy_(off)
+        for v, s in zip(carried, saved):
+            if isinstance(v, ops.TokenHistory):
+                v.restore(s)
+            else:
+                v.copy_(s)
         g = torch.cuda.CUDAGraph()
         with torch.cuda.graph(g):
             self._step_ops()
-        self.lens_old.copy_(lo); self.lens_new.copy_(ln)
-        if tk is not None:
-            self.tokens.copy_(tk)
         torch.cuda.synchronize()
         self.graph = g
         return g
@@ -640,27 +611,23 @@ class DecodeStack:
         """Time the decode step's collectives ALONE (TP > 1): the 2 x layers all-reduces of [B, hidden] bf16 + the lm_head
         all-gathers, back to back in one CUDA graph, `reps` replays -> ms per step.  No compute overlaps them here, so
         ms_per_step_alone / step time is an upper bound of the collective's share of the step."""
-        import torch.distributed as dist_
         assert self.tp > 1
         g = torch.cuda.CUDAGraph()
         def ops_():
             for _ in range(2 * len(self.layers)):
                 self._allreduce(self.part)
             if self.logprobs:
-                self._gather_records()
-            elif self.collective == "nccl":
-                dist_.all_gather_into_tensor(self.all_val, self.loc_val, group=self.tp_group)
-                dist_.all_gather_into_tensor(self.all_ids, self.loc_ids, group=self.tp_group)
+                self._gather(self.loc_rec, self.all_rec)
             else:
-                self.comm.allgather(self.loc_val, self.all_val)
-                self.comm.allgather(self.loc_ids, self.all_ids)
+                self._gather(self.loc_val, self.all_val)
+                self._gather(self.loc_ids, self.all_ids)
         ops_()
         torch.cuda.synchronize()
         with torch.cuda.graph(g):
             ops_()
         g.replay()
         torch.cuda.synchronize()
-        dist_.barrier(group=self.tp_group)
+        dist.barrier(group=self.tp_group)
         torch.cuda.synchronize()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
@@ -669,7 +636,7 @@ class DecodeStack:
         e1.record()
         torch.cuda.synchronize()
         t = torch.tensor([e0.elapsed_time(e1) / reps], device=self.device)
-        dist_.all_reduce(t, op=dist_.ReduceOp.MAX, group=self.tp_group)
+        dist.all_reduce(t, op=dist.ReduceOp.MAX, group=self.tp_group)
         return {"ms_per_step_alone": round(float(t.item()), 4), "all_reduces_per_step": 2 * len(self.layers),
                 "bytes_per_all_reduce": self.part.numel() * 2, "impl": self.collective_impl}
 

@@ -88,6 +88,13 @@ class GemmWQ:
     def tc_cluster(self):
         return lib.b2_gemm_wq_tc_cluster(self.h)
 
+    def launches(self, M):
+        """Kernel launches of one call over M rows, as wq_gemm.cu dispatches them: one up to 16 rows; above, one per 64 rows
+        on the wgmma kernel, or one per 16 rows on the mma.sync kernel that sub-channel int8 weights keep."""
+        if M <= 16:
+            return 1
+        return -(-M // (16 if self.wbits == 8 and self.group_size != -1 else 64))
+
     def __call__(self, a, ws, out=None, act=ACT_NONE, alpha=1.0, residual=None, norm_in=None, sumsq_out=None, xg_out=None):
         """Fused RMSNorm (b2_gemm_fuse), two forms:
         M <= 16, self-contained: norm_in = (None, gamma [K], K, eps) — the GEMV normalises its own activations.
@@ -106,7 +113,7 @@ class GemmWQ:
         ldc = out.stride(-2) if out.dim() > 1 else self.N
         if norm_in is None and sumsq_out is None and xg_out is None:
             check(lib.b2_gemm_wq_run(self.h, _ptr(a), lda, _ptr(out), ldc, M, _ptr(self.bias), _ptr(residual), act,
-                                     float(alpha), _ptr(wsb), wsb.numel(), _stream()), "b2_gemm_wq_run")
+                                     float(alpha), _ptr(wsb), wsb.numel(), _stream()), "b2_gemm_wq_run", self.launches(M))
             return out
         f = GemmFuse()
         if norm_in is not None:
@@ -119,7 +126,8 @@ class GemmWQ:
             xg, g_out = xg_out
             f.xg_out, f.gamma_out, f.ldxg = xg.data_ptr(), g_out.data_ptr(), xg.stride(-2) if xg.dim() > 1 else self.N
         check(lib.b2_gemm_wq_run_fused(self.h, _ptr(a), lda, _ptr(out), ldc, M, _ptr(self.bias), _ptr(residual), act,
-                                       float(alpha), _ptr(wsb), wsb.numel(), C.byref(f), _stream()), "b2_gemm_wq_run_fused")
+                                       float(alpha), _ptr(wsb), wsb.numel(), C.byref(f), _stream()), "b2_gemm_wq_run_fused",
+              self.launches(M))
         return out
 
     def run_fp8(self, q8, ws, out=None, act=ACT_NONE, alpha=1.0, residual=None):
@@ -749,14 +757,22 @@ def sample_shard_merge(all_records, state, offsets, out=None):
     return out
 
 
+class _SampleTPBuffers(dict):
+    def view(self, rows):
+        """the buffers of the first `rows` rows, sharing the storage (DecodeStack.set_batch)"""
+        n = self["state"].shape[0]
+        return _SampleTPBuffers(state=self["state"][:rows], rec=[r[:rows] for r in self["rec"]],
+                                all=[a.view(-1)[:a.numel() // n * rows].view(a.shape[0], -1) for a in self["all"]])
+
+
 def sample_tp_buffers(rows, nranks, device="cuda"):
     """The buffers of sample_tp() for `rows` rows and `nranks` ranks: this rank's state, each phase's own records and
-    their all-gathered form ([nranks, rows * bytes], the layout an all-gather writes)."""
+    their all-gathered form ([nranks, rows * bytes], the layout an all-gather writes).  view(r) gives the first r rows'."""
     P = _lib.SAMPLE_SHARD_PHASES
     u8 = dict(dtype=torch.uint8, device=device)
-    return {"state": torch.empty(rows, sample_shard_state_bytes(), **u8),
-            "rec": [torch.empty(rows, sample_shard_record_bytes(p), **u8) for p in range(P)],
-            "all": [torch.empty(nranks, rows * sample_shard_record_bytes(p), **u8) for p in range(P)]}
+    return _SampleTPBuffers(state=torch.empty(rows, sample_shard_state_bytes(), **u8),
+                            rec=[torch.empty(rows, sample_shard_record_bytes(p), **u8) for p in range(P)],
+                            all=[torch.empty(nranks, rows * sample_shard_record_bytes(p), **u8) for p in range(P)])
 
 
 def sample_tp(logits_shard, id_offset, n_total, temperature, top_k, top_p, seeds, offsets, exchange, nranks, out=None,

@@ -1,6 +1,7 @@
 """GPU, 2 devices: DecodeStack(tp_size=2, sample=True).  Each rank's ids must equal b2_sample applied to the
 concatenation of the ranks' logits shards at the same offsets, every rank's offsets must match, and the step must run the
-greedy TP step's launches plus the number its docstring states.  Skipped on a machine with one GPU."""
+greedy TP step's launches plus the number its docstring states; with collective "b2" both stacks' launch counts equal the
+kernel nodes of a captured step.  Skipped on a machine with one GPU."""
 import os
 import socket
 
@@ -63,7 +64,12 @@ def _worker(rank, world, port, ret, collective, logprobs, penalties, graph):
         st.comm.check_error()
     extra = {"nccl": 5, "b2": 9, "fused": 9}[collective] + (4 if logprobs else 0) * (collective != "nccl") + \
         (2 if logprobs else 0) * (collective == "nccl")
-    ret[rank] = (ok, msgs, st.launches_per_step, greedy.launches_per_step, extra)
+    recorded = []  # (kernel nodes of a captured step, launches_per_step), sampled and greedy
+    if collective == "b2":  # every exchange is a library kernel, so the graph holds exactly the counted launches
+        sys.path.insert(0, os.path.join(root, "tests"))
+        from test_stack_launches_gpu import graph_kernels, recorded_step
+        recorded = [(len(graph_kernels(recorded_step(s))), s.launches_per_step) for s in (st, greedy)]
+    ret[rank] = (ok, msgs, st.launches_per_step, greedy.launches_per_step, extra, recorded)
     dist.barrier()
     os._exit(0)  # graphs hold captured collectives: leave without tearing the communicators down
 
@@ -85,6 +91,7 @@ def test_tp2_sample_matches_whole_row_draw(collective, logprobs, penalties, grap
         p.join(300)
         assert p.exitcode == 0
     for r in range(2):
-        ok, msgs, n_sample, n_greedy, extra = ret[r]
+        ok, msgs, n_sample, n_greedy, extra, recorded = ret[r]
         assert ok, msgs
         assert n_sample == n_greedy + extra, (n_sample, n_greedy, extra)
+        assert all(nodes == n for nodes, n in recorded), recorded
