@@ -40,9 +40,15 @@ inline auto with_kv_mode(int qm, F&& f) {
   return f(std::integral_constant<int, B2_KV_U4>{});
 }
 
+// A rotary's pairing style (b2_rope_cfg.style): B2_ROPE_NEOX or B2_ROPE_INTERLEAVED, else B2_ERR_PARAM.  NULL rope passes.
+inline int rope_style_check(const b2_rope_cfg* rope) {
+  return rope && rope->style != B2_ROPE_NEOX && rope->style != B2_ROPE_INTERLEAVED ? B2_ERR_PARAM : B2_OK;
+}
+
 // The argument checks of a scaled-rotary table (b2_rope_table), shared by b2_rotary_table and the table form of the append.
 inline int rope_table_check(const b2_rope_cfg* rope, const b2_rope_table* t) {
   if (!rope || !t || !t->inv_freq || t->stride < 0) return B2_ERR_PARAM;
+  if (int st = rope_style_check(rope)) return st;
   if (rope->rotary_dim != 128 && rope->rotary_dim != 64) return B2_ERR_UNSUPPORTED;
   if (t->stride != 0 && t->stride < rope->rotary_dim / 2) return B2_ERR_PARAM;
   if (((uintptr_t)t->inv_freq & 15) || (t->stride & 3)) return B2_ERR_UNSUPPORTED;  // whole-vector loads of 4 frequencies
@@ -347,27 +353,58 @@ __device__ __forceinline__ void head_rmsnorm(float (&x)[4], const __nv_bfloat16*
   for (int i = 0; i < 4; ++i) x[i] = F::to_f(F::from_f((x[i] * rs) * gv[i]));
 }
 
-// ---- NeoX rotary of one 128-wide q or k head row held 4 consecutive values per lane, with the inverse frequencies read
-// from a caller-given table row (b2_rope_table; the stand-alone b2_rotary_table and the table form of the span-cache append
-// both call this, so they cannot drift apart).  For d = 4 lane + i < rotary_dim, f = d % half:
+// ---- rotary pairing (b2_rope_cfg.style) of one 128-wide q or k head row held 4 consecutive values per lane: the partner of
+// each of the lane's dims d = 4 lane + i, with half = rotary_dim / 2.  NeoX: d ^ half, in lane ^ (half / 4) (a shuffle; the
+// whole warp calls it).
+// Interleaved: d ^ 1, the neighbouring value in the same lane (no shuffle).
+template <int RS>
+__device__ __forceinline__ void rope_partners(const float (&x)[4], float (&other)[4], int half) {
+  if constexpr (RS == B2_ROPE_NEOX) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) other[i] = __shfl_xor_sync(0xffffffffu, x[i], half == 64 ? 16 : 8);
+  } else {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) other[i] = x[i ^ 1];
+  }
+}
+
+// One element of the computed-frequency rotary (b2_rope_cfg), before the FT rounding: frequency index fi, `first` selects the
+// "first half" expression.  Both pairing styles call it, so they run the same instructions on the same operands.
+__device__ __forceinline__ float rope_rotate(float x, float other, int fi, bool first, int pos, float log2_base, int rotary_dim) {
+  const float inv = exp2f(-log2_base * (2.0f * fi / (float)rotary_dim));
+  float sn, cs;
+  sincosf((float)pos * inv, &sn, &cs);
+  return first ? x * cs - other * sn : x * cs + other * sn;
+}
+
+// ---- rotary of one 128-wide q or k head row held 4 consecutive values per lane, with the inverse frequencies read from a
+// caller-given table row (b2_rope_table; the stand-alone b2_rotary_table and the table form of the span-cache append both
+// call this, so they cannot drift apart).  For d = 4 lane + i < rotary_dim, f = d % half (NeoX) or d / 2 (interleaved):
 //   ang = fl32(pos * inv[f]);  sincosf;  c = fl32(cs * af);  s = fl32(sn * af);
 //   x[i] <- FT(fma(x[i], c, -+fl32(partner * s))), one FT rounding (returned widened); dims >= rotary_dim keep x.
-// The whole warp calls it (it shuffles); rotary_dim is 128 or 64.  inv: 16-byte aligned, so a lane's 4 frequencies
-// (f = 4 lane % half ... + 3) are one vector load.  The products are written as intrinsics so that no FMA contraction can
-// differ between the two callers.
-template <bool H>
+// The whole warp calls it (NeoX shuffles); rotary_dim is 128 or 64.  inv: 16-byte aligned, so a lane's frequencies are one
+// vector load (NeoX: f = 4 lane % half ... + 3; interleaved: f = 2 lane, 2 lane + 1).  The products are written as
+// intrinsics so that no FMA contraction can differ between the two callers or the two styles.
+template <bool H, int RS = B2_ROPE_NEOX>
 __device__ __forceinline__ void rope_from_table(float (&x)[4], int pos, const float* inv, float af, int rotary_dim, int lane) {
   using F = Ft<H>;
   const int half = rotary_dim >> 1;
   float other[4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i) other[i] = __shfl_xor_sync(0xffffffffu, x[i], half == 64 ? 16 : 8);
+  rope_partners<RS>(x, other, half);
   if (lane * 4 >= rotary_dim) return;
-  const float4 fr = *reinterpret_cast<const float4*>(inv + ((lane * 4) & (half - 1)));
-  const float fv[4] = {fr.x, fr.y, fr.z, fr.w};
-  const bool lower = lane * 4 < half;  // the same for the lane's 4 dims: half is a multiple of 4
+  float fv[4];
+  if constexpr (RS == B2_ROPE_NEOX) {
+    const float4 fr = *reinterpret_cast<const float4*>(inv + ((lane * 4) & (half - 1)));
+    fv[0] = fr.x; fv[1] = fr.y; fv[2] = fr.z; fv[3] = fr.w;
+  } else {
+    const float2 fr = *reinterpret_cast<const float2*>(inv + lane * 2);
+    fv[0] = fv[1] = fr.x;
+    fv[2] = fv[3] = fr.y;
+  }
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
+    // NeoX: the same for the lane's 4 dims (half is a multiple of 4); interleaved: the even dims
+    const bool lower = RS == B2_ROPE_NEOX ? lane * 4 < half : (i & 1) == 0;
     float sn, cs;
     sincosf(__fmul_rn((float)pos, fv[i]), &sn, &cs);
     const float c = __fmul_rn(cs, af), s = __fmul_rn(sn, af);

@@ -148,9 +148,10 @@ __global__ void __launch_bounds__(256) quant_fp8_kernel(uint8_t* __restrict__ y,
   }
 }
 
-// in-place NeoX rotary on the q and k heads: one warp per (sequence, head)
-__global__ void __launch_bounds__(128) rotary_kernel(__nv_bfloat16* __restrict__ qkv, const int32_t* __restrict__ pos, int batch,
-                                                     int n_heads, int n_groups, int rotary_dim, float log2_base) {
+// in-place rotary on the q and k heads: one warp per (sequence, head); RS: the pairing style (b2_rope_cfg.style)
+template <int RS>
+__device__ __forceinline__ void rotary_row(__nv_bfloat16* __restrict__ qkv, const int32_t* __restrict__ pos, int batch,
+                                           int n_heads, int n_groups, int rotary_dim, float log2_base) {
   pdl_wait();
   pdl_launch_dependents();
   const int lane = threadIdx.x & 31;
@@ -164,29 +165,36 @@ __global__ void __launch_bounds__(128) rotary_kernel(__nv_bfloat16* __restrict__
   float x[4] = {bf16_lo(raw.x), bf16_hi(raw.x), bf16_lo(raw.y), bf16_hi(raw.y)};
   const int half = rotary_dim >> 1;
   float other[4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i) other[i] = __shfl_xor_sync(0xffffffffu, x[i], half == 64 ? 16 : 8);
+  rope_partners<RS>(x, other, half);
   const int ps = pos[b];
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
     const int d = lane * 4 + i;
     if (d < rotary_dim) {
-      const int fi = d % half;
-      const float inv = exp2f(-log2_base * (2.0f * fi / (float)rotary_dim));
-      float sn, cs;
-      sincosf((float)ps * inv, &sn, &cs);
-      x[i] = d < half ? x[i] * cs - other[i] * sn : x[i] * cs + other[i] * sn;
+      const int fi = RS == B2_ROPE_NEOX ? d % half : d >> 1;
+      const bool first = RS == B2_ROPE_NEOX ? d < half : (d & 1) == 0;
+      x[i] = rope_rotate(x[i], other[i], fi, first, ps, log2_base, rotary_dim);
     }
   }
   *reinterpret_cast<uint2*>(ptr) = make_uint2(pack_bf16x2(x[0], x[1]), pack_bf16x2(x[2], x[3]));
 }
 
-// in-place NeoX rotary from a caller-given frequency table (b2_rotary_table): one warp per (row, q or k head); row b reads
+__global__ void __launch_bounds__(128) rotary_kernel(__nv_bfloat16* __restrict__ qkv, const int32_t* __restrict__ pos, int batch,
+                                                     int n_heads, int n_groups, int rotary_dim, float log2_base) {
+  rotary_row<B2_ROPE_NEOX>(qkv, pos, batch, n_heads, n_groups, rotary_dim, log2_base);
+}
+
+__global__ void __launch_bounds__(128) rotary_il_kernel(__nv_bfloat16* __restrict__ qkv, const int32_t* __restrict__ pos,
+                                                        int batch, int n_heads, int n_groups, int rotary_dim, float log2_base) {
+  rotary_row<B2_ROPE_INTERLEAVED>(qkv, pos, batch, n_heads, n_groups, rotary_dim, log2_base);
+}
+
+// in-place rotary from a caller-given frequency table (b2_rotary_table): one warp per (row, q or k head); row b reads
 // the table row inv + b * stride (rope_from_table)
-template <bool H>
-__global__ void __launch_bounds__(128) rotary_table_kernel(__nv_bfloat16* __restrict__ qkv, const int32_t* __restrict__ pos,
-                                                           int batch, int n_heads, int n_groups, int rotary_dim,
-                                                           const float* __restrict__ inv, int64_t stride, float af) {
+template <bool H, int RS>
+__device__ __forceinline__ void rotary_table_row(__nv_bfloat16* __restrict__ qkv, const int32_t* __restrict__ pos, int batch,
+                                                 int n_heads, int n_groups, int rotary_dim, const float* __restrict__ inv,
+                                                 int64_t stride, float af) {
   using F = Ft<H>;
   pdl_wait();
   pdl_launch_dependents();
@@ -199,8 +207,22 @@ __global__ void __launch_bounds__(128) rotary_table_kernel(__nv_bfloat16* __rest
   __nv_bfloat16* ptr = qkv + ((size_t)b * slots + h) * 128 + lane * 4;
   const uint2 raw = *reinterpret_cast<const uint2*>(ptr);
   float x[4] = {F::lo(raw.x), F::hi(raw.x), F::lo(raw.y), F::hi(raw.y)};
-  rope_from_table<H>(x, pos[b], inv + (size_t)b * stride, af, rotary_dim, lane);
+  rope_from_table<H, RS>(x, pos[b], inv + (size_t)b * stride, af, rotary_dim, lane);
   *reinterpret_cast<uint2*>(ptr) = make_uint2(F::pack(x[0], x[1]), F::pack(x[2], x[3]));
+}
+
+template <bool H>
+__global__ void __launch_bounds__(128) rotary_table_kernel(__nv_bfloat16* __restrict__ qkv, const int32_t* __restrict__ pos,
+                                                           int batch, int n_heads, int n_groups, int rotary_dim,
+                                                           const float* __restrict__ inv, int64_t stride, float af) {
+  rotary_table_row<H, B2_ROPE_NEOX>(qkv, pos, batch, n_heads, n_groups, rotary_dim, inv, stride, af);
+}
+
+template <bool H>
+__global__ void __launch_bounds__(128) rotary_table_il_kernel(__nv_bfloat16* __restrict__ qkv, const int32_t* __restrict__ pos,
+                                                              int batch, int n_heads, int n_groups, int rotary_dim,
+                                                              const float* __restrict__ inv, int64_t stride, float af) {
+  rotary_table_row<H, B2_ROPE_INTERLEAVED>(qkv, pos, batch, n_heads, n_groups, rotary_dim, inv, stride, af);
 }
 
 // QKLayerNormNoBeta (b2_qk_rmsnorm): one warp per (row, head) of x [rows, ld]; heads [0, n_heads) normalised with q_gamma,
@@ -429,9 +451,11 @@ int b2_quant_fp8(void* y, int64_t ldy, float* scale, float* tile_sums, const voi
 int b2_rotary(void* qkv, const int32_t* pos, int batch, int n_heads, int n_groups, int head_size, const b2_rope_cfg* rope,
               void* stream) {
   if (!qkv || !pos || !rope || batch <= 0) return B2_ERR_PARAM;
+  if (int st = rope_style_check(rope)) return st;
   if (head_size != 128 || (rope->rotary_dim != 128 && rope->rotary_dim != 64) || !aligned(qkv, 8)) return B2_ERR_UNSUPPORTED;
   const int warps = batch * (n_heads + n_groups);
-  B2_LAUNCH_CHECK("rotary", launch(rotary_kernel, dim3((warps + 3) / 4), dim3(128), 0, (cudaStream_t)stream, true,
+  const auto kern = rope->style == B2_ROPE_INTERLEAVED ? rotary_il_kernel : rotary_kernel;
+  B2_LAUNCH_CHECK("rotary", launch(kern, dim3((warps + 3) / 4), dim3(128), 0, (cudaStream_t)stream, true,
                                    (__nv_bfloat16*)qkv, pos, batch, n_heads, n_groups, rope->rotary_dim, log2f(rope->base)));
   return B2_OK;
 }
@@ -442,7 +466,9 @@ int b2_rotary_table(void* qkv, const int32_t* pos, int batch, int n_heads, int n
   if (int st = rope_table_check(rope, table)) return st;
   if (head_size != 128 || (ft != B2_DT_BF16 && ft != B2_DT_F16) || !aligned(qkv, 8)) return B2_ERR_UNSUPPORTED;
   const int warps = batch * (n_heads + n_groups);
-  const auto kern = ft == B2_DT_F16 ? rotary_table_kernel<true> : rotary_table_kernel<false>;
+  const bool il = rope->style == B2_ROPE_INTERLEAVED;
+  const auto kern = ft == B2_DT_F16 ? (il ? rotary_table_il_kernel<true> : rotary_table_kernel<true>)
+                                    : (il ? rotary_table_il_kernel<false> : rotary_table_kernel<false>);
   B2_LAUNCH_CHECK("rotary_table", launch(kern, dim3((warps + 3) / 4), dim3(128), 0, (cudaStream_t)stream, true, (__nv_bfloat16*)qkv,
                                          pos, batch, n_heads, n_groups, rope->rotary_dim, table->inv_freq, table->stride,
                                          table->attn_factor));

@@ -1111,7 +1111,8 @@ __device__ __forceinline__ void append_row(const AppendParams& p, int row, int& 
 // QKN: each q and k head row is first normalised (head_rmsnorm with q_gamma / k_gamma) and rounded to FT, like the
 // reference's QKLayerNormNoBeta writes an FT tensor for its Rotary; V rows are not.
 // TAB: the rotary reads its frequencies from the caller's table (rope_from_table, always on) instead of computing them.
-template <int QM, bool H, bool MT, bool TREE, bool QKN, bool TAB, typename P>
+// RS: the rotary's pairing style (b2_rope_cfg.style).
+template <int QM, bool H, bool MT, bool TREE, bool QKN, bool TAB, int RS = B2_ROPE_NEOX, typename P>
 __device__ __forceinline__ void cache_append_warp(const P& p) {
   using F = Ft<H>;
   pdl_wait();
@@ -1132,24 +1133,22 @@ __device__ __forceinline__ void cache_append_warp(const P& p) {
   }
 
   if constexpr (TAB) {
-    if (!is_v) rope_from_table<H>(x, pos, p.inv_freq + (size_t)b * p.table_stride, p.attn_factor, p.rotary_dim, lane);
+    if (!is_v) rope_from_table<H, RS>(x, pos, p.inv_freq + (size_t)b * p.table_stride, p.attn_factor, p.rotary_dim, lane);
   } else if (p.rope && !is_v) {
-    // NeoX rotate-half over the first rotary_dim dims: out[i] = x[i]cos - x[i+h]sin ; out[i+h] = x[i+h]cos + x[i]sin
+    // NeoX rotate-half over the first rotary_dim dims: out[i] = x[i]cos - x[i+h]sin ; out[i+h] = x[i+h]cos + x[i]sin.
+    // Interleaved: out[2j] = x[2j]cos - x[2j+1]sin ; out[2j+1] = x[2j+1]cos + x[2j]sin, frequency j.
     const int half = p.rotary_dim >> 1;
     float other[4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) other[i] = __shfl_xor_sync(0xffffffffu, x[i], half == 64 ? 16 : 8);
+    rope_partners<RS>(x, other, half);
     if (half == 64 || half == 32) {
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
         const int d = lane * 4 + i;
         if (d < p.rotary_dim) {
-          const int fi = d % half;
-          const float inv = exp2f(-p.log2_base * (2.0f * fi / (float)p.rotary_dim));
-          float sn, cs;
-          sincosf((float)pos * inv, &sn, &cs);
+          const int fi = RS == B2_ROPE_NEOX ? d % half : d >> 1;
+          const bool first = RS == B2_ROPE_NEOX ? d < half : (d & 1) == 0;
           // round to bf16 like the reference's Rotary op output (it feeds the cache through an FT tensor)
-          x[i] = F::to_f(F::from_f(d < half ? x[i] * cs - other[i] * sn : x[i] * cs + other[i] * sn));
+          x[i] = F::to_f(F::from_f(rope_rotate(x[i], other[i], fi, first, pos, p.log2_base, p.rotary_dim)));
         }
       }
     }
@@ -1176,6 +1175,17 @@ __global__ void __launch_bounds__(128) cache_append_kernel(const AppendArgs<QKN>
 template <int QM, bool H, bool MT, bool TREE, bool QKN>
 __global__ void __launch_bounds__(128) cache_append_table_kernel(const AppendTableParams p) {
   cache_append_warp<QM, H, MT, TREE, QKN, true>(p);
+}
+
+// the same two kernels with the interleaved pairing (B2_ROPE_INTERLEAVED); the NeoX kernels above keep their code
+template <int QM, bool H, bool MT, bool TREE, bool QKN>
+__global__ void __launch_bounds__(128) cache_append_il_kernel(const AppendArgs<QKN> p) {
+  cache_append_warp<QM, H, MT, TREE, QKN, false, B2_ROPE_INTERLEAVED>(p);
+}
+
+template <int QM, bool H, bool MT, bool TREE, bool QKN>
+__global__ void __launch_bounds__(128) cache_append_table_il_kernel(const AppendTableParams p) {
+  cache_append_warp<QM, H, MT, TREE, QKN, true, B2_ROPE_INTERLEAVED>(p);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1513,7 +1523,9 @@ static int cache_append_launch(const b2_span_cfg* cfg, void* const* k_spans, voi
                                const int32_t* old_lens, const int32_t* parents, int form, int batch, int q_len,
                                const b2_rope_cfg* rope, void* stream_, const b2_qk_norm* norm = nullptr,
                                const b2_rope_table* table = nullptr) {
+  if (int st = rope_style_check(rope)) return st;
   if (rope && (rope->rotary_dim != 128 && rope->rotary_dim != 64)) return B2_ERR_UNSUPPORTED;
+  const bool il = rope && rope->style == B2_ROPE_INTERLEAVED;
   AppendTableParams p;  // each kernel takes the base it needs (AppendArgs)
   p.inv_freq = table ? table->inv_freq : nullptr;
   p.table_stride = table ? table->stride : 0;
@@ -1536,6 +1548,10 @@ static int cache_append_launch(const b2_span_cfg* cfg, void* const* k_spans, voi
     return with_flag(cfg->ft == B2_DT_F16, [&](auto H) {
       return with_step_form(form, [&](auto MT, auto TREE) {
         return with_flag(norm != nullptr, [&](auto QKN) {
+          if (il) {
+            if (table) return launch(cache_append_table_il_kernel<QM, H, MT, TREE, QKN>, grid, block, 0, (cudaStream_t)stream_, true, p);
+            return launch(cache_append_il_kernel<QM, H, MT, TREE, QKN>, grid, block, 0, (cudaStream_t)stream_, true, p);
+          }
           if (table) return launch(cache_append_table_kernel<QM, H, MT, TREE, QKN>, grid, block, 0, (cudaStream_t)stream_, true, p);
           return launch(cache_append_kernel<QM, H, MT, TREE, QKN>, grid, block, 0, (cudaStream_t)stream_, true, p);
         });
@@ -1554,6 +1570,8 @@ extern "C" {
 int b2_span_cache_append(const b2_span_cfg* cfg, void* const* k_spans, void* const* v_spans, void* q_out,
                          const void* qkv, const int32_t* old_lens, int batch, const b2_rope_cfg* rope, void* stream_) {
   if (int st = append_check(cfg, k_spans && v_spans && q_out && qkv && old_lens && batch > 0, 0, 1)) return st;
+  if (int st = rope_style_check(rope)) return st;
+  if (cfg->head_size == 64 && rope && rope->style != B2_ROPE_NEOX) return B2_ERR_UNSUPPORTED;  // span_attn64.cu: NeoX only
   if (cfg->head_size == 64) return span_append64_run(cfg, k_spans, v_spans, q_out, qkv, old_lens, batch, rope, (cudaStream_t)stream_);
   return cache_append_launch(cfg, k_spans, v_spans, q_out, qkv, old_lens, nullptr, 0, batch, 1, rope, stream_);
 }

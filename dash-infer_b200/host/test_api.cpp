@@ -8,6 +8,7 @@
 #include "allreduce_op.h"
 #include "gemm_lowp_gpu.h"
 #include "qk_layernorm_op.h"
+#include "rotary_mulquery_op.h"
 #include "span_attn_op_cuda.h"
 
 using namespace allspark;
@@ -265,6 +266,54 @@ int as_test_qk_layernorm(int nranks, int batch, int num_heads, int groups, int h
     return cudaGetLastError() == cudaSuccess ? 0 : -3;
   } catch (const std::exception& e) {
     AS_LOG_ERROR("as_test_qk_layernorm: %s", e.what());
+    return -1;
+  }
+}
+
+// RotaryMulQuery with the attributes of the reference's GLM converter (head counts of the whole model, one rank) on x_host
+// [batch][(num_heads + 2 groups) * head_dim] in the test dtype at positions pos_host[b] (gen_ctx->step); out_host receives the
+// rotated rows.  Returns the AsStatus of the first step that fails (Init refuses unsupported rotary / invfreq types).
+int as_test_rotary_mulquery(int batch, int num_heads, int groups, int hidden_size, int rotary_type, int invfreq_type,
+                            float rope_ratio, float rotary_base, const int* pos_host, const void* x_host, void* out_host) {
+  try {
+    CUDAContext ctx;
+    ctx.SetDtype(g_test_ft);
+    const int head_dim = hidden_size / num_heads;
+    const int64_t W = (int64_t)(num_heads + 2 * groups) * head_dim;
+    TensorMap tensors, weights, weights_buffer;
+    auto t = std::make_shared<AsTensor>("qkv", DeviceType::CUDA, g_test_ft, DataMode::DENSE, Shape{batch, 1, W});
+    t->CopyDataFrom(x_host, t->GetSizeInByte(), DeviceType::CPU);
+    tensors["qkv"] = t;
+    RuntimeContext rt(false);
+    for (int b = 0; b < batch; ++b) {
+      auto g = std::make_unique<GenerateContext>();
+      g->step = pos_host[b];
+      rt.PushBackGenCtx(std::move(g));
+    }
+    OperatorProto proto;
+    proto.op_type_ = "RotaryMulQuery"; proto.op_name_ = "decoder.layer.0.rotary";
+    proto.inputs_.push_back({"qkv"}); proto.outputs_.push_back({"qkv_rotary"});
+    proto.SetAttr<int>("num_heads", num_heads);
+    proto.SetAttr<int>("multi_query_group_num", groups);
+    proto.SetAttr<int>("hidden_size", hidden_size);
+    proto.SetAttr<int>("rotary_type", rotary_type);
+    proto.SetAttr<int>("invfreq_type", invfreq_type);
+    proto.SetAttr<float>("rope_ratio", rope_ratio);
+    proto.SetAttr<float>("rotary_base", rotary_base);
+    auto op = OpFactory::getInstance().GetOperator({"RotaryMulQuery", DeviceType::CUDA})();
+    AsStatus st = op->InitV2(proto, ctx, weights, weights_buffer, &tensors, &rt);
+    if (st != AsStatus::ALLSPARK_SUCCESS) return (int)st;
+    st = op->CallReshape(&rt);
+    if (st != AsStatus::ALLSPARK_SUCCESS) return (int)st;
+    st = op->CallForward(&rt);
+    if (st != AsStatus::ALLSPARK_SUCCESS) return (int)st;
+    ctx.Synchronize();
+    auto out = tensors["qkv_rotary"];
+    if (out->GetShape().Count() != (int64_t)batch * W) return -2;
+    out->CopyDataTo(out_host, out->GetSizeInByte(), DeviceType::CPU);
+    return cudaGetLastError() == cudaSuccess ? 0 : -3;
+  } catch (const std::exception& e) {
+    AS_LOG_ERROR("as_test_rotary_mulquery: %s", e.what());
     return -1;
   }
 }

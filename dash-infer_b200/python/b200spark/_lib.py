@@ -48,7 +48,7 @@ class GemmFuse(C.Structure):
 
 
 class RopeCfg(C.Structure):
-    _fields_ = [("base", C.c_float), ("rotary_dim", C.c_int32), ("reserved", C.c_int32)]
+    _fields_ = [("base", C.c_float), ("rotary_dim", C.c_int32), ("style", C.c_int32)]
 
 
 class QkNorm(C.Structure):
@@ -76,6 +76,7 @@ ACT_SWIGLU = 100
 BIN_ADD, BIN_MUL = 1, 2
 KV_NONE, KV_I8, KV_U4 = 0, 1, 2
 KV_FP8 = 3  # extension (not a span::QuantMode value): fp8-e4m3 KV cache, head 128 only
+ROPE_NEOX, ROPE_INTERLEAVED = 0, 1  # b2_rope_cfg.style: rotate-half pairs (d, d + rotary_dim / 2), or (2i, 2i + 1)
 COMM_HANDLE_BYTES = 64
 MAX_TOP_LOGPROBS = 10  # B2_MAX_TOP_LOGPROBS
 SAMPLE_MAX_N = 262144  # B2_SAMPLE_MAX_N

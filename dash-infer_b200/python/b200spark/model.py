@@ -37,6 +37,10 @@ class ModelConfig:
     # a Hugging Face rope_scaling entry (ops.rope_table: linear, yarn, llama3), applied statically: one frequency table for
     # every position and sequence; None: the unscaled rotary (rope_base^(-2f / head)).  Head 128 only.
     rope_scaling: dict | None = None
+    # the rotary covers the first rotary_dim dims of each q and k head (None: the whole head; GLM: half of it), paired NeoX
+    # rotate-half ("neox": d with d + rotary_dim / 2) or GPT-J / ChatGLM style ("interleaved": 2i with 2i + 1, head 128 only)
+    rotary_dim: int | None = None
+    rope_style: str = "neox"
 
 
 QWEN2_7B = ModelConfig("Qwen2-7B", 3584, 28, 4, 18944, 28, 152064)
@@ -55,6 +59,13 @@ QWEN25_7B = ModelConfig("Qwen2.5-7B", 3584, 28, 4, 18944, 28, 152064, rope_scali
 LLAMA31_8B = ModelConfig("Llama-3.1-8B", 4096, 32, 8, 14336, 32, 128256, rope_base=5e5, eps=1e-5, qkv_bias=False,
                          rope_scaling={"rope_type": "llama3", "factor": 8.0, "low_freq_factor": 1.0, "high_freq_factor": 4.0,
                                        "original_max_position_embeddings": 8192})
+# GLM-4 / ChatGLM3 (shapes of the published config.json files): 2 kv heads, QKV bias, the interleaved rotary over half of
+# each head.  The -chat long-context variants only raise rope_ratio, which multiplies the base: GLM-4-9B-chat's 500 is
+# dataclasses.replace(GLM4_9B, rope_base=1e4 * 500).
+GLM4_9B = ModelConfig("GLM-4-9B", 4096, 32, 2, 13696, 40, 151552, rope_base=1e4, eps=1.5625e-7, qkv_bias=True, rotary_dim=64,
+                      rope_style="interleaved")
+CHATGLM3_6B = ModelConfig("ChatGLM3-6B", 4096, 32, 2, 13696, 28, 65024, rope_base=1e4, eps=1e-5, qkv_bias=True, rotary_dim=64,
+                          rope_style="interleaved")
 
 KV_MODES = {"none": KV_NONE, "bf16": KV_NONE, "i8": KV_I8, "u4": KV_U4, "fp8": KV_FP8}
 
@@ -200,6 +211,8 @@ class DecodeStack:
         assert not tree or (q_len > 1 and tp_size == 1 and cfg.head == 128), "draft trees: q_len > 1, single GPU, head size 128"
         assert not cfg.qk_norm or cfg.head == 128, "per-head Q/K norm: head size 128"
         assert cfg.rope_scaling is None or cfg.head == 128, "rope scaling: head size 128"
+        assert cfg.rope_style in ops.ROPE_STYLES, "rope_style: 'neox' or 'interleaved'"
+        assert cfg.rope_style == "neox" or cfg.head == 128, "interleaved rotary: head size 128 (the head-64 append is NeoX only)"
         assert 0 <= logprobs <= ops._lib.MAX_TOP_LOGPROBS, "logprobs: 0 .. 10 alternatives"
         assert not sample or q_len == 1, "sample=True: single-token steps (q_len == 1); sampled verify steps: sampled_verify=True"
         assert not sampled_verify or (q_len > 1 and tp_size == 1 and not sample and not penalties), \
@@ -278,8 +291,12 @@ class DecodeStack:
         self.attn = ops.SpanAttn(self.layers[0]["cache"].cfg, rows)
         self.ws = ops.Workspace(device)
         # rope scaling: one fp32 frequency table on the device, shared by every layer and sequence (every TP rank builds the
-        # same one); without it the append computes base^(-2f / head) itself, as before
-        self.rope = (cfg.rope_base, hd) if cfg.rope_scaling is None else ops.rope_table(cfg.rope_scaling, cfg.rope_base, hd, device)
+        # same one); without it the append computes base^(-2f / rotary_dim) itself, as before.  A pairing other than NeoX
+        # rides as a third element, in both forms.
+        rd = cfg.rotary_dim or hd
+        self.rope = (cfg.rope_base, rd) if cfg.rope_scaling is None else ops.rope_table(cfg.rope_scaling, cfg.rope_base, rd, device)
+        if cfg.rope_style != "neox":
+            self.rope = tuple(self.rope) + (cfg.rope_style,)
         rec = ops.logprobs_partial_bytes(logprobs) if logprobs else 0  # bytes of one row's logprob record (TP > 1)
         if tp > 1 and self.collective != "nccl" and self.comm is None:  # the largest exchange: activations, or a record
             rec_max = max(rec, ops.sample_shard_record_bytes(1) if sample else 0)

@@ -8,7 +8,7 @@ import torch
 
 from . import _lib
 from ._lib import (ACT_NONE, BIN_ADD, BIN_MUL, DT_BF16, DT_I8, DT_U8, KV_I8, KV_NONE, KV_U4, GemmDesc, GemmFuse, PenaltyParams,
-                   QkNorm, RopeCfg, RopeTable, SpanCfg, check, lib)
+                   ROPE_INTERLEAVED, ROPE_NEOX, QkNorm, RopeCfg, RopeTable, SpanCfg, check, lib)
 
 
 def _stream():
@@ -341,10 +341,21 @@ def rope_table(scaling, base, rotary_dim, device=None):
     return (inv.to(device) if device is not None else inv), float(af)
 
 
+ROPE_STYLES = {"neox": ROPE_NEOX, "interleaved": ROPE_INTERLEAVED}
+
+
+def rope_style(style):
+    """b2_rope_cfg.style of "neox" / "interleaved" or of the int itself (ROPE_NEOX, ROPE_INTERLEAVED; others are passed on
+    for the library to refuse)"""
+    return ROPE_STYLES[style] if isinstance(style, str) else int(style)
+
+
 def _rope_table(rope, rows, device):
-    """(inv_freq, attn_factor) -> (RopeCfg, RopeTable): inv_freq fp32 [rotary_dim / 2] (one row shared by every sequence) or
-    [rows, >= rotary_dim / 2] (row b for sequence b, stride inv_freq.stride(0)) on the activations' device"""
-    inv, af = rope
+    """(inv_freq, attn_factor[, style]) -> (RopeCfg, RopeTable): inv_freq fp32 [rotary_dim / 2] (one row shared by every
+    sequence) or [rows, >= rotary_dim / 2] (row b for sequence b, stride inv_freq.stride(0)) on the activations' device;
+    style: the pairing (rope_style), NeoX when left out"""
+    inv, af = rope[:2]
+    style = rope_style(rope[2]) if len(rope) > 2 else ROPE_NEOX
     assert inv.dtype == torch.float32 and inv.device == device and inv.stride(-1) == 1, \
         "rope table: fp32 inverse frequencies on the activations' device"
     if inv.dim() == 1:
@@ -352,7 +363,7 @@ def _rope_table(rope, rows, device):
     else:
         assert inv.dim() == 2 and inv.shape[0] == rows, "rope table: [rotary_dim / 2] or one row per sequence"
         rd, stride = 2 * inv.shape[1], inv.stride(0)
-    return RopeCfg(0.0, int(rd), 0), RopeTable(inv.data_ptr(), int(stride), float(af), 0)
+    return RopeCfg(0.0, int(rd), style), RopeTable(inv.data_ptr(), int(stride), float(af), 0)
 
 
 def _cache_append(cache, qkv, old_lens, q_out=None, rope=None, q_len=None, parents=None, qk_norm=None):
@@ -362,7 +373,9 @@ def _cache_append(cache, qkv, old_lens, q_out=None, rope=None, q_len=None, paren
     old_lens[b] + depth(t).  qk_norm = (q_gamma, k_gamma, eps): the per-head Q/K RMSNorm before rotary
     (b2_span_cache_append_qknorm), every step form.  rope = (base, rotary_dim): the rotary with base^(-2f / rotary_dim);
     rope = (inv_freq tensor, attn_factor): the scaled rotary from a frequency table (rope_table; one row, or one row per
-    sequence) in every step form, with or without qk_norm (b2_span_cache_append_rope_table)."""
+    sequence) in every step form, with or without qk_norm (b2_span_cache_append_rope_table).  Either tuple may carry a
+    third element, the pairing style (rope_style: "neox" / "interleaved" or ROPE_NEOX / ROPE_INTERLEAVED); NeoX without
+    it."""
     cfg = cache.cfg
     rows = qkv.shape[0]
     assert rows % (q_len or 1) == 0 and (parents is None or (q_len and parents.dtype == torch.int32 and parents.is_contiguous()))
@@ -376,7 +389,7 @@ def _cache_append(cache, qkv, old_lens, q_out=None, rope=None, q_len=None, paren
                                                   C.byref(tab), C.byref(nrm) if nrm is not None else None, _stream()),
               "b2_span_cache_append_rope_table")
         return q_out
-    r = RopeCfg(float(rope[0]), int(rope[1]), 0) if rope is not None else None
+    r = RopeCfg(float(rope[0]), int(rope[1]), rope_style(rope[2]) if len(rope) > 2 else ROPE_NEOX) if rope is not None else None
     tail = (C.byref(r) if r is not None else None, _stream())
     if qk_norm is not None:
         nrm = _qk_norm(qk_norm, qkv.dtype, qkv.device)
@@ -552,18 +565,19 @@ def quant_fp8(x, gamma=None, eps=1e-6, out=None):
     return out
 
 
-def rotary(qkv, pos, n_heads, n_groups, base=1e6, rotary_dim=128, table=None):
-    """In-place NeoX rotary of the q and k heads of qkv [rows, (n_heads + 2 n_groups) * 128] at positions pos [rows].
-    table = (inv_freq, attn_factor) (rope_table; [rotary_dim / 2], or [rows, >= rotary_dim / 2] with row b for qkv row b):
-    the scaled form b2_rotary_table, bf16 or fp16, base and rotary_dim unused; otherwise b2_rotary, bf16 only."""
+def rotary(qkv, pos, n_heads, n_groups, base=1e6, rotary_dim=128, table=None, style=ROPE_NEOX):
+    """In-place rotary of the q and k heads of qkv [rows, (n_heads + 2 n_groups) * 128] at positions pos [rows], pairing
+    style (rope_style: NeoX rotate-half by default, or "interleaved").  table = (inv_freq, attn_factor) (rope_table;
+    [rotary_dim / 2], or [rows, >= rotary_dim / 2] with row b for qkv row b): the scaled form b2_rotary_table, bf16 or fp16,
+    base and rotary_dim unused; otherwise b2_rotary, bf16 only."""
     if table is not None:
-        r, tab = _rope_table(table, qkv.shape[0], qkv.device)
+        r, tab = _rope_table(tuple(table[:2]) + (style,), qkv.shape[0], qkv.device)
         check(lib.b2_rotary_table(_ptr(qkv), _ptr(pos), qkv.shape[0], n_heads, n_groups, 128, C.byref(r), C.byref(tab), _ft(qkv),
                                   _stream()), "b2_rotary_table")
         return qkv
     if qkv.dtype != torch.bfloat16:  # b2_rotary is bf16 only (fp16 models rotate in the fused cache append)
         raise TypeError(f"rotary: qkv must be bfloat16, got {qkv.dtype}")
-    r = RopeCfg(float(base), int(rotary_dim), 0)
+    r = RopeCfg(float(base), int(rotary_dim), rope_style(style))
     check(lib.b2_rotary(_ptr(qkv), _ptr(pos), qkv.shape[0], n_heads, n_groups, 128, C.byref(r), _stream()), "b2_rotary")
     return qkv
 

@@ -199,15 +199,30 @@ size_t b2_span_bytes(const b2_span_cfg* cfg);
  *   qkv      [batch, (n_heads + 2*n_groups) * head_size] FT (post-RoPE unless rope != NULL)
  *   q_out    [batch, n_heads * head_size] FT
  *   old_lens [batch] int32 device: tokens already cached (= write position)
- * rope: optional fused rotary (NeoX rotate-half over rotary_dim, position = old_lens[b]); pass NULL
+ * rope: optional fused rotary (over the first rotary_dim dims, position = old_lens[b], pairing as rope->style); pass NULL
  * when the graph has a separate Rotary op.  Quantised modes follow QuantParam<I8/U4>::Builder
  * (span-attention/src/cache_quant/impl_i8.cuh:106-140, impl_u4.cuh:146-182) with IEEE division; B2_KV_FP8 quantizes as
  * described at its enum. */
 typedef struct {
   float base;          /* e.g. 1e6 for Qwen2 */
   int32_t rotary_dim;  /* <= head_size, even */
-  int32_t reserved;
+  int32_t style;       /* B2_ROPE_NEOX or B2_ROPE_INTERLEAVED */
 } b2_rope_cfg;
+/* Pairing styles of the rotary (b2_rope_cfg.style).  Dims d >= rotary_dim are never touched.
+ *   B2_ROPE_NEOX (0): rotate-half (Qwen2, Llama).  With half = rotary_dim / 2, dim d < rotary_dim uses frequency index
+ *     f = d % half and partner d + half (d < half: the "first half" expression) or d - half ("second half").  Computed
+ *     frequencies: inv = exp2f(-log2f(base) * (2f / rotary_dim)), ang = fl32(pos * inv), sn, cs = sincosf(ang),
+ *     first half: y = FT(x[d] cs - x[partner] sn), second half: y = FT(x[d] cs + x[partner] sn), one FT rounding
+ *     (whether the products fuse into an fma is the compiler's choice, the same in both styles).
+ *   B2_ROPE_INTERLEAVED (1): GPT-J / ChatGLM "half_inner" pairs (x[2i], x[2i+1]) at frequency i.  Dim d < rotary_dim uses
+ *     f = d / 2 and partner d ^ 1; even d takes the "first half" expression, odd d the "second half" one.  Every other
+ *     instruction is that of the NeoX form of the same entry point (angle, sincosf, attn_factor, products, fma, rounding),
+ *     so with P the permutation that de-interleaves the first rotary_dim dims of a head (evens, then odds) and keeps the
+ *     rest: interleaved(x) = P^-1 neox(P x), bit for bit (q_out, span rows, and quantized {zero, scale} and codes after P^-1).
+ *     A lane of the append holds 4 consecutive dims, so the pair is in one lane: no shuffle.
+ * Every entry point that takes a b2_rope_cfg honours style; a style outside {0, 1} is B2_ERR_PARAM and B2_ROPE_INTERLEAVED
+ * on the head-64 append is B2_ERR_UNSUPPORTED, before any launch. */
+enum { B2_ROPE_NEOX = 0, B2_ROPE_INTERLEAVED = 1 };
 int b2_span_cache_append(const b2_span_cfg* cfg, void* const* k_spans, void* const* v_spans,
                          void* q_out, const void* qkv, const int32_t* old_lens, int batch,
                          const b2_rope_cfg* rope, void* stream);
@@ -318,6 +333,8 @@ int b2_span_cache_append_qknorm(const b2_span_cfg* cfg, void* const* k_spans, vo
  *   ang = fl32(pos * inv[f]);  sn, cs = sincosf(ang);  c = fl32(cs * attn_factor);  s = fl32(sn * attn_factor);
  *   d < half:  t = fl32(x[d + half] * s),  y = FT(fma(x[d], c, -t));
  *   d >= half: t = fl32(x[d - half] * s),  y = FT(fma(x[d], c, t)),   one FT rounding.
+ * B2_ROPE_INTERLEAVED: f = d / 2; even d: t = fl32(x[d + 1] * s), y = FT(fma(x[d], c, -t)); odd d: t = fl32(x[d - 1] * s),
+ * y = FT(fma(x[d], c, t)) (the pairing rule at b2_rope_cfg).
  * attn_factor is YaRN's mscale (Hugging Face scales the cos / sin caches, so both q and k); 1.0 leaves cs and sn unchanged. */
 typedef struct {
   const float* inv_freq; /* fp32 [rows][stride] (>= rotary_dim / 2 per row), device, 16-byte aligned, stride % 4 == 0 */
@@ -350,7 +367,7 @@ int b2_rmsnorm_ft(void* y, const void* x, const void* gamma, int rows, int cols,
 int b2_binary_ft(void* out, const void* a, const void* b, int64_t n, int op, int ft, void* stream);
 int b2_argmax_ft(int64_t* ids_out, float* vals_out /* or NULL */, const void* logits, int batch, int n, int64_t ld, int64_t id_offset,
                  int ft, void* stream);
-/* in-place NeoX rotary on the q and k heads of qkv [batch, (nH+2nG)*head]; position = pos[b] */
+/* in-place rotary (pairing rope->style) on the q and k heads of qkv [batch, (nH+2nG)*head]; position = pos[b] */
 int b2_rotary(void* qkv, const int32_t* pos, int batch, int n_heads, int n_groups, int head_size,
               const b2_rope_cfg* rope, void* stream);
 /* b2_rotary with the frequencies of a b2_rope_table (arithmetic and errors there; row b of qkv uses inv_freq + b * stride),
